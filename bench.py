@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- pod x throttle admission checks/sec of the batched throttle-admission pass.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config C2] [--l2 rotate|flush]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config C2] [--l2 rotate|flush] [--dump-outputs DIR]
   (N>1: python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...)
 
 A "step" is ONE pass of the hot path over one synthetic snapshot: reconcile every throttle against the
@@ -14,9 +14,11 @@ the other BASELINE shapes on this many GPUs (N=1: C2 with arrival-order rows, C3
 N>1: the shape BASELINE.json quotes for that N -- C3@2, C4@4, C5@8 -- STRONG-sharded by rows).
 
 Timing (`--l2 rotate`, the default): E engine contexts hold E copies of the snapshot (E x footprint >= 2 x the
-126 MB L2), the timed region launches K passes back to back cycling through them -- every pass reads inputs that
+50 MB L2 of an H100), the timed region launches K passes back to back cycling through them -- every pass reads inputs that
 left L2 E-1 passes ago -- between ONE pair of CUDA events on the launching stream; ms_per_step = region / K.
 `--l2 flush`: one context, a 512 MiB write + 512 MiB read between steps (outside the per-step event pairs).
+`--dump-outputs DIR`: after the timed steps, what the last timed pass computed is written to DIR as float64 .npy files
+(dump_outputs); the inputs are seeded, so two builds run with the same arguments can be compared output for output.
 
 One JSON line on rank 0 (keys per the driver contract + roofline + cpu_baseline).
 """
@@ -38,6 +40,8 @@ sys.path.insert(0, ROOT)
 
 METRIC = "pod_x_throttle_admission_checks_per_sec"
 UNIT = "checks/s"
+L2_BYTES = 50e6  # H100
+DUMP_BYTES = 64 << 20
 
 
 def parse_args():
@@ -55,11 +59,14 @@ def parse_args():
                     help="how every timed pass gets cold inputs: rotate through enough snapshot copies to exceed L2 twice over (back-to-back "
                          "launches, one event pair) or flush L2 between steps (512 MiB write + 512 MiB read, per-step event pairs)")
     ap.add_argument("--no-extras", action="store_true", help="headline workload only: skip the `configs` array")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed pass computed to DIR/<name>.npy (float64, at most 64 MB in all)")
     return ap.parse_args()
 
 
 def measured_peaks():
-    """HBM copy bandwidth measured on this pool's B200s by the driver; fallback per B200_PROFILING.md."""
+    """HBM bandwidth the roofline fractions are taken of: MEASURED_PEAKS.json when the bench machine provides one, else the
+    H100 SXM data-sheet figure (3.35 TB/s; a data-sheet peak, not a measured one)."""
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     try:
         d = json.load(open(p))
@@ -68,13 +75,13 @@ def measured_peaks():
                 return float(d[k]), "measured (MEASURED_PEAKS.json)"
     except Exception:
         pass
-    return 6650.0, "fallback (B200_PROFILING.md: 6.65 TB/s)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not measured"
 
 
 class ClockSampler:
     """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
-         "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
+         "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,name,power.limit")
 
     def __init__(self, device: int):
         self.device, self.proc, self.lines = device, None, []
@@ -94,19 +101,24 @@ class ClockSampler:
 
     def stop(self):
         if not self.proc:
-            return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvidia-smi unavailable"]}
+            return {"sm_mhz": None, "sm_max_mhz": None, "gpu": None, "power_limit_w": None, "reasons": ["nvidia-smi unavailable"]}
         time.sleep(0.15)
         self.proc.terminate()
         try:
             self.proc.wait(timeout=2)
         except Exception:
             self.proc.kill()
-        sm, mx, reasons = [], [], set()
+        sm, mx, reasons, gpu, plim = [], [], set(), None, None
         names = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
         for ln in self.lines:
             f = [x.strip() for x in ln.split(",")]
-            if len(f) < 9:
+            if len(f) < 11:
                 continue
+            gpu = f[9]
+            try:
+                plim = float(f[10])
+            except ValueError:
+                pass
             try:
                 sm.append(float(f[1])); mx.append(float(f[2]))
             except ValueError:
@@ -114,7 +126,7 @@ class ClockSampler:
             for name, val in zip(names, f[5:9]):
                 if val.lower().startswith("active"):
                     reasons.add(name)
-        return {"sm_mhz": statistics.median(sm) if sm else None, "sm_max_mhz": max(mx) if mx else None,
+        return {"sm_mhz": statistics.median(sm) if sm else None, "sm_max_mhz": max(mx) if mx else None, "gpu": gpu, "power_limit_w": plim,
                 "reasons": sorted(reasons), "samples": len(sm)}
 
 
@@ -150,20 +162,6 @@ def moved_bytes_estimate(snap, Wp):
     return (n + p) * row + (n + p) * words * 4 + p * (words * 8 + 1) + p * (8 * R + 12) + M * (16 * R + 48 + 8 * (2 * R + 1) * 2)
 
 
-def measured_traffic(config, rows_scale):
-    """dram__bytes_read.sum + dram__bytes_write.sum of one k_pass launch from THIS round's `ncu --set full` capture, if the
-    committed summary (profiles/r2_traffic.json, written by tools/ncu_traffic.py from the .ncu-rep) is for this workload."""
-    try:
-        d = json.load(open(os.path.join(ROOT, "profiles", "r2_traffic.json")))
-        e = d.get(f"{config}x{rows_scale}")
-        if e:
-            pipes = {k: e[k] for k in ("sm_throughput_pct", "issue_active_pct", "alu_pipe_pct", "lsu_pipe_pct", "dram_throughput_pct") if k in e and e[k] == e[k]}
-            return e["dram_bytes_read"] + e["dram_bytes_write"], e.get("source"), pipes
-    except Exception:
-        pass
-    return None, None, None
-
-
 def algorithmic_bytes(snap, Wp):
     """SURVEY.md section 8(d): bytes one pass must move, per kernel."""
     L, R, M = snap.L, snap.R, snap.m
@@ -186,7 +184,7 @@ def run_reference(args, rank, world):
     toolchain exists in this image (SURVEY.md 8c), so this times the ORACLE's reference-shaped port
     (oracle/ko_model.h: string maps, per-call selector construction, ResourceAmountOfPod recomputed per use)
     with every host thread (each worker pinned to its own CPU), on the same config.  Each step = one full pass over
-    the snapshot (~0.1 s at C2 on 128 threads), K steps after W warm-ups as asked; `value` is taken from the MEDIAN
+    the snapshot (~0.1 s at C2 on 16 threads), K steps after W warm-ups as asked; `value` is taken from the MEDIAN
     step (thread start-up and allocator noise make single passes scatter)."""
     if rank != 0:
         return
@@ -312,7 +310,7 @@ class Bench:
     def l2_flush(self):
         torch = self.torch
         if self.flush is None:
-            self.flush = torch.empty(512 << 20, dtype=torch.uint8, device="cuda")  # > 126 MB L2
+            self.flush = torch.empty(512 << 20, dtype=torch.uint8, device="cuda")  # > 50 MB L2
             self.drain = torch.empty(512 << 20, dtype=torch.uint8, device="cuda").view(torch.int64)
         self.flush.zero_()  # WRITE a buffer larger than L2: evicts the snapshot, every pass reads its inputs from HBM ...
         self.drain.sum()    # ... then READ another one, so that what sits in L2 is clean (no foreign write-backs inside the timed region)
@@ -362,9 +360,9 @@ class Bench:
 
 
 def rotation_count(footprint_bytes, world):
-    """Contexts whose snapshots together exceed twice the 126 MB L2 (an LRU-ish cache has then forgotten a snapshot by the
+    """Contexts whose snapshots together exceed twice the 50 MB L2 of an H100 (an LRU-ish cache has then forgotten a snapshot by the
     time its turn comes again); capped -- with several ranks every context also carries a communicator."""
-    need = int(np.ceil(2 * 126e6 / max(footprint_bytes, 1)))
+    need = int(np.ceil(2 * L2_BYTES / max(footprint_bytes, 1)))
     return max(1, min(need, 16 if world == 1 else 10))
 
 
@@ -395,6 +393,31 @@ def measure_config(bench, name, snap, steps, warmup, mode, peak, sharded=None, k
     for e in engines:
         e.close()
     return out, None, ab
+
+
+def dump_outputs(eng, out_dir):
+    """What a caller of the timed path reads back after its pass (Engine.download), as float64 .npy files: the per-throttle status
+    columns whole; the per-pod rows (match bitmaps, check codes, admit bits) whole when everything fits DUMP_BYTES, otherwise the
+    same fixed seeded sample of rows every run, whose row indices are written beside them (running_rows / pending_rows)."""
+    res = eng.download()
+    per_thr = {f: getattr(res, f) for f in ("used", "used_present", "used_cnt", "throttled", "calc_thr", "calc_present", "calc_cnt", "override_active")}
+    per_pod = {"run_bitmap": (res.run_bitmap, "running"), "pend_bitmap": (res.pend_bitmap, "pending"), "codes": (res.codes, "pending"),
+               "admit": (res.admit, "pending")}
+    n_rows = {"running": res.run_bitmap.shape[0], "pending": res.admit.shape[0]}
+    budget = DUMP_BYTES - sum(8 * a.size for a in per_thr.values())
+    frac = min(1.0, budget / (sum(8 * a.size for a, _ in per_pod.values()) + 8 * sum(n_rows.values())))
+    rows = {}
+    for kind, n in n_rows.items():
+        k = int(n * frac)
+        rows[kind] = np.arange(n) if k >= n else np.sort(np.random.default_rng(0).choice(n, k, replace=False))
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in per_thr.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a.astype(np.float64))
+    for name, (a, kind) in per_pod.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a[rows[kind]].astype(np.float64))
+    for kind, r in rows.items():
+        if r.shape[0] < n_rows[kind]:
+            np.save(os.path.join(out_dir, kind + "_rows.npy"), r.astype(np.float64))
 
 
 def measure_e2e(bench, eng, snap, Wp, args, checks_per_step):
@@ -677,6 +700,8 @@ def main():
     t_wall = time.perf_counter() - t_wall0
     clocks = sampler.stop() if rank == 0 else None
     bench.restore_stdout()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(engines[(args.steps - 1) % len(engines)], args.dump_outputs)  # the context the last timed pass ran on
     eng = engines[0]
     Wp = eng.words_per_row
     launches_per_step = head["launches_per_step"]
@@ -705,14 +730,11 @@ def main():
     # The timed region launches ONE kernel per step (k_pass: match + reconcile + finalize + decide tiles), so that is the
     # dominant kernel and its average launch duration is region / K.  The three-kernel breakdown (kt_enable_timing switches
     # the library to its PDL-chained launch path) is reported beside it: `reconcile` is where the bytes are.
-    # traffic: dram__bytes_read.sum + dram__bytes_write.sum of one k_pass launch needs ncu, which bench.py does not run: they are
-    # read from the committed capture of this workload (profiles/r2_traffic.json <- tools/ncu_traffic.py <- the .ncu-rep), with
-    # the pipe utilisations of the same capture (SURVEY 8(d): ALU pipe next to HBM %); null when there is no capture.
+    # traffic: dram__bytes_read.sum + dram__bytes_write.sum of one k_pass launch needs ncu, which bench.py does not run
     roofline = dict(head["roofline"])
-    traffic, traffic_src, pipes = measured_traffic(args.config, args.rows_scale)
     moved = moved_bytes_estimate(snap, Wp)
-    roofline.update({"traffic": traffic, "traffic_source": traffic_src or "none committed for this workload (ncu is not run inside bench.py)",
-                     "pipes_under_ncu": pipes, "moved_bytes_estimate": moved, "frac_moved": moved / (pass_ms * 1e-3) / 1e9 / peak,
+    roofline.update({"traffic": None, "traffic_source": "not measured (ncu is not run inside bench.py)",
+                     "pipes_under_ncu": None, "moved_bytes_estimate": moved, "frac_moved": moved / (pass_ms * 1e-3) / 1e9 / peak,
                      "note": "achieved / frac use SURVEY.md 8(d)'s algorithmic bytes (dense bitmap written once per pass); the pass maintains its "
                              "bitmaps word by word and stores int32 row offsets, so it moves fewer bytes than that -- frac_moved is the same time "
                              "against the bytes it has to move (latency-bound at this size either way)",

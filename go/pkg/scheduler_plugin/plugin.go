@@ -1,7 +1,7 @@
 // NOT COMPILED IN THIS REPOSITORY'S ENVIRONMENT (no Go toolchain in the image; see go/README.md).
 //
-// The kube-scheduler plugin of kube-throttler with its admission hot path on a B200.  Exported surface, plugin name,
-// framework statuses, reason strings and events are the reference's (/root/reference/pkg/scheduler_plugin/plugin.go:45-279);
+// The kube-scheduler plugin of kube-throttler with its admission hot path on an H100.  Exported surface, plugin name,
+// framework statuses, reason strings and events are the reference's (everpeace/kube-throttler pkg/scheduler_plugin/plugin.go:45-279);
 // what differs is behind it: instead of two Go controllers that walk listers per pod and per throttle
 // (pkg/controllers), informer events are forwarded to the engine behind include/kt_host.h, which keeps the pod /
 // throttle / namespace snapshot packed in HBM and answers PreFilter, Reserve and the reconcile of EVERY throttle with

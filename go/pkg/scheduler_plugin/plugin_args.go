@@ -1,9 +1,9 @@
 // NOT COMPILED IN THIS REPOSITORY'S ENVIRONMENT (no Go toolchain in the image; see go/README.md).
 //
 // Plugin arguments of the kube-throttler scheduler plugin, decoded exactly as the reference does
-// (/root/reference/pkg/scheduler_plugin/plugin_args.go:33-60): the same struct, the same JSON tags -- misspellings
+// (everpeace/kube-throttler pkg/scheduler_plugin/plugin_args.go:33-60): the same struct, the same JSON tags -- misspellings
 // included, they are the wire format of existing pluginConfig objects -- the same defaults and error texts.
-// The B200 build adds nothing to the wire format: the GPU ordinal comes from the environment (KT_B200_DEVICE).
+// The GPU build adds nothing to the wire format: the GPU ordinal comes from the environment (KT_B200_DEVICE).
 
 package scheduler_plugin
 

@@ -1,5 +1,5 @@
 /*
- * kt_b200.h -- C ABI of the B200-native throttle-admission engine.
+ * kt_b200.h -- C ABI of the H100-native throttle-admission engine.
  *
  * This is the drop-in boundary for the ONE hot path of everpeace/kube-throttler:
  * the per-pod PreFilter/Reserve check (pkg/scheduler_plugin/plugin.go:148-238) plus
@@ -14,7 +14,7 @@
  * library owns all device memory.  Re-entrant from arbitrary OS threads (cgo calls hop
  * threads): every call takes the context mutex and does cudaSetDevice itself.
  *
- * There is deliberately NO CPU fallback: on a machine without a usable sm_100 GPU
+ * There is deliberately NO CPU fallback: on a machine without a usable sm_90 GPU
  * kt_create() fails with KT_ERR_CUDA.
  *
  * Data model (all integers; exact decimal arithmetic is the packer's job, see

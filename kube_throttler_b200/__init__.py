@@ -1,4 +1,4 @@
-"""kube_throttler_b200 -- B200-native throttle-admission hot path of everpeace/kube-throttler.
+"""kube_throttler_b200 -- H100-native throttle-admission hot path of everpeace/kube-throttler.
 
 The product is the C-ABI shared library `libkt_b200.so` (include/kt_b200.h; CUDA kernels in csrc/).
 This Python module is a thin ctypes binding used by the tests and bench.py -- the same calls a Go
@@ -29,7 +29,7 @@ class KtError(RuntimeError):
 
 
 def build(force: bool = False) -> str:
-    """Compile csrc/ for sm_100a in-tree (nvcc cross-compiles without a GPU)."""
+    """Compile csrc/ for sm_90a in-tree (nvcc cross-compiles without a GPU)."""
     srcs = [os.path.join(_HERE, "csrc", f) for f in ("kt_engine.cu", "kt_tables.cc", "kt_host.cc", "kt_kernels.cuh", "kt_tables.h", "kt_json.h", "kt_quantity.h")]
     srcs.append(os.path.join(_HERE, "..", "include", "kt_b200.h"))
     srcs.append(os.path.join(_HERE, "..", "include", "kt_host.h"))

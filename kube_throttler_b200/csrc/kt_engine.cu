@@ -530,7 +530,7 @@ cudaError_t dispatch_check(kt_ctx* c, const PodView& pv, const TableView& tb, co
 
 extern "C" {
 
-const char* kt_version(void) { return "kt_b200 0.1 (sm_100a, abi 1)"; }
+const char* kt_version(void) { return "kt_b200 0.1 (sm_90a, abi 1)"; }
 
 const char* kt_last_error(const kt_ctx* ctx) { return ctx ? ctx->err.c_str() : "null context"; }
 

@@ -1,4 +1,4 @@
-// kt_kernels.cuh -- sm_100a kernels of the throttle-admission pass (hand-written CUDA, no libraries).
+// kt_kernels.cuh -- sm_90a kernels of the throttle-admission pass (hand-written CUDA, no libraries).
 //
 //   k_reconcile   running pods  -> affectedPods bitmap + per-throttle partial sums
 //                 (replaces throttle_controller.go:221-246 affectedPods + :116-119 used-sum,
@@ -57,7 +57,7 @@ constexpr uint32_t kFull = 0xffffffffu;
 #endif
 constexpr int kStageChunk = KT_STAGE_CHUNK;  // resources whose pre-record values and sums a decide lane requests together
 #ifndef KT_EVAL_PAIR  // 1: a lane's first two words are evaluated with their table gathers interleaved (eval_word2).  Measured
-#define KT_EVAL_PAIR 0  // slower at the 80-register cap of a resident pass (spills): C2 21.6 vs 20.9 us, C2 x10 100 vs 92 us -- off
+#define KT_EVAL_PAIR 0  // measured slower at the 80-register cap of a resident pass (spills) -- off
 #endif
 #ifndef KT_DECIDE_UNROLLED
 #define KT_DECIDE_UNROLLED 0
@@ -129,7 +129,7 @@ struct WordCursor {
 };
 
 #ifndef KT_SCATTER_WORDS  // a warp whose lanes start in more distinct words than this takes the per-lane paths
-#define KT_SCATTER_WORDS 32  // 32 = never: measured slower than the rounds at C2 in arrival order (profiles/README.md r2); the product keeps rows clustered (kt_host.cc row arenas)
+#define KT_SCATTER_WORDS 32  // 32 = never: measured slower than the rounds at C2 in arrival order; the product keeps rows clustered (kt_host.cc row arenas)
 #endif
 // Do the lanes of this warp live in many different namespaces (rows in arrival order)?  Judged by their first words.
 __device__ __forceinline__ bool warp_is_scattered(const WordCursor& wc) {
@@ -663,7 +663,7 @@ __device__ __forceinline__ unsigned long long warp_sum_u64(unsigned long long v)
 // One elected lane arms the barrier with the byte count and issues the copies; the data lands in shared memory without passing
 // through anybody's registers and the consumers sleep on the barrier's phase instead of a scoreboard.  SASS: UBLKCP / SYNCS.
 #ifndef KT_BULK_ROWS  // 1: a reconcile tile's column slices (row offsets, requests, flags ...) are staged with bulk copies; 0: per-lane LDG.
-#define KT_BULK_ROWS 0  // Measured slower (profiles/README.md r2b: C2 +0.5 us, C2 x10 +4 us, C4 +0.7 us -- sixteen 0.5-1 KB copies per tile) -- off
+#define KT_BULK_ROWS 0  // measured slower at C2, C2 x10 and C4 (sixteen 0.5-1 KB copies per tile) -- off
 #endif
 #ifndef KT_SMEM_ADD32  // 1: 64-bit shared-memory accumulator adds as two native 32-bit atomics with a carry; 0: atomicAdd(u64) (a CAS loop)
 #define KT_SMEM_ADD32 1
@@ -1775,7 +1775,7 @@ __device__ __forceinline__ void check_decide_tile(const PodView& pods, const Tab
 // ------------------------------------------------------------------------------------------------
 // The SHARED decide tiles of a resident pass.  When every match and reconcile CTA of the grid is on the device at once, the
 // decide work is not left to the P/TILE CTAs that matched the pending pods (one lane per pod walking its words and pairs one
-// after the other while every other SM has gone idle: 7 of the C2 pass's 19 us): every CTA that has finished its own tile --
+// after the other while every other SM has gone idle): every CTA that has finished its own tile --
 // match or reconcile -- draws sub-tiles of TILE/4 pending pods from a second ticket counter.  FOUR lanes per pod: lane q
 // fetches the pod's q-th word of the round and claims its staging slot (same-word lanes of a warp elect one claimant; a word
 // that finds no slot -- rows in arrival order -- is checked pair by pair straight from L2), and the pod's pairs are dealt out
@@ -1790,7 +1790,7 @@ __device__ __forceinline__ void check_decide_tile(const PodView& pods, const Tab
 #ifndef KT_QUAD_FENCE  // 1: a shared decide tile looks at its three counters with relaxed loads and acquires once, with a fence; 0: three acquire loads
 #define KT_QUAD_FENCE 1
 #endif
-#ifndef KT_QUAD_DRYRUN  // measured (profiles/README.md r2b): the walk itself costs what it saves -- off
+#ifndef KT_QUAD_DRYRUN  // measured: the walk itself costs what it saves -- off
 #define KT_QUAD_DRYRUN 0
 #endif
 template <int TILE, int RT>
@@ -2066,7 +2066,7 @@ __device__ __forceinline__ unsigned long long globaltimer_ns() {
 }
 
 // TILE: pods per CTA (= threads).  128 everywhere except ClusterThrottle-heavy tables, where every pod walks a dozen words and a
-// CTA's accumulator slots (one per word, 2 KB each at R = 8) are better shared by twice the pods (C3: 156 -> 119 us).
+// CTA's accumulator slots (one per word, 2 KB each at R = 8) are better shared by twice the pods (measured faster at C3).
 template <int TPC, int B, int RT, bool REG, int TILE = kTileReconcile>
 __global__ void __launch_bounds__(TILE, KT_PASS_THREADS / TILE) k_pass(const __grid_constant__ PassArgs a) {
   extern __shared__ __align__(16) unsigned char smem_raw[];

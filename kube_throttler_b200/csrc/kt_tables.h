@@ -1,5 +1,5 @@
 // kt_tables.h -- selector compiler: turns the CSR selector table of include/kt_b200.h into the
-// bit-sliced match tables the sm_100a kernels scan (DESIGN.md "Bit-sliced selector match").
+// bit-sliced match tables the sm_90a kernels scan (DESIGN.md "Bit-sliced selector match").
 //
 // This is packer-side work that runs when Throttles/ClusterThrottles/Namespaces change, not per pass.
 // It replaces what the reference redoes on EVERY MatchesToPod call:

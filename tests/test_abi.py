@@ -1,4 +1,4 @@
-"""The C-ABI library builds for sm_100a, loads on a CPU-only box and exports every symbol that
+"""The C-ABI library builds for sm_90a, loads on a CPU-only box and exports every symbol that
 include/kt_b200.h declares.  No compute calls: there is no GPU here and no CPU fallback to call."""
 import ctypes as C
 import os
@@ -47,8 +47,8 @@ def test_struct_layouts(kt):
     assert C.sizeof(abi.Timing) == 24
 
 
-def test_library_is_sm100a_cuda(kt):
-    """The shipped .so carries sm_100a SASS for the three hot kernels (no PTX-JIT, no other arch)."""
+def test_library_is_sm90a_cuda(kt):
+    """The shipped .so carries sm_90a SASS for the three hot kernels (no PTX-JIT, no other arch)."""
     import shutil
     import subprocess
 
@@ -56,7 +56,7 @@ def test_library_is_sm100a_cuda(kt):
     if not os.path.exists(cuobjdump):
         pytest.skip("cuobjdump not available")
     out = subprocess.run([cuobjdump, "-lelf", kt.LIB_PATH], capture_output=True, text=True).stdout
-    assert "sm_100a" in out
+    assert "sm_90a" in out
     sass = subprocess.run([cuobjdump, "-sass", kt.LIB_PATH], capture_output=True, text=True).stdout
     for k in ("k_reconcile", "k_finalize", "k_check"):
         assert k in sass

@@ -44,7 +44,7 @@ def test_two_gpu_parity():
     import torch
 
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs >= 2 GPUs (run under gpurun --gpus 2)")
+        pytest.skip("needs >= 2 GPUs")
     r = _torchrun(2, os.path.join("tools", "multi_gpu_parity.py"), "C3")
     assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-3000:]
     assert "OK" in r.stdout
@@ -55,7 +55,7 @@ def test_missing_rank_times_out_instead_of_hanging():
     import torch
 
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs >= 2 GPUs (run under gpurun --gpus 2)")
+        pytest.skip("needs >= 2 GPUs")
     r = _torchrun(2, os.path.join("tools", "multi_gpu_timeout.py"), timeout=300)
     assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-3000:]
     assert "multi-gpu timeout: OK" in r.stdout

@@ -2,7 +2,7 @@
 BOTH implementations of the plugin surface through the same test bodies:
   [oracle]  the object-level ORACLE (plugin PreFilter/Reserve + both controllers), CPU only;
   [b200]    the PRODUCT: include/kt_host.h above the CUDA engine (marked gpu: every match, sum and compare
-            of these scenarios runs in the sm_100a kernels, the host only packs and spells).
+            of these scenarios runs in the sm_90a kernels, the host only packs and spells).
 
 The integration suite needs Go + kind + a real kube-scheduler, none of which exist here; its scenarios
 are deterministic decision sequences, so they are transcribed as golden vectors:

@@ -1,6 +1,6 @@
 // What a CUDA-event pair around ONE launch costs on this box, as a function of grid size, dynamic shared memory and the state
 // of L2 (flushed by a 512 MiB memset + read beforehand, as bench.py does, or left alone); and what back-to-back launches cost.
-// nvcc -arch=sm_100a -O3 -o launch_floor launch_floor.cu && ./launch_floor
+// nvcc -arch=sm_90a -O3 -o launch_floor launch_floor.cu && ./launch_floor
 #include <cstdio>
 #include <cuda_runtime.h>
 #include <algorithm>
@@ -28,7 +28,7 @@ int main() {
   cudaFuncSetAttribute(k_touch, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 << 10);
   for (int flushed = 0; flushed < 2; ++flushed)
     for (int smem : {0, 24 << 10, 34 << 10})
-      for (int grid : {148, 444, 888, 1003, 2000}) {
+      for (int grid : {132, 396, 792, 1003, 2000}) {
         for (int kind = 0; kind < 2; ++kind) {
           std::vector<float> t;
           for (int it = 0; it < 30; ++it) {
@@ -46,7 +46,7 @@ int main() {
         }
       }
   // back to back: K launches between one event pair
-  for (int grid : {148, 1003}) {
+  for (int grid : {132, 1003}) {
     cudaEventRecord(a, s);
     for (int i = 0; i < 200; ++i) k_touch<<<grid, 128, 24 << 10, s>>>(src, dst, 1 << 20);
     cudaEventRecord(b, s);

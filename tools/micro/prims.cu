@@ -1,7 +1,7 @@
 // Latency (SM cycles, %clock64) of the building blocks of the pass's hand-offs, one warp of one CTA on an otherwise idle GPU
 // and again with every other SM streaming from HBM: relaxed / acquire loads from L2, fences, returning atomics, nanosleep,
 // a CTA barrier, a 3 KB bulk copy (cp.async.bulk + mbarrier) against the same bytes fetched with LDG.128, LDS chains.
-// nvcc -arch=sm_100a -O3 -o prims prims.cu && ./prims
+// nvcc -arch=sm_90a -O3 -o prims prims.cu && ./prims
 #include <cstdio>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -73,7 +73,7 @@ int main() {
                              "__syncthreads (128 thr)", "bulk copy 3 KB + mbarrier wait", "3 KB by one warp, LDG.128 + STS", "8 dependent LDS", "2 independent L2 trips",
                              "2 dependent L2 trips", "RED.ADD", "__threadfence + RED (signal)"};
   for (int busy = 0; busy < 2; ++busy) {
-    k_prims<<<busy ? 148 * 4 : 1, busy ? 256 : 128>>>(g, blob, out, busy);
+    k_prims<<<busy ? 132 * 4 : 1, busy ? 256 : 128>>>(g, blob, out, busy);
     cudaError_t e = cudaDeviceSynchronize();
     if (e != cudaSuccess) { printf("error %s\n", cudaGetErrorString(e)); return 1; }
     long long h[NOPS]; cudaMemcpy(h, out, sizeof h, cudaMemcpyDeviceToHost);

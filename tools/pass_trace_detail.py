@@ -27,14 +27,14 @@ matches = np.array([int(np.unpackbits(bm[i * 128:(i + 1) * 128].view(np.uint8)).
 nns = np.array([len(set(ns[i * 128:(i + 1) * 128])) for i in range(nr)])
 words = np.array([int((bm[i * 128:(i + 1) * 128] != 0).any(axis=0).sum()) for i in range(nr)])
 sm = rec[:, 1].astype(int)
-per_sm = np.bincount(sm, minlength=148)
+per_sm = np.bincount(sm, minlength=132)
 print("corr(dur, matches) %.2f  corr(dur, words) %.2f  corr(dur, ctas_on_sm) %.2f  corr(end, start) %.2f" % (
     np.corrcoef(dur, matches)[0, 1], np.corrcoef(dur, words)[0, 1], np.corrcoef(dur, per_sm[sm])[0, 1], np.corrcoef(end, (rec[:, 2] - t0) / 1e3)[0, 1]))
 order = np.argsort(-end)[:12]
 for i in order:
     print(f"tile {i:4d} sm {sm[i]:3d} (ctas on sm {per_sm[sm[i]]}) start {(rec[i,2]-t0)/1e3:5.1f} end {end[i]:5.1f} dur {dur[i]:5.1f} matches {matches[i]:5d} words {words[i]} ns {nns[i]}")
 print("dur percentiles", np.percentile(dur, [5, 25, 50, 75, 95, 100]).round(1), "end percentiles", np.percentile(end, [5, 25, 50, 75, 95, 100]).round(1))
-allsm = np.bincount(rows[:, 1].astype(int), minlength=148)
+allsm = np.bincount(rows[:, 1].astype(int), minlength=132)
 print("CTAs per SM (all roles): min %d max %d" % (allsm.min(), allsm.max()))
 for lo, hi in ((0, 200), (200, 500), (500, 900), (900, 2000), (2000, 100000)):
     m = (matches >= lo) & (matches < hi)
