@@ -284,7 +284,11 @@ int kt_set_reserved(kt_ctx* ctx, const int64_t* reserved /*[R][m]*/,
 /* ---- the pass ------------------------------------------------------------------- */
 /* One batched pass: reconcile every throttle (throttle_controller.go:84-133) and check
  * every pending pod against every throttle (CheckThrottled, :349-397).  Asynchronous on
- * the context stream unless a getter is called; kt_sync() waits. */
+ * the context stream unless a getter is called; kt_sync() waits.
+ * Value domain: quantities are signed.  Every request, threshold, used and reserved value,
+ * and for every resource column the sum of |v| over the running and pending requests, the
+ * reservations and the status, must stay below 2^62 (the host layer, kt_host.cc, checks
+ * the pod columns' sums before it uploads).  Sums are then exact in int64. */
 int kt_evaluate(kt_ctx* ctx, int64_t now_unix_ns, uint32_t flags);
 
 /* ---- queue-ordered greedy admission ------------------------------------------------ */
@@ -296,8 +300,8 @@ int kt_evaluate(kt_ctx* ctx, int64_t now_unix_ns, uint32_t flags);
  * (kt_upload_status) + the uploaded reservations (kt_set_reserved), isThrottledOnEqual from `flags` (KT_EVAL_ON_EQUAL or 0).
  * Afterwards admit[row] says which rows were admitted and codes[row] holds the 2-bit codes each REJECTED row saw at its turn
  * (kt_get_check / kt_get_check_rows); the pending match rows (kt_get_match_rows) name the throttles an admitted pod must be
- * reserved on by the caller's reservation cache.  Requests must be non-negative (the fixpoint relies on the checks being
- * monotone in the reserved amounts). */
+ * reserved on by the caller's reservation cache; the rows outside the queue keep the codes and admit bits of a
+ * KT_EVAL_GIVEN_STATUS | KT_EVAL_SKIP_RECONCILE pass.  Requests may be negative; the value domain is kt_evaluate's. */
 int kt_admit_queue(kt_ctx* ctx, int64_t first, int64_t count, uint32_t flags, int32_t* rounds, int64_t* admitted);
 
 /* ---- one end-to-end step in one call --------------------------------------------- */

@@ -10,12 +10,14 @@
 //   * the load pod i sees on throttle t is the sum of the requests of the ADMITTED pods before i in t's list -- an exclusive
 //     prefix sum along the list;
 //   * which pods are admitted is the unknown.  Every pod is Undecided, Admitted or surely-reJected.  One round computes, for
-//     every (pod, throttle) pair, the check under the smallest load it can still see (earlier Admitted pods only) and the
-//     largest (earlier Admitted + Undecided).  CheckThrottledFor is monotone in the load (requests are non-negative: S3 / S4
-//     only ever turn true as used + reserved grows; S1 / S2 do not look at it), so a pod that passes all its pairs under the
-//     LARGEST load is admitted whatever the pods before it do, and a pod that fails a pair under the SMALLEST load is
-//     rejected whatever they do.  Rounds repeat until nobody is Undecided; the first undecided pod of the queue sees equal
-//     bounds, so every round decides somebody, and pods on disjoint throttles are decided together.  A last round, with
+//     every (pod, throttle) pair, the check under the smallest load it can still see and the largest: every earlier Admitted
+//     pod adds its request to both, every earlier Undecided pod adds min(v, 0) to the smallest and max(v, 0) to the largest
+//     (requests may be negative), its presence bits and its pod count to the largest only.  CheckThrottledFor is monotone
+//     in each resource's load and presence separately (S3 / S4 only ever turn true as used + reserved grows; S1 / S2 do not
+//     look at it), so a pod that passes all its pairs under the LARGEST load is admitted whatever the pods before it do, and
+//     a pod that fails a pair under the SMALLEST load is rejected whatever they do.  Rounds repeat until nobody is
+//     Undecided; the first undecided pod of the queue sees equal bounds, so every round decides somebody, and pods on
+//     disjoint throttles are decided together.  A last round, with
 //     every load exact, writes the 2-bit codes each rejected pod saw at its turn.
 //
 // Typical queues settle in 2-4 rounds (a throttle with room for 300 of 1000 queued pods: round 1 admits the 300, round 2
@@ -140,8 +142,8 @@ __device__ __forceinline__ uint32_t warp_excl_or(uint32_t v, int lane, uint32_t*
 }
 
 // One round, one warp per throttle: walk the toucher list 32 positions at a time; exclusive prefix sums of the requests of the
-// Admitted (smallest load) and of the Admitted + Undecided (largest load) pods give every pair its two loads; the pair is
-// checked under both (the 4 steps of CheckThrottledFor, throttle_types.go:128-153 / clusterthrottle_types.go:30-55, GIVEN_STATUS
+// Admitted pods plus the negative (smallest load) or positive (largest load) requests of the Undecided ones give every pair
+// its two loads; the pair is checked under both (the 4 steps of CheckThrottledFor, throttle_types.go:128-153 / clusterthrottle_types.go:30-55, GIVEN_STATUS
 // constants from the pre-record).  RMAX bounds R at compile time for the register arrays.
 template <int RMAX>
 __global__ void __launch_bounds__(128) k_admit_round(AdmitView a) {
@@ -182,11 +184,11 @@ __global__ void __launch_bounds__(128) k_admit_round(AdmitView a) {
       v[r] = (r < R && on && ((present >> r) & 1)) ? a.req[(int64_t)r * a.n + p] : 0;
       if (v[r] != 0) nz |= 1u << r;
     }
-    const bool in0 = st == kAdmitted, in1 = st != kRejected;
+    const bool in0 = st == kAdmitted, in1 = st != kRejected, und = st == kUndecided;
     uint32_t code[2];
 #pragma unroll
     for (int z = 0; z < 2; ++z) {
-      const bool in = z ? in1 : in0;
+      const bool in = z ? in1 : in0;  // the pod's count and presence
       // what the pods before this position have reserved on the throttle (Reserve adds ResourceAmountOfPod: every request key
       // of the pod, zero or not, and Counts{Pod: 1})
       long long tot;
@@ -208,7 +210,9 @@ __global__ void __launch_bounds__(128) k_admit_round(AdmitView a) {
       for (int r = 0; r < RMAX; ++r) {
         if (r < R) {  // uniform
           long long rtot;
-          const long long e = run[z][r] + warp_excl_scan(in ? v[r] : 0, lane, &rtot);
+          // the pod's request: all of it if Admitted; if Undecided, only the part that moves this bound
+          const long long vz = und ? (z ? (v[r] > 0 ? v[r] : 0) : (v[r] < 0 ? v[r] : 0)) : (in0 ? v[r] : 0);
+          const long long e = run[z][r] + warp_excl_scan(vz, lane, &rtot);
           run[z][r] += rtot;
           if ((nz >> r) & 1) {  // IsThrottledFor only looks at the pod's non-zero requests (Q5)
             const bool has = (ph.thr_has >> r) & 1;

@@ -1203,7 +1203,7 @@ int kt_admit_queue(kt_ctx* c, int64_t first, int64_t count, uint32_t flags, int3
     KT_CUDA(c, cudaStreamSynchronize(c->stream));
     ++rounds;
     if (undecided_before == 0) break;
-    if (rounds > count + 2) return fail(c, KT_ERR_STATE, "kt_admit_queue did not converge (negative requests in the queue?)");
+    if (rounds > count + 2) return fail(c, KT_ERR_STATE, "kt_admit_queue did not converge");
   }
   if (rounds_out) *rounds_out = rounds;
   if (admitted_out) *admitted_out = counters[1];

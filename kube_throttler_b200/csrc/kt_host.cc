@@ -1938,8 +1938,6 @@ struct kth_plugin {
     for (auto& p : queue) {
       const int id = ns_dict.find(p.ns);
       if (id < 0 || !namespaces[(size_t)id].exists) return false;  // "namespace not found": Error as well
-      for (auto& kv : p.request)
-        if (kv.second.mant < 0) return false;  // the prefix-sum fixpoint needs the checks to be monotone in the reserved amounts
     }
     return true;
   }
@@ -2000,7 +1998,7 @@ struct kth_plugin {
     const size_t n = queue.size();
     if (admit_queue_on_device_possible(queue)) return admit_queue_on_device(queue);
     // (below: the same semantics with host-orchestrated passes -- kept for queues the device fixpoint does not take: a pod that
-    // PreFilter answers with Error must not be reserved, and the fixpoint relies on non-negative requests)
+    // PreFilter answers with Error must not be reserved)
     std::vector<std::string> results(n);
     std::vector<int> round_of(n, 0);
     std::vector<size_t> undecided(n);

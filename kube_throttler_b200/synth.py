@@ -283,10 +283,66 @@ def true_used_numpy(snap: abi.Snapshot):
     return used, present, cnt
 
 
+VALUE_REGIMES = ("wide", "carry", "signed")
+HIGH_LIMB = 1 << 44  # warp_sum_u64 adds bits 44-63 as its third limb
+
+
+def _rewrite_values(pods: abi.PodCols, rng, regime: str, bound: int) -> None:
+    """Replace every present request by a value of the regime (absent ones stay 0)."""
+    R, n = pods.req.shape
+    has = ((pods.present[None, :] >> np.arange(R, dtype=np.uint32)[:, None]) & 1).astype(bool)
+    if regime == "wide":      # [2^44, bound) with random low bits: the high limb of every warp sum is busy
+        v = rng.integers(HIGH_LIMB, bound, size=(R, n), dtype=np.int64)
+    elif regime == "carry":   # low 32 bits all ones (so the low 22 too): every limb and every 32-bit half carries
+        v = (rng.integers(0, min(1 << 14, bound >> 32), size=(R, n), dtype=np.int64) << 32) | 0xFFFFFFFF
+    elif regime == "signed":  # both signs, a tenth present with value zero
+        v = rng.integers(-(1 << 40), 1 << 40, size=(R, n), dtype=np.int64)
+        v = np.where(rng.random((R, n)) < 0.1, 0, v)
+    else:
+        raise ValueError(f"values={regime!r}: expected one of {VALUE_REGIMES}")
+    pods.req = np.ascontiguousarray(np.where(has, v, 0).astype(np.int64))
+
+
+def _equality_thresholds(snap: abi.Snapshot, rng, frac: float = 0.12) -> None:
+    """Thresholds exactly at the edges of the check, from the exact matched sums (Python ints): on about half of the chosen
+    throttles S3's alreadyUsed == threshold (a resource column and the count), on the others S4's alreadyUsed + the request of one
+    matched pending pod == threshold (a column the pod requests non-zero, and the count).  A `>` / `>=` mix-up then changes
+    codes under both isThrottledOnEqual settings.  Throttles with overrides are left alone (their spec threshold is not the
+    calculated one)."""
+    used, _, ucnt = true_used_numpy(snap)
+    m, R = snap.m, snap.R
+    pend = snap.pending
+    live = ((snap.thr_flags & abi.THR_RESPONSIBLE) != 0) & ((snap.thr_flags & abi.THR_SELECTOR_ERROR) == 0)
+    pick = np.nonzero((rng.random(m) < frac) & live & (np.diff(snap.ovr_off) == 0))[0]
+    thr, thr_present, thr_cnt = snap.thr.copy(), snap.thr_present.copy(), snap.thr_cnt.copy()
+    s4 = False
+    for t in pick.tolist():
+        already = [int(used[r, t]) + int(snap.reserved[r, t]) for r in range(R)]  # Python ints: exact
+        cnt = int(ucnt[t]) + int(snap.reserved_cnt[t])
+        rows = _candidate_rows(snap, pend, t, None)
+        rows = rows[match_matrix_numpy(snap, pend, t, rows)] if rows.size else rows
+        s4 = not s4 and rows.size > 0  # alternate, among the throttles some pending pod affects
+        if not s4:      # S3
+            r = int(rng.integers(R))
+            thr[r, t], thr_cnt[t] = already[r], cnt
+        else:           # S4: one pending pod the throttle affects
+            i = int(rows[rng.integers(rows.size)])
+            cols = [r for r in range(R) if (int(pend.present[i]) >> r) & 1 and int(pend.req[r, i]) != 0]
+            r = cols[int(rng.integers(len(cols)))] if cols else int(rng.integers(R))
+            thr[r, t], thr_cnt[t] = already[r] + int(pend.req[r, i]), cnt + 1
+        thr_present[t] |= np.uint32((1 << r) | abi.COUNT_BIT)
+    snap.thr, snap.thr_present, snap.thr_cnt = thr, thr_present, thr_cnt
+
+
 def generate(config: str = "C2", *, seed=None, m=None, n=None, p=None, R=None, n_ns=None, cluster_frac=None,
              override_frac=None, L: int = 8, sort_by_namespace: bool = True, now: int = NOW_2026,
-             calibrate: bool = True, q_max: int = 0, column_layout: bool = False) -> abi.Snapshot:
-    """Build the snapshot of a BASELINE config (or a scaled variant via keyword overrides)."""
+             calibrate: bool = True, q_max: int = 0, column_layout: bool = False, values=None) -> abi.Snapshot:
+    """Build the snapshot of a BASELINE config (or a scaled variant via keyword overrides).
+
+    values: None keeps the requests of the config (cpu milli, memory bytes, ...); "wide", "carry" or "signed" rewrites the
+    request columns of the running and pending pods (VALUE_REGIMES, _rewrite_values) before the thresholds are calibrated, within
+    the domain the host layer guarantees (per column, sum of |v| over running + pending + reservations + status below 2^62), and
+    adds exact-equality thresholds (_equality_thresholds)."""
     base = dict(CONFIGS[config])
     for k, v in dict(seed=seed, m=m, n=n, p=p, R=R, n_ns=n_ns, cluster_frac=cluster_frac, override_frac=override_frac).items():
         if v is not None:
@@ -308,6 +364,15 @@ def generate(config: str = "C2", *, seed=None, m=None, n=None, p=None, R=None, n
 
     running = _gen_pods(rng, n, n_ns, R, L, True, sort_by_namespace)
     pending = _gen_pods(rng, p, n_ns, R, L, False, sort_by_namespace)
+    vrng = None
+    if values is not None:  # its own stream: the default snapshots stay byte-identical
+        vrng = np.random.Generator(np.random.PCG64([seed, VALUE_REGIMES.index(values) if values in VALUE_REGIMES else 99]))
+        # running + pending at most 2^60, status used at most as much again, reservations small: below 2^62 per column
+        bound = (1 << 60) // (n + p)
+        if bound <= HIGH_LIMB + (1 << 40):
+            raise ValueError(f"values={values!r}: {n + p} pods leave no room above 2^44 under the 2^62 column bound")
+        for pods in (running, pending):
+            _rewrite_values(pods, vrng, values, bound)
 
     # throttles: Throttles grouped by namespace first, then ClusterThrottles
     m_c = int(round(m * cluster_frac))
@@ -339,6 +404,10 @@ def generate(config: str = "C2", *, seed=None, m=None, n=None, p=None, R=None, n
     #   0: threshold below the used sum (q in [0.5,1))   1: about one pod of headroom   2: ample headroom (q in [1.2,2])
     typical = np.array([4000, 8 << 30, 8, 100 << 30] + [4] * max(0, R - 4), np.int64)[:R]
     one_pod = np.array([2000, 1 << 30, 2, 50 << 30] + [2] * max(0, R - 4), np.int64)[:R]
+    if values is not None:  # the same regimes of headroom, in units of the rewritten requests
+        one_pod = np.array([max(1, int(np.median(np.abs(pods_r[pods_r != 0])))) if (pods_r != 0).any() else 1
+                            for pods_r in pending.req], np.int64)
+        typical = 4 * one_pod
     regime = rng.integers(0, 3, size=m)
     base_amt = np.where(used > 0, used, typical[:, None])
     q = np.where(regime[None, :] == 0, rng.uniform(0.5, 1.0, size=(R, m)), rng.uniform(1.2, 2.0, size=(R, m)))
@@ -418,6 +487,9 @@ def generate(config: str = "C2", *, seed=None, m=None, n=None, p=None, R=None, n
         reserved[1] = np.where(mem, rcnt * (256 << 20), 0)
         rpresent = np.where(mem, rpresent | 2, rpresent).astype(np.uint32)
     snap.reserved, snap.reserved_present, snap.reserved_cnt = reserved, rpresent, rcnt
+    if vrng is not None:
+        snap.meta["values"] = values
+        _equality_thresholds(snap.normalize(), vrng)
     return snap.normalize()
 
 

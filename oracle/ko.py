@@ -75,6 +75,9 @@ def lib():
         L.ko_world_reserved.argtypes = [C.c_void_p, C.c_int, C.c_char_p]
         L.ko_columnar_evaluate.restype = C.c_int
         L.ko_columnar_evaluate.argtypes = [C.POINTER(ColumnarArgs)]
+        L.ko_columnar_admit_queue.restype = C.c_int
+        L.ko_columnar_admit_queue.argtypes = [C.POINTER(ColumnarArgs), C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
+                                              C.POINTER(C.c_int64)]
         L.ko_world_from_columns.restype = C.c_void_p
         L.ko_world_from_columns.argtypes = [C.POINTER(ColumnarArgs)]
         L.ko_world_run_columns.restype = C.c_double
@@ -185,6 +188,26 @@ def columnar_evaluate(snap: abi.Snapshot, flags: int = abi.EVAL_FRESH_STATUS, wo
     if rc != 0:
         raise RuntimeError("ko_columnar_evaluate failed")
     return out
+
+
+def columnar_admit_queue(snap: abi.Snapshot, first: int, count: int, flags: int = 0, words_per_row: Optional[int] = None):
+    """Queue-ordered greedy admission of the pending rows [first, first + count), one pod per cycle, against snap.status and
+    snap.reserved (flags: KT_EVAL_ON_EQUAL or 0).  Returns (PassResult with pend_bitmap / codes / admit filled, admitted count,
+    (reserved, reserved_present, reserved_cnt) after the queue)."""
+    snap.normalize()
+    if snap.status is None:
+        raise ValueError("columnar_admit_queue checks against the observed status: snap.status is required")
+    out = abi.PassResult.alloc(snap, words_per_row or abi.default_words_per_row(snap.m))
+    keep: list = []
+    a = _args(snap, flags, out, keep)
+    res = np.zeros((snap.R, snap.m), np.int64)
+    res_present = np.zeros(snap.m, np.uint32)
+    res_cnt = np.zeros(snap.m, np.int64)
+    admitted = C.c_int64(0)
+    rc = lib().ko_columnar_admit_queue(C.byref(a), first, count, abi.ptr(res), abi.ptr(res_present), abi.ptr(res_cnt), C.byref(admitted))
+    if rc != 0:
+        raise RuntimeError("ko_columnar_admit_queue failed")
+    return out, admitted.value, (res, res_present, res_cnt)
 
 
 def object_evaluate(snap: abi.Snapshot, flags: int = abi.EVAL_FRESH_STATUS, threads: int = 1, max_pending: int = 0,

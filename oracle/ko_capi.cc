@@ -496,6 +496,21 @@ int ko_columnar_evaluate(const ko_columnar_args* a) {
   return columnar_evaluate(in, out);
 }
 
+// columnar_admit_queue: a->codes / admit / pend_bitmap receive the pending rows (each nullable), res* the final reservations.
+int ko_columnar_admit_queue(const ko_columnar_args* a, int64_t first, int64_t count, int64_t* res, uint32_t* res_present, int64_t* res_cnt,
+                            int64_t* admitted) {
+  ColumnarInput in = to_input(a);
+  ColumnarOutput out;
+  out.rec = kt_reconcile_out{};
+  out.pend_bitmap = a->pend_bitmap;
+  out.codes = a->codes;
+  out.admit = a->admit;
+  const int64_t n = columnar_admit_queue(in, first, count, out, res, res_present, res_cnt);
+  if (n < 0) return -1;
+  *admitted = n;
+  return 0;
+}
+
 // ---------- object World from columns -------------------------------------------------
 // Names: label key "k<id>", value "v<id>", namespace "ns<id>", resource "r<i>", throttles "t<idx>".
 // Column integers become whole-unit Quantities (any common scale gives identical decisions).

@@ -143,6 +143,59 @@ inline Amount add(const Amount& a, const Amount& b, int R) {
   return o;
 }
 
+inline bool live_throttle(const ColumnarInput& in, int32_t t) {
+  return (in.thr.flags[t] & KT_THR_RESPONSIBLE) && !(in.thr.flags[t] & KT_THR_SELECTOR_ERROR);
+}
+
+// PreFilter's view of throttle t under KT_EVAL_GIVEN_STATUS: the observed status's threshold (the spec's while the status has
+// none), used amounts and throttled mask.
+inline void given_status_view(const ColumnarInput& in, int32_t t, Amount* threshold, Amount* st_used, uint32_t* st_throttled) {
+  const int R = in.lim.n_resources;
+  const int32_t M = in.m;
+  const kt_status_cols& s = *in.status;
+  if (s.calculated[t]) {
+    threshold->present = s.calc_present[t];
+    threshold->cnt = s.calc_cnt[t];
+    for (int r = 0; r < R; ++r) threshold->v[r] = s.calc_thr[(int64_t)r * M + t];
+  } else {
+    threshold->present = in.thr.thr_present[t];
+    threshold->cnt = in.thr.thr_cnt[t];
+    for (int r = 0; r < R; ++r) threshold->v[r] = in.thr.thr[(int64_t)r * M + t];
+  }
+  st_used->present = s.used_present[t];
+  st_used->cnt = s.used_cnt[t];
+  for (int r = 0; r < R; ++r) st_used->v[r] = s.used[(int64_t)r * M + t];
+  *st_throttled = s.throttled[t];
+}
+
+// CheckThrottledFor(pod, reserved, onEqual) of pending pod p on throttle t: the 2-bit code.  already = used + reserved.
+inline uint32_t check_code(const ColumnarInput& in, int32_t t, const Amount& threshold, const Amount& already, uint32_t st_throttled, int64_t p) {
+  const int R = in.lim.n_resources;
+  const bool on_equal = in.flags & KT_EVAL_ON_EQUAL;
+  const bool e3 = in.thr.kind[t] == KT_KIND_THROTTLE ? true : on_equal;  // Q1
+  Amount pod{};
+  pod.present = in.pending.present[p] | KT_COUNT_BIT;
+  pod.cnt = 1;
+  uint32_t nz = 0;
+  for (int r = 0; r < R; ++r) {
+    pod.v[r] = in.pending.req[(int64_t)r * in.pending.n + p];
+    if (((pod.present >> r) & 1) && pod.v[r] != 0) nz |= 1u << r;
+  }
+  if (is_throttled_for(is_throttled(threshold, pod, false, R), nz)) return KT_CHECK_POD_REQUESTS_EXCEEDS_THRESHOLD;
+  if (is_throttled_for(st_throttled, nz)) return KT_CHECK_ACTIVE;
+  if (is_throttled_for(is_throttled(threshold, already, e3, R), nz)) return KT_CHECK_ACTIVE;
+  const Amount tot = add(already, pod, R);
+  return is_throttled_for(is_throttled(threshold, tot, on_equal, R), nz) ? KT_CHECK_INSUFFICIENT : KT_CHECK_NOT_THROTTLED;
+}
+
+inline Amount reserved_of(const int64_t* reserved, const uint32_t* present, const int64_t* cnt, int32_t M, int32_t t, int R) {
+  Amount res{};
+  res.present = present ? present[t] : 0;
+  res.cnt = cnt ? cnt[t] : 0;
+  for (int r = 0; r < R; ++r) res.v[r] = reserved ? reserved[(int64_t)r * M + t] : 0;
+  return res;
+}
+
 }  // namespace col
 
 // The whole pass.  Returns 0 or -1 (bad input).
@@ -153,7 +206,6 @@ inline int columnar_evaluate(const ColumnarInput& in, const ColumnarOutput& out)
   const int32_t M = in.m, W = in.words_per_row;
   if (W * 32 < M) return -1;
   const bool given = in.flags & KT_EVAL_GIVEN_STATUS;
-  const bool on_equal = in.flags & KT_EVAL_ON_EQUAL;
 
   if (out.run_bitmap) std::memset(out.run_bitmap, 0, sizeof(uint32_t) * (size_t)N * W);
   if (out.pend_bitmap) std::memset(out.pend_bitmap, 0, sizeof(uint32_t) * (size_t)P * W);
@@ -223,63 +275,88 @@ inline int columnar_evaluate(const ColumnarInput& in, const ColumnarOutput& out)
 
   // ---- check half -----------------------------------------------------------------------
   for (int32_t t = 0; t < M; ++t) {
-    bool live = (in.thr.flags[t] & KT_THR_RESPONSIBLE) && !(in.thr.flags[t] & KT_THR_SELECTOR_ERROR);
-    if (!live) continue;
+    if (!live_throttle(in, t)) continue;
     // which status does PreFilter see?
     Amount threshold, st_used;
     uint32_t st_throttled;
     if (given) {
-      const kt_status_cols& s = *in.status;
-      if (s.calculated[t]) {
-        threshold.present = s.calc_present[t];
-        threshold.cnt = s.calc_cnt[t];
-        for (int r = 0; r < R; ++r) threshold.v[r] = s.calc_thr[(int64_t)r * M + t];
-      } else {
-        threshold.present = in.thr.thr_present[t];
-        threshold.cnt = in.thr.thr_cnt[t];
-        for (int r = 0; r < R; ++r) threshold.v[r] = in.thr.thr[(int64_t)r * M + t];
-      }
-      st_used.present = s.used_present[t];
-      st_used.cnt = s.used_cnt[t];
-      for (int r = 0; r < R; ++r) st_used.v[r] = s.used[(int64_t)r * M + t];
-      st_throttled = s.throttled[t];
+      given_status_view(in, t, &threshold, &st_used, &st_throttled);
     } else {
       threshold = calc[t];
       st_used = used[t];
       st_throttled = throttled[t];
     }
-    Amount res{};
-    res.present = in.reserved_present ? in.reserved_present[t] : 0;
-    res.cnt = in.reserved_cnt ? in.reserved_cnt[t] : 0;
-    for (int r = 0; r < R; ++r) res.v[r] = in.reserved ? in.reserved[(int64_t)r * M + t] : 0;
-    Amount already = add(st_used, res, R);
-    bool e3 = in.thr.kind[t] == KT_KIND_THROTTLE ? true : on_equal;  // Q1
-    uint32_t mask3 = is_throttled(threshold, already, e3, R);
+    const Amount already = add(st_used, reserved_of(in.reserved, in.reserved_present, in.reserved_cnt, M, t, R), R);
 
     for (int64_t p = 0; p < P; ++p) {
       if (!throttle_matches(in, t, in.pending, p)) continue;
       if (out.pend_bitmap) out.pend_bitmap[(size_t)p * W + (t >> 5)] |= 1u << (t & 31);
-      Amount pod{};
-      pod.present = in.pending.present[p] | KT_COUNT_BIT;
-      pod.cnt = 1;
-      uint32_t nz = 0;
-      for (int r = 0; r < R; ++r) {
-        pod.v[r] = in.pending.req[(int64_t)r * P + p];
-        if (((pod.present >> r) & 1) && pod.v[r] != 0) nz |= 1u << r;
-      }
-      uint32_t code;
-      if (is_throttled_for(is_throttled(threshold, pod, false, R), nz)) code = KT_CHECK_POD_REQUESTS_EXCEEDS_THRESHOLD;
-      else if (is_throttled_for(st_throttled, nz)) code = KT_CHECK_ACTIVE;
-      else if (is_throttled_for(mask3, nz)) code = KT_CHECK_ACTIVE;
-      else {
-        Amount tot = add(already, pod, R);
-        code = is_throttled_for(is_throttled(threshold, tot, on_equal, R), nz) ? KT_CHECK_INSUFFICIENT : KT_CHECK_NOT_THROTTLED;
-      }
+      const uint32_t code = check_code(in, t, threshold, already, st_throttled, p);
       if (out.codes) out.codes[(size_t)p * 2 * W + (t >> 4)] |= code << (2 * (t & 15));
       if (code != KT_CHECK_NOT_THROTTLED && out.admit) out.admit[p] = 0;
     }
   }
   return 0;
+}
+
+// Queue-ordered greedy admission, one pod per cycle (scheduler_plugin/plugin.go:148-238): the pending rows
+// [first, first + count) in row order, each checked (PreFilter) against the observed status + the reservations so far; on
+// Success its ResourceAmountOfPod -- every present request, zero or not, and Counts{Pod: 1} -- joins the reservation of
+// every throttle it affects (Reserve, reserved_resource_amounts.go:66-136).  Rows outside the queue keep the codes of one
+// KT_EVAL_GIVEN_STATUS | KT_EVAL_SKIP_RECONCILE pass.  in.status is required; in.flags contributes KT_EVAL_ON_EQUAL only.
+// res / res_present / res_cnt ([R][m], [m], [m]) receive the final reservations.  O(P x m) for the one pass, then
+// O(count x m).  Returns the admitted count, or -1 (bad input).
+inline int64_t columnar_admit_queue(const ColumnarInput& in_, int64_t first, int64_t count, const ColumnarOutput& out_, int64_t* res,
+                                    uint32_t* res_present, int64_t* res_cnt) {
+  using namespace col;
+  const int R = in_.lim.n_resources;
+  const int64_t P = in_.pending.n;
+  const int32_t M = in_.m, W = in_.words_per_row;
+  if (!in_.status || first < 0 || count < 0 || first + count > P || W * 32 < M) return -1;
+  ColumnarInput in = in_;
+  in.flags = KT_EVAL_GIVEN_STATUS | KT_EVAL_SKIP_RECONCILE | (in_.flags & KT_EVAL_ON_EQUAL);
+  for (int32_t t = 0; t < M; ++t) {
+    const Amount a = reserved_of(in_.reserved, in_.reserved_present, in_.reserved_cnt, M, t, R);
+    for (int r = 0; r < R; ++r) res[(int64_t)r * M + t] = a.v[r];
+    res_present[t] = a.present;
+    res_cnt[t] = a.cnt;
+  }
+  std::vector<uint32_t> bitmap((size_t)P * W + 1, 0);
+  ColumnarOutput out = out_;
+  out.pend_bitmap = bitmap.data();
+  if (columnar_evaluate(in, out) != 0) return -1;
+  if (out_.pend_bitmap) std::memcpy(out_.pend_bitmap, bitmap.data(), sizeof(uint32_t) * (size_t)P * W);
+
+  std::vector<Amount> threshold(M), st_used(M);
+  std::vector<uint32_t> st_throttled(M, 0);
+  for (int32_t t = 0; t < M; ++t)
+    if (live_throttle(in, t)) given_status_view(in, t, &threshold[t], &st_used[t], &st_throttled[t]);
+  const uint32_t rmask = R >= 32 ? 0xffffffffu : ((1u << R) - 1u);
+  int64_t admitted = 0;
+  for (int64_t p = first; p < first + count; ++p) {
+    const uint32_t* row = &bitmap[(size_t)p * W];
+    bool ok = true;
+    if (out.codes) std::memset(&out.codes[(size_t)p * 2 * W], 0, sizeof(uint32_t) * 2 * W);
+    for (int32_t t = 0; t < M; ++t) {
+      if (!((row[t >> 5] >> (t & 31)) & 1)) continue;  // the pass sets bits of live throttles only
+      const Amount already = add(st_used[t], reserved_of(res, res_present, res_cnt, M, t, R), R);
+      const uint32_t code = check_code(in, t, threshold[t], already, st_throttled[t], p);
+      if (out.codes) out.codes[(size_t)p * 2 * W + (t >> 4)] |= code << (2 * (t & 15));
+      if (code != KT_CHECK_NOT_THROTTLED) ok = false;
+    }
+    if (out.admit) out.admit[p] = ok;
+    if (!ok) continue;
+    ++admitted;
+    const uint32_t pres = in.pending.present[p] & rmask;
+    for (int32_t t = 0; t < M; ++t) {
+      if (!((row[t >> 5] >> (t & 31)) & 1)) continue;
+      for (int r = 0; r < R; ++r)
+        if ((pres >> r) & 1) res[(int64_t)r * M + t] += in.pending.req[(int64_t)r * P + p];
+      res_present[t] |= pres | KT_COUNT_BIT;
+      res_cnt[t] += 1;
+    }
+  }
+  return admitted;
 }
 
 }  // namespace ko

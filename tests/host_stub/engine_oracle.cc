@@ -31,6 +31,8 @@ struct ko_columnar_args {
   uint32_t* run_bitmap; uint32_t* pend_bitmap; uint32_t* codes; uint8_t* admit;
 };
 extern "C" int ko_columnar_evaluate(const ko_columnar_args* a);
+extern "C" int ko_columnar_admit_queue(const ko_columnar_args* a, int64_t first, int64_t count, int64_t* res, uint32_t* res_present,
+                                       int64_t* res_cnt, int64_t* admitted);
 
 namespace {
 template <class T>
@@ -70,7 +72,11 @@ struct kt_ctx {
 
 static int fail(kt_ctx* c, int code, const char* msg) { c->err = msg; return code; }
 
+struct AdmitCall { int64_t first, count, admitted; };  // a queue to admit after the pass
+
 extern "C" {
+static int evaluate(kt_ctx* c, int64_t now, uint32_t flags, AdmitCall* q);
+
 int kt_create(kt_ctx** out, int, const kt_limits* lim) {
   if (!out || !lim || lim->abi_version != KT_ABI_VERSION) return KT_ERR_INVALID;
   if (lim->n_resources < 1 || lim->n_resources > KT_MAX_RESOURCES || lim->label_slots < 1 || lim->label_slots > KT_MAX_LABEL_SLOTS) return KT_ERR_LIMIT;
@@ -154,7 +160,25 @@ int kt_set_reserved(kt_ctx* c, const int64_t* reserved, const uint32_t* present,
 }
 int32_t kt_match_words(const kt_ctx* c) { return c && c->have_throttles ? c->words() : 0; }
 
-int kt_evaluate(kt_ctx* c, int64_t now, uint32_t flags) {
+int kt_evaluate(kt_ctx* c, int64_t now, uint32_t flags) { return evaluate(c, now, flags, nullptr); }
+
+// Queue-ordered greedy admission: the columnar oracle's pod-by-pod loop (columnar_admit_queue; the device runs a prefix-sum
+// fixpoint, csrc/kt_admit.cuh) -- PreFilter against the observed status + the reservations so far, and on Success the pod's
+// ResourceAmountOfPod joins the reservation of every throttle it affects (plugin.go:148-238).  The reservations uploaded with
+// kt_set_reserved are left as they were, as on the device.
+int kt_admit_queue(kt_ctx* c, int64_t first, int64_t count, uint32_t flags, int32_t* rounds, int64_t* admitted) {
+  if (!c || first < 0 || count < 0) return KT_ERR_INVALID;
+  if (!c->have_status) return fail(c, KT_ERR_STATE, "kt_admit_queue without kt_upload_status");
+  if (first + count > c->pods[KT_PODS_PENDING].n) return fail(c, KT_ERR_INVALID, "queue rows outside the pending table");
+  AdmitCall q{first, count, 0};
+  const int rc = evaluate(c, 0, KT_EVAL_GIVEN_STATUS | KT_EVAL_SKIP_RECONCILE | (flags & KT_EVAL_ON_EQUAL), &q);
+  if (rc != KT_OK) return rc;
+  if (rounds) *rounds = 2;
+  if (admitted) *admitted = q.admitted;
+  return KT_OK;
+}
+
+static int evaluate(kt_ctx* c, int64_t now, uint32_t flags, AdmitCall* q) {
   if (!c) return KT_ERR_INVALID;
   if (!c->have_throttles) return fail(c, KT_ERR_STATE, "kt_evaluate before kt_upload_throttles");
   if ((flags & KT_EVAL_GIVEN_STATUS) && !c->have_status) return fail(c, KT_ERR_STATE, "KT_EVAL_GIVEN_STATUS without kt_upload_status");
@@ -189,6 +213,12 @@ int kt_evaluate(kt_ctx* c, int64_t now, uint32_t flags) {
                            c->o_calc_present.data(), c->o_calc_cnt.data(), c->o_ovr_active.data()};
   a.run_bitmap = c->run_bitmap.data(); a.pend_bitmap = c->pend_bitmap.data(); a.codes = c->codes.data(); a.admit = c->admit.data();
   if (ko_columnar_evaluate(&a) != 0) return fail(c, KT_ERR_INVALID, "ko_columnar_evaluate failed");
+  if (q) {  // the queue rows again, pod by pod (the pass above gave the reconcile columns and the rows outside the queue)
+    std::vector<int64_t> res(R * M + 1), res_cnt(M + 1);
+    std::vector<uint32_t> res_present(M + 1);
+    if (ko_columnar_admit_queue(&a, q->first, q->count, res.data(), res_present.data(), res_cnt.data(), &q->admitted) != 0)
+      return fail(c, KT_ERR_INVALID, "ko_columnar_admit_queue failed");
+  }
   c->evaluated = true;
   return KT_OK;
 }
@@ -281,54 +311,6 @@ int kt_get_reconcile_rows(kt_ctx* c, int64_t k, const int32_t* idx, const kt_rec
     if (o->calc_present) o->calc_present[i] = c->o_calc_present[t];
     if (o->override_active) o->override_active[i] = c->o_ovr_active[t];
   }
-  return KT_OK;
-}
-// Queue-ordered greedy admission, the slow and obvious way (the device runs a prefix-sum fixpoint, csrc/kt_admit.cuh): one
-// pod at a time in row order -- PreFilter against the observed status + the reservations so far, and on Success the pod's
-// ResourceAmountOfPod joins the reservation of every throttle it affects (plugin.go:148-238, reserved_resource_amounts.go:66-136).
-int kt_admit_queue(kt_ctx* c, int64_t first, int64_t count, uint32_t flags, int32_t* rounds, int64_t* admitted) {
-  if (!c || first < 0 || count < 0) return KT_ERR_INVALID;
-  if (!c->have_status) return fail(c, KT_ERR_STATE, "kt_admit_queue without kt_upload_status");
-  const Pods& pend = c->pods[KT_PODS_PENDING];
-  if (first + count > pend.n) return fail(c, KT_ERR_INVALID, "queue rows outside the pending table");
-  const size_t M = (size_t)c->m, R = (size_t)c->lim.n_resources, Wp = (size_t)c->words();
-  const uint32_t f = KT_EVAL_GIVEN_STATUS | KT_EVAL_SKIP_RECONCILE | (flags & KT_EVAL_ON_EQUAL);
-  const auto saved_r = c->reserved; const auto saved_p = c->reserved_present; const auto saved_c = c->reserved_cnt;
-  const bool saved_have = c->have_reserved;
-  if (!c->have_reserved) { c->reserved.assign(R * M, 0); c->reserved_present.assign(M, 0); c->reserved_cnt.assign(M, 0); }
-  c->have_reserved = true;
-  int rc = kt_evaluate(c, 0, f);
-  std::vector<uint32_t> codes = c->codes;
-  std::vector<uint8_t> admit = c->admit;
-  int64_t n_adm = 0;
-  bool dirty = false;
-  for (int64_t i = first; rc == KT_OK && i < first + count; ++i) {
-    if (dirty) { rc = kt_evaluate(c, 0, f); dirty = false; }
-    if (rc != KT_OK) break;
-    std::memcpy(&codes[(size_t)i * 2 * Wp], &c->codes[(size_t)i * 2 * Wp], 2 * Wp * 4);
-    admit[(size_t)i] = c->admit[(size_t)i];
-    if (!admit[(size_t)i]) continue;
-    ++n_adm;
-    const uint32_t present = pend.present[(size_t)i];
-    for (size_t w = 0; w < Wp; ++w)
-      for (uint32_t bits = c->pend_bitmap[(size_t)i * Wp + w]; bits; bits &= bits - 1) {
-        const size_t t = w * 32 + (size_t)__builtin_ctz(bits);
-        if (t >= M) continue;
-        for (size_t r = 0; r < R; ++r)
-          if ((present >> r) & 1) c->reserved[r * M + t] += pend.req[r * (size_t)pend.n + (size_t)i];
-        c->reserved_present[t] |= (present & (R >= 32 ? 0xffffffffu : ((1u << R) - 1u))) | KT_COUNT_BIT;
-        c->reserved_cnt[t] += 1;
-        dirty = true;
-      }
-  }
-  c->reserved = saved_r; c->reserved_present = saved_p; c->reserved_cnt = saved_c;
-  c->have_reserved = saved_have;
-  if (rc != KT_OK) return rc;
-  c->codes = codes;
-  c->admit = admit;
-  c->evaluated = true;
-  if (rounds) *rounds = 2;
-  if (admitted) *admitted = n_adm;
   return KT_OK;
 }
 // the sparse list of the double: the non-zero code words of the dense rows, in row order

@@ -67,6 +67,12 @@ def test_c1_example(kt, oracle):
     dict(config="C3", m=300, n=6000, p=800, column_layout=True),          # ClusterThrottles in the host layer's column order (by namespace set)
     dict(config="C2", m=150, n=300, p=6000),                              # far more pending than running rows: 50 CTAs serve ~200 decide sub-tiles / status tiles
     dict(config="C3", m=400, n=500, p=5000, sort_by_namespace=False),     # the same with ClusterThrottles and rows in arrival order: several rounds per sub-tile, pairs checked straight from L2
+] + [  # request values at the edges of the 64-bit sums (synth.VALUE_REGIMES) through the register (R=4), direct-RED (R=8, more
+    # distinct words than slots) and shared-memory (R=12) accumulation paths
+    dict(kw, values=v) for v in synth.VALUE_REGIMES for kw in (
+        dict(config="C2", m=200, n=5000, p=700),
+        dict(config="C3", m=1000, n=20000, p=2000, sort_by_namespace=False),
+        dict(config="C2", m=150, n=4000, p=600, R=12))
 ])
 def test_scaled_configs(kt, oracle, kw):
     kw = dict(kw)
@@ -105,15 +111,17 @@ def test_sparse_dictionary_ids(kt, oracle, mode):
     np.testing.assert_array_equal(got.used, base.used)
 
 
-def test_on_equal_flag(kt, oracle):
-    snap = synth.generate("C3", m=300, n=6000, p=800)
+@pytest.mark.parametrize("values", (None,) + synth.VALUE_REGIMES)
+def test_on_equal_flag(kt, oracle, values):
+    snap = synth.generate("C3", m=300, n=6000, p=800, values=values)
     got, want = run_both(kt, oracle, snap, abi.EVAL_ON_EQUAL)
     assert_same(snap, got, want)
 
 
-def test_given_status(kt, oracle):
+@pytest.mark.parametrize("values", (None,) + synth.VALUE_REGIMES)
+def test_given_status(kt, oracle, values):
     """PreFilter between reconciles: the check uses an uploaded (stale) status, not this pass's."""
-    snap = synth.generate("C4", m=400, n=6000, p=900)
+    snap = synth.generate("C4", m=400, n=6000, p=900, values=values)
     fresh = oracle.columnar_evaluate(snap)
     rng = np.random.default_rng(7)
     m, R = snap.m, snap.R
@@ -172,12 +180,13 @@ def test_repeat_pass_is_idempotent(kt):
     eng.close()
 
 
-def test_fused_and_chained_paths_agree(kt, oracle):
+@pytest.mark.parametrize("values", (None,) + synth.VALUE_REGIMES)
+def test_fused_and_chained_paths_agree(kt, oracle, values):
     """kt_evaluate runs the whole pass as ONE launch (k_pass: ticketed reconcile / finalize / check tiles with in-kernel
     hand-offs); with per-kernel timing enabled it runs the three PDL-chained kernels instead.  Same bits either way,
     pass after pass (the ticket / done counters re-arm themselves)."""
     for kw in (dict(config="C3", m=300, n=6000, p=800), dict(config="C2", m=1000, n=30000, p=3000), dict(config="C2", m=40, n=70, p=33, R=1)):
-        kw = dict(kw)
+        kw = dict(kw, values=values)
         snap = synth.generate(kw.pop("config"), **kw)
         eng = kt.Engine(snap.R, snap.L, snap.LN)
         eng.upload_snapshot(snap)
@@ -251,20 +260,27 @@ def test_no_gpu_error_contract(kt):
     eng.close()
 
 
-def test_packed_upload_equals_wide_upload(kt, oracle):
+@pytest.mark.parametrize("values", (None,) + synth.VALUE_REGIMES)
+def test_packed_upload_equals_wide_upload(kt, oracle, values):
     """kt_upload_pods_packed (16-bit label-pair indices, presence in the meta word) expands to exactly the int64 columns
-    kt_upload_pods would have copied: same bits out."""
+    kt_upload_pods would have copied: same bits out.  Requests beyond int32 (the value regimes) travel dictionary-coded; the
+    int32 packer refuses them."""
     for kw in (dict(config="C3", m=300, n=6000, p=800), dict(config="C2", m=200, n=5000, p=700, L=12), dict(config="C2", m=40, n=70, p=33, R=1, L=3),
                dict(config="C4", m=500, n=3000, p=400)):
-        kw = dict(kw)
+        kw = dict(kw, values=values)
         snap = synth.generate(kw.pop("config"), **kw)
         eng = kt.Engine(snap.R, snap.L, snap.LN)
         eng.upload_snapshot(snap)
         want = None
         for coded in (False, True):  # int32 request columns, then dictionary-coded ones
+            if values is not None and not coded:
+                for pods in (snap.running, snap.pending):
+                    with pytest.raises(ValueError):
+                        abi.packed_pods(pods, code_requests=False)
+                continue
             for kind, pods in ((abi.PODS_RUNNING, snap.running), (abi.PODS_PENDING, snap.pending)):
                 pk = abi.packed_pods(pods, code_requests=coded)
-                if pods.n >= 1000:  # the pair dictionary is a fixed cost: only rows amortise it
+                if pods.n >= 1000 and values is None:  # the pair dictionary is a fixed cost: only rows amortise it
                     assert pk.nbytes < 0.65 * sum(a.nbytes for a in (pods.labels, pods.req, pods.present, pods.flags, pods.ns_id))
                 eng.upload_pods_packed(kind, pk)
             eng.evaluate(snap.now)
@@ -430,59 +446,100 @@ def test_step_api_equals_separate_calls(kt, oracle):
         eng.close()
 
 
-@pytest.mark.parametrize("kw", [dict(config="C2", m=200, n=4000, p=1000), dict(config="C3", m=120, n=3000, p=600, seed=9)])
-def test_device_queue_admission_equals_pod_by_pod(kt, oracle, kw):
+C2Q = dict(config="C2", m=200, n=4000, p=2600)
+
+
+@pytest.mark.parametrize("world,first,count,flags", [
+    (dict(config="C2", m=200, n=4000, p=1000), 0, None, 0),
+    (dict(config="C3", m=120, n=3000, p=600, seed=9), 0, None, 0),
+    (C2Q, 0, 1, 0),                  # queue lengths around one CSR block (kAdmitBlock = 1024 queue positions)
+    (C2Q, 0, 1023, 0),
+    (C2Q, 0, 1024, 0),
+    (C2Q, 0, 1025, 0),
+    (C2Q, 0, 2500, 0),
+    (C2Q, 41, 1025, 0),              # a sub-range of the pending table: the rows around it keep the pass's codes and admit bits
+    (C2Q, 1500, 1024, abi.EVAL_ON_EQUAL),
+    (dict(config="C4", m=2500, n=20000, p=1500), 0, None, 0),  # M > 1024: k_admit_starts scans ranges; overrides active
+    (dict(config="C2", m=200, n=4000, p=1000, R=1), 0, None, 0),            # each k_admit_round<RMAX>, and the first R past each bound
+    (dict(config="C3", m=200, n=3000, p=800, R=5), 0, None, 0),
+    (dict(config="C3", m=200, n=3000, p=800, R=9), 0, None, abi.EVAL_ON_EQUAL),
+    (dict(config="C3", m=120, n=2000, p=600, R=31, L=16), 0, None, 0),
+    (dict(config="C3", m=120, n=3000, p=600, seed=9), 0, None, abi.EVAL_ON_EQUAL),
+    (dict(config="C2", m=200, n=4000, p=1000, throttled=True, zero_counts=True), 0, None, 0),
+    (dict(config="C2", m=200, n=4000, p=1000, orphans=True), 0, None, 0),   # pods that affect no throttle
+    (dict(config="C2", m=200, n=4000, p=1500, values="signed"), 0, None, 0),
+    (dict(config="C3", m=200, n=3000, p=1200, values="signed"), 100, 1000, abi.EVAL_ON_EQUAL),
+])
+def test_device_queue_admission_equals_pod_by_pod(kt, oracle, world, first, count, flags):
     """SURVEY 8f.2: kt_admit_queue (per-throttle prefix sums over the admitted pods, iterated to the fixpoint on the device) gives
-    every pod of a 1000-pod queue the verdict and the check codes it gets when the queue is admitted ONE POD PER CYCLE --
-    PreFilter against observed status + reservations, Reserve on Success (plugin.go:148-238) -- emulated here with one oracle
-    evaluation per admitted pod."""
-    kw = dict(kw)
-    snap = synth.generate(kw.pop("config"), **kw)
-    fresh = oracle.columnar_evaluate(snap)
-    m, R, P = snap.m, snap.R, snap.pending.n
-    snap.status = dict(calculated=np.ones(m, np.uint8), calc_thr=fresh.calc_thr.copy(), calc_present=fresh.calc_present.copy(), calc_cnt=fresh.calc_cnt.copy(),
-                       used=fresh.used.copy(), used_present=fresh.used_present.copy(), used_cnt=fresh.used_cnt.copy(), throttled=fresh.throttled.copy())
-    # room for a few pods on most throttles, so that admissions and rejections interleave along the queue
-    rng = np.random.default_rng(3)
-    snap.thr = np.where(snap.thr > 0, fresh.used + (snap.thr * rng.uniform(0.0, 0.08, size=snap.thr.shape)).astype(np.int64) + 1, 0)
-    snap.thr_cnt = np.where(snap.thr_cnt > 0, fresh.used_cnt + rng.integers(0, 6, size=m), snap.thr_cnt)
-    snap.status["calc_thr"], snap.status["calc_cnt"] = snap.thr.copy(), snap.thr_cnt.copy()
-    snap.status["calc_present"] = snap.thr_present.copy()
-    snap.status["throttled"] = np.zeros(m, np.uint32)
-    snap.normalize()
-    flags = abi.EVAL_GIVEN_STATUS | abi.EVAL_SKIP_RECONCILE
+    every pod of the queue the verdict and the check codes it gets when the queue is admitted ONE POD PER CYCLE -- PreFilter
+    against observed status + reservations, Reserve on Success (plugin.go:148-238) -- as the columnar oracle's
+    columnar_admit_queue walks it; the pending rows outside the queue keep the codes of a GIVEN_STATUS | SKIP_RECONCILE pass."""
+    from test_oracle_admission import FLAGS, admission_world
+
+    world = dict(world)
+    snap = admission_world(oracle, world.pop("config"), **world)
+    P = snap.pending.n
+    count = P - first if count is None else count
     eng = kt.Engine(snap.R, snap.L, snap.LN)
     eng.upload_snapshot(snap)
-    rounds, admitted = eng.admit_queue(0, P)
+    rounds, admitted = eng.admit_queue(first, count, flags)
     got = eng.download()
     eng.close()
-    # the reference sequence, one pod per cycle
-    W = got.words_per_row
-    base_reserved, base_present, base_cnt = snap.reserved.copy(), snap.reserved_present.copy(), snap.reserved_cnt.copy()
-    want_codes = np.zeros((P, 2 * W), np.uint32)
-    want_admit = np.zeros(P, np.uint8)
-    cur = oracle.columnar_evaluate(snap, flags, words_per_row=W)
-    bitmap = cur.pend_bitmap
-    rmask = np.uint32((1 << R) - 1)
-    n_adm = 0
-    for i in range(P):
-        want_codes[i], want_admit[i] = cur.codes[i], cur.admit[i]
-        if not cur.admit[i]:
-            continue
-        n_adm += 1
-        ts = np.nonzero(((bitmap[i][:, None] >> np.arange(32, dtype=np.uint32)) & 1).reshape(-1)[:m])[0]
-        if ts.size == 0:
-            continue
-        pres = snap.pending.present[i] & rmask
-        for r in range(R):
-            if (pres >> np.uint32(r)) & 1:
-                snap.reserved[r, ts] += snap.pending.req[r, i]
-        snap.reserved_present[ts] |= pres | abi.COUNT_BIT
-        snap.reserved_cnt[ts] += 1
-        snap.normalize()
-        cur = oracle.columnar_evaluate(snap, flags, words_per_row=W)
-    snap.reserved, snap.reserved_present, snap.reserved_cnt = base_reserved, base_present, base_cnt
-    np.testing.assert_array_equal(got.admit, want_admit)
-    np.testing.assert_array_equal(got.codes, want_codes)
-    assert admitted == n_adm and 0.05 * P < n_adm < 0.95 * P, (n_adm, P)  # not degenerate
+    want, n_adm, _ = oracle.columnar_admit_queue(snap, first, count, flags, words_per_row=got.words_per_row)
+    np.testing.assert_array_equal(got.pend_bitmap, want.pend_bitmap)
+    np.testing.assert_array_equal(got.admit, want.admit)
+    np.testing.assert_array_equal(got.codes, want.codes)
+    assert admitted == n_adm
+    if first > 0 or first + count < P:  # the rows outside the queue, once more against the plain pass
+        out = np.ones(P, bool)
+        out[first:first + count] = False
+        plain = oracle.columnar_evaluate(snap, FLAGS | flags, words_per_row=got.words_per_row)
+        np.testing.assert_array_equal(got.codes[out], plain.codes[out])
+        np.testing.assert_array_equal(got.admit[out], plain.admit[out])
+    if count >= 500:
+        assert 0.05 * count < n_adm < 0.95 * count, (n_adm, count)  # not degenerate
     assert 2 <= rounds <= 64, rounds
+
+
+def _two_pod_world():
+    """T1: cpu threshold 10, observed used 5.  T2: pod: 0.  Queue: A (cpu -5, on T1 and T2), then B (cpu 8, on T1)."""
+    L, R, LN = 2, 1, 1
+    lab = np.full((L, 2), abi.LABEL_EMPTY, np.int64)
+    lab[0] = (np.int64(0) << 32) | 0                 # k0=v0: both pods (T1's selector)
+    lab[1, 0] = (np.int64(1) << 32) | 0              # k1=v0: A only (T2's selector)
+    pending = abi.PodCols(lab, np.array([[-5, 8]], np.int64), np.ones(2, np.uint32), np.full(2, abi.POD_SCHEDULER_MATCH | abi.POD_NOT_FINISHED, np.uint32),
+                          np.zeros(2, np.int32))
+    running = abi.PodCols(np.full((L, 0), abi.LABEL_EMPTY, np.int64), np.zeros((R, 0), np.int64), np.zeros(0, np.uint32), np.zeros(0, np.uint32),
+                          np.zeros(0, np.int32))
+    sel = synth.build_selector_csr([0, 1, 2], [[(0, abi.OP_IN, [0])], [(1, abi.OP_IN, [0])]], [[], []])
+    thr, thr_present, thr_cnt = np.array([[10, 0]], np.int64), np.array([1, abi.COUNT_BIT], np.uint32), np.array([0, 0], np.int64)
+    snap = abi.Snapshot(
+        R=R, L=L, LN=LN, running=running, pending=pending, ns_labels=np.full((LN, 1), abi.LABEL_EMPTY, np.int64),
+        kind=np.zeros(2, np.uint8), thr_ns=np.zeros(2, np.int32), thr_flags=np.full(2, abi.THR_RESPONSIBLE, np.uint8),
+        thr=thr, thr_present=thr_present, thr_cnt=thr_cnt,
+        ovr_off=np.zeros(3, np.int32), ovr_begin=np.zeros(0, np.int64), ovr_end=np.zeros(0, np.int64),
+        ovr_flags=np.zeros(0, np.uint8), ovr_thr=np.zeros((R, 0), np.int64), ovr_present=np.zeros(0, np.uint32),
+        ovr_cnt=np.zeros(0, np.int64), now=synth.NOW_2026, **sel)
+    snap.status = dict(calculated=np.ones(2, np.uint8), calc_thr=thr.copy(), calc_present=thr_present.copy(), calc_cnt=thr_cnt.copy(),
+                       used=np.array([[5, 0]], np.int64), used_present=np.array([1 | abi.COUNT_BIT, 0], np.uint32),
+                       used_cnt=np.array([1, 0], np.int64), throttled=np.zeros(2, np.uint32))
+    return snap.normalize()
+
+
+def test_device_queue_admission_with_a_negative_request(kt, oracle):
+    """A negative undecided request lowers the load the pods behind it see.  One pod per cycle: A is rejected (S1 on T2's pod
+    count of 0), so B sees 5 + 8 > 10 on T1 and is insufficient.  Bounding the load from above by "Admitted + Undecided" let B
+    see 5 - 5 + 8 and admitted it."""
+    snap = _two_pod_world()
+    want, n_adm, _ = oracle.columnar_admit_queue(snap, 0, 2, 0, words_per_row=4)
+    assert list(want.admit) == [0, 0] and n_adm == 0
+    assert list(want.code_matrix(2)[:, 0]) == [0, abi.CHECK_INSUFFICIENT] and want.code_matrix(2)[0, 1] == abi.CHECK_POD_REQUESTS_EXCEEDS_THRESHOLD
+    eng = kt.Engine(snap.R, snap.L, snap.LN)
+    eng.upload_snapshot(snap)
+    rounds, admitted = eng.admit_queue(0, 2)
+    got = eng.download()
+    eng.close()
+    np.testing.assert_array_equal(got.admit, want.admit)
+    np.testing.assert_array_equal(got.codes, want.codes)
+    assert admitted == 0

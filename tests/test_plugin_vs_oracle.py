@@ -343,6 +343,69 @@ def test_admit_queue_with_pods_that_already_hold_a_reservation(oracle, new_plugi
     dut.close()
 
 
+@pytest.mark.parametrize("seed", [11, 19])
+def test_admit_queue_with_negative_requests(oracle, new_plugin, seed):
+    """Quantities are signed, and a negative request of an undecided pod LOWERS the load the pods behind it see: the device's
+    fixpoint bounds that load with the undecided pods' negative parts from below and their positive parts from above.  Such a
+    queue is admitted on the device (onDevice) with the verdicts and reservations of one pod per cycle.  The first queue is the
+    smallest one the unsigned bounds got wrong: A (cpu -5, on t1 and on t2 with pod: 0) is rejected, so B (cpu 8) sees t1's
+    5 + 8 > 10 -- under "Admitted + Undecided" it saw 5 - 5 + 8 and was admitted."""
+    from test_scenarios import pod, throttle
+
+    rng = random.Random(seed)
+    ref, dut = oracle.World(THROTTLER, SCHED), new_plugin(THROTTLER, SCHED)
+    both = lambda *m: (ref.apply(*m), dut.apply(*m))
+    nss = [f"ns{i}" for i in range(3)]
+    for n in nss:
+        both(namespace(n, {"team": rng.choice(VALS), "env": rng.choice(VALS)}))
+    throttles = [throttle("ns0", "t1", {"app": "x"}, cpu="10"), throttle("ns0", "t2", {"tier": "y"}, pod_cnt=0)]
+    both(*throttles)
+    both(pod("ns0", "r0", "5", {"app": "x"}, node="n1", phase="Running"))
+
+    def more():  # after the two-pod queue: random throttles with roomy thresholds, as in test_admit_queue_equals_one_pod_per_cycle
+        for i in range(30):
+            t = rand_throttle(rng, i + 3, nss)
+            thr = t["spec"]["threshold"]
+            if "resourceCounts" in thr:
+                thr["resourceCounts"]["pod"] = rng.choice([2, 5, 9, 40])
+            if "cpu" in thr.get("resourceRequests", {}):
+                thr["resourceRequests"]["cpu"] = rng.choice(["1", "2500m", "7", "30"])
+            t["spec"].pop("temporaryThresholdOverrides", None)
+            throttles.append(t)
+            both(t)
+        both(*[rand_pod(rng, rng.choice(nss), f"p{i}", True) for i in range(30)])
+        queue = []
+        for i in range(120):
+            p = rand_pod(rng, rng.choice(nss), f"q{i}", False)
+            if rng.random() < 0.3:
+                p["spec"]["containers"][0]["resources"]["requests"]["cpu"] = "-500m"
+            queue.append(p)
+        return queue
+
+    verdicts = []
+    for queue in ([pod("ns0", "a", "-5", {"app": "x", "tier": "y"}), pod("ns0", "b", "8", {"app": "x"})], None):
+        queue = queue or more()
+        ref.reconcile_all(NOW), dut.reconcile_all(NOW)
+        want = []
+        verdicts.append(want)
+        for p in queue:  # one pod per scheduling cycle
+            r = ref.prefilter(p)
+            if r["code"] == "Success":
+                assert ref.reserve(p)["code"] == "Success"
+            want.append(norm_prefilter(r))
+        got = dut.admit_queue(queue)
+        assert got.get("onDevice") is True
+        assert [norm_prefilter(x["preFilter"]) for x in got["results"]] == want
+        assert got["admitted"] == sum(w["code"] == "Success" for w in want)
+        for t in throttles:
+            k, nn = t["kind"], t["metadata"].get("namespace", "") + "/" + t["metadata"]["name"]
+            a, b = ref.reserved(k, nn), dut.reserved(k, nn)
+            assert sorted(a["pods"]) == sorted(b["pods"]) and norm_amount(a["amount"]) == norm_amount(b["amount"]), (nn, a, b)
+    assert [w["reasons"] for w in verdicts[0]] == [["throttle[pod-requests-exceeds-threshold]=ns0/t2"], ["throttle[insufficient]=ns0/t1"]]
+    assert 5 < sum(w["code"] == "Success" for w in verdicts[1]) < len(queue) - 5
+    dut.close()
+
+
 def test_engine_limits_grow(oracle, new_plugin):
     """More label slots / resource columns / namespace labels than the engine was created with: the host layer re-creates
     the engine with larger limits and re-uploads its caches; decisions stay identical to the oracle's."""
