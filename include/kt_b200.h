@@ -192,13 +192,14 @@ int kt_set_stream(kt_ctx* ctx, void* cuda_stream);
 int kt_sync(kt_ctx* ctx);
 /* Record CUDA events around each kernel of kt_evaluate so kt_get_timing reports device times. */
 int kt_enable_timing(kt_ctx* ctx, int on);
-/* Tracing of the fused pass: with tracing on, every CTA of the next kt_evaluate records {ticket, SM id, start, end,
- * then up to 12 stage stamps whose meaning depends on the tile's role -- see the tile functions in csrc/kt_kernels.cuh}
- * (global timer, ns), then 16 SM-cycle counts of the shared decide tile's steps; kt_get_trace copies up to cap rows of 32
- * uint64 and returns the row count (or a negative kt_status).  Tickets are handed out in role order: pending-match tiles,
- * reconcile tiles, finalize tiles, pending-decide tiles (roles[] reports the four tile counts; a pass whose match and reconcile
- * tiles fit the device at once has no finalize / decide CTAs of its own -- that work is drawn from a queue by the CTAs that have
- * finished their tile, and the rows of those CTAs carry the stamps of their first decide sub-tile).  Diagnostic only; off by default. */
+/* Tracing of the fused pass: with tracing on, every pending-match, reconcile and status tile of the next kt_evaluate records a
+ * row of 32 uint64: [0] ticket, [1] SM id, [2] start, [3] end, [4..15] up to 12 stage stamps whose meaning depends on the tile's
+ * role -- see the tile functions in csrc/kt_kernels.cuh -- (global timer, ns), [16..27] 12 SM-cycle counts of a shared decide
+ * sub-tile's steps, [28] the CTA that ran the tile, [29] that CTA's exit time.  Rows: pending-match tiles, reconcile tiles, then
+ * status tiles; roles[] = {match tiles, reconcile tiles, status tiles, CTAs launched}.  The CTAs draw tiles until none is left,
+ * then the status tiles and decide work from the same queue; a CTA's last match / reconcile row carries the stamps of its first
+ * decide sub-tile and its exit time.  kt_get_trace copies up to cap rows and returns the row count (or a negative kt_status).
+ * Diagnostic only; off by default. */
 int kt_enable_trace(kt_ctx* ctx, int on);
 int64_t kt_get_trace(kt_ctx* ctx, uint64_t* rows /*[cap][32]*/, int64_t cap, uint32_t roles[4]);
 /* Pinned host memory for zero-staging H2D/D2H (cudaHostAlloc / cudaFreeHost). */

@@ -173,8 +173,8 @@ class Engine:
         self._ck(self._L.kt_enable_trace(self._h, int(on)))
 
     def trace(self):
-        """(rows[n][32] = ticket, sm, start_ns, end_ns, 12 stage stamps (4.. per role, see kt_kernels.cuh), 16 cycle counts; roles[4] = tiles per role)
-        of the last fused pass."""
+        """(rows[n][32] = ticket, sm, start_ns, end_ns, 12 stage stamps (4.. per role, see kt_kernels.cuh), 12 cycle counts, CTA, CTA exit_ns;
+        roles[4] = match tiles, reconcile tiles, status tiles, CTAs launched) of the last fused pass: one row per match / reconcile / status tile."""
         roles = np.zeros(4, np.uint32)
         n = self._L.kt_get_trace(self._h, None, 0, roles.ctypes.data)
         rows = np.zeros((int(roles.sum()), 32), np.uint64)

@@ -146,9 +146,9 @@ struct kt_ctx {
   size_t part_stride = 0;  // bytes between the two halves
   unsigned part_parity = 0;  // half that holds the sums of the last reconcile
   DevBuf d_sync;   // PassSync counters of the fused pass (zero between launches)
-  DevBuf d_trace;  // optional per-CTA trace rows of the fused pass
+  DevBuf d_trace;  // optional trace rows of the fused pass, one per match / reconcile / status tile
   bool trace = false;
-  uint32_t trace_roles[4] = {0, 0, 0, 0};
+  uint32_t trace_roles[4] = {0, 0, 0, 0};  // match tiles, reconcile tiles, status tiles, CTAs launched
   PassSync* last_sync = nullptr;  // counters of the last fused pass: its error flag is checked when results are fetched
   bool fused = true;  // one-launch pass (k_pass) when the whole pass is asked for; three PDL-chained kernels otherwise
   DevBuf d_changed;  // device-side status diff: {count[2] u32 by pass parity, pad to 16 B, idx[M] i32, flag[M] u8}
@@ -454,6 +454,20 @@ cudaError_t launch_check(kt_ctx* c, const PodView& pv, const TableView& tb, cons
                 (const unsigned char*)c->d_pre.as<unsigned char>(), px, c->pods[KT_PODS_PENDING].bitmap.as<uint32_t>(),
                 c->d_codes.as<uint32_t>(), c->d_admit.as<unsigned char>(), sparse_view(c));
 }
+// Occupancy of k_pass compiled for THREADS resident threads per SM: CTAs the device holds at once.
+template <int TPC, int B, int RT, bool REG, int TILE, int THREADS>
+cudaError_t pass_capacity(kt_ctx* c, size_t smem, unsigned* capacity) {
+  int per_sm = 0;
+  cudaError_t e = cudaFuncSetAttribute((const void*)k_pass<TPC, B, RT, REG, TILE, THREADS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (e != cudaSuccess) return e;
+  e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_pass<TPC, B, RT, REG, TILE, THREADS>, TILE, smem);
+  *capacity = (unsigned)per_sm * (unsigned)c->sm_count;
+  return e;
+}
+// A pass whose first-phase tiles are more than this many rounds of the 512-thread grid runs the 768-thread build.  Measured on
+// either side (C4: 3.3 rounds, 46 us both ways; C5 and C2 x 10: 16 rounds, 178 against 167 us); where between 3.3 and 16 the two
+// cross has not been measured.
+constexpr unsigned kDeepRounds = 8;
 template <int TPC, int B, int RT, bool REG, int TILE>
 cudaError_t launch_pass(kt_ctx* c, const PassArgs& a0) {
   const int L = c->lim.label_slots, R = c->lim.n_resources;
@@ -464,26 +478,26 @@ cudaError_t launch_pass(kt_ctx* c, const PassArgs& a0) {
   a.n_rec = (unsigned)((a.run.n + TILE - 1) / TILE);
   a.n_fin = (unsigned)(((long long)a.tb.M * a.G + TILE - 1) / TILE);
   a.n_chk = (unsigned)((a.pend.n + TILE - 1) / TILE);
-  a.n_status = (a.n_fin + kStatusBatch - 1) / kStatusBatch;
-  // Does the whole grid fit on the device at once?  Then the match CTAs stay on as the decide tiles (k_pass, "resident").
-  int per_sm = 0;
-  cudaError_t e = cudaFuncSetAttribute((const void*)k_pass<TPC, B, RT, REG, TILE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  // Persistent grid: as many CTAs as the device holds at once (never more than there are first-phase tiles); each one draws
+  // tiles until the ticket counter runs out, so every CTA is placed at the start and the second phase is shared by all of them.
+  const unsigned tiles = a.n_chk + a.n_rec;
+  unsigned capacity = 0;
+  cudaError_t e = pass_capacity<TPC, B, RT, REG, TILE, kPassThreadsShallow>(c, smem, &capacity);
   if (e != cudaSuccess) return e;
-  e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_pass<TPC, B, RT, REG, TILE>, TILE, smem);
-  if (e != cudaSuccess) return e;
-  const unsigned capacity = (unsigned)per_sm * (unsigned)c->sm_count;
-  // (the status CTAs come last and are waited for by nobody on this GPU -- with peers only by decide tiles, after every
-  // reconcile tile has left -- so they do not count)
-  a.resident = (KT_PASS_RESIDENT != 0 && a.n_chk + a.n_rec <= capacity) ? 1u : 0u;
-  if (a.resident && KT_PASS_RESIDENT == 2) {
-    // shared second phase: the CTAs draw the decide sub-tiles and the status tiles from a ticket counter once their own tile
-    // is done; the grid is the match and reconcile tiles only
-    a.resident = 2u;
-    a.n_sub = (unsigned)((a.pend.n + TILE / 4 - 1) / (TILE / 4));
-    a.n_status = 0;
-  }
-  if (c->trace) { c->trace_roles[0] = a.n_chk; c->trace_roles[1] = a.n_rec; c->trace_roles[2] = a.n_status; c->trace_roles[3] = a.resident ? 0 : a.n_chk; }
-  return launch(c, k_pass<TPC, B, RT, REG, TILE>, (a.resident ? 1u : 2u) * a.n_chk + a.n_rec + a.n_status, TILE, smem, /*pdl=*/KT_PASS_PDL != 0, a);
+  const bool deep = tiles > kDeepRounds * capacity;
+  if (deep && (e = pass_capacity<TPC, B, RT, REG, TILE, kPassThreadsDeep>(c, smem, &capacity)) != cudaSuccess) return e;
+  const unsigned grid = tiles < capacity ? tiles : capacity;
+  // The decide work: four lanes per pod in sub-tiles of TILE/4 pods spread it over every CTA, but each sub-tile stages its own
+  // pre-records and finishes its own constants -- a latency chain of several L2 trips.  That pays while the sub-tiles take at
+  // most two rounds of the grid (C4: 625 sub-tiles on 528 CTAs, 46 us against 50 us); beyond that (C5: 3125 sub-tiles on 792 CTAs,
+  // 185 us against 167 us) the rounds queue up and lane-per-pod tiles of TILE pods do the same work in a quarter of the pieces.  The
+  // factor 2 lies between those two shapes (1.2 and 5.9 rounds); where between them the two cross has not been measured.
+  const unsigned n_quad = (unsigned)((a.pend.n + TILE / 4 - 1) / (TILE / 4));
+  a.quad = n_quad <= 2 * grid;
+  a.n_sub = a.quad ? n_quad : a.n_chk;
+  if (c->trace) { c->trace_roles[0] = a.n_chk; c->trace_roles[1] = a.n_rec; c->trace_roles[2] = a.n_fin; c->trace_roles[3] = grid; }
+  return deep ? launch(c, k_pass<TPC, B, RT, REG, TILE, kPassThreadsDeep>, grid, TILE, smem, /*pdl=*/KT_PASS_PDL != 0, a)
+              : launch(c, k_pass<TPC, B, RT, REG, TILE, kPassThreadsShallow>, grid, TILE, smem, /*pdl=*/KT_PASS_PDL != 0, a);
 }
 cudaError_t dispatch_pass(kt_ctx* c, const PassArgs& a) {
   const bool t1 = c->ht.TPpad == 1, b2 = c->ht.B <= 2;
@@ -611,7 +625,7 @@ int64_t kt_get_trace(kt_ctx* c, uint64_t* rows, int64_t cap, uint32_t roles[4]) 
   std::lock_guard<std::mutex> lk(c->mu);
   int rc = set_device(c);
   if (rc) return rc;
-  const int64_t total = (int64_t)c->trace_roles[0] + c->trace_roles[1] + c->trace_roles[2] + c->trace_roles[3];
+  const int64_t total = (int64_t)c->trace_roles[0] + c->trace_roles[1] + c->trace_roles[2];
   if (roles) std::memcpy(roles, c->trace_roles, sizeof c->trace_roles);
   if (!c->trace || !c->d_trace.p || total == 0) return 0;
   const int64_t n = total < cap ? total : cap;
@@ -1085,11 +1099,10 @@ static int evaluate_locked(kt_ctx* c, int64_t now, uint32_t flags) {
     a.n_fin = (unsigned)(((long long)M * G + kTileReconcile - 1) / kTileReconcile);
     a.n_chk = (unsigned)((pend.n + kTileReconcile - 1) / kTileReconcile);
     if (c->trace) {
-      const size_t rows = (size_t)2 * a.n_chk + a.n_rec + a.n_fin;  // (an upper bound of the grid: resident passes launch fewer CTAs)
+      const size_t rows = (size_t)a.n_chk + a.n_rec + a.n_fin;  // one per match, reconcile and status tile (at 128-row tiles: an upper bound for 256-row ones)
       KT_CUDA(c, c->d_trace.reserve(rows * kTraceRow * 8));
       KT_CUDA(c, cudaMemsetAsync(c->d_trace.p, 0, rows * kTraceRow * 8, c->stream));
       a.trace = c->d_trace.as<unsigned long long>();
-      c->trace_roles[0] = a.n_chk; c->trace_roles[1] = a.n_rec; c->trace_roles[2] = a.n_fin; c->trace_roles[3] = a.n_chk;  // (prep tiles are counted with the match tiles)
     }
     KT_CUDA(c, dispatch_pass(c, a));
     run.bitmap_clean = pend.bitmap_clean = true;  // zero-filled (if need be) and written by this pass: maintained from here on

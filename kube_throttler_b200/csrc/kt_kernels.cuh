@@ -16,11 +16,10 @@
 // shuffles so that one lane = one THROTTLE, which adds up its pods' requests from shared memory without
 // any atomics; warps meet in per-CTA shared-memory accumulators and only those reach HBM (RED.ADD.64).
 //
-// A whole pass is ONE launch, k_pass: every CTA draws a ticket and becomes a pending-match tile (which also writes the
-// per-throttle pre-records), a reconcile tile, a status tile or a pending-decide tile; hand-offs are counters in L2.  When every
-// match and reconcile tile fits the device at once, the status tiles and the decide work (sub-tiles of TILE/4 pods, four lanes
-// per pod, pre-records staged with cp.async.bulk on mbarriers) are a ticket queue served by every CTA that has finished its own
-// tile (check_decide_quad).  Partial passes, per-kernel timing and the NCCL fallback run the same tile functions as the three
+// A whole pass is ONE launch, k_pass: a grid no larger than the device holds at once, whose CTAs draw tickets from one counter
+// until none is left -- pending-match tiles (which also write the per-throttle pre-records), reconcile tiles, then the second
+// phase: status tiles and decide sub-tiles (TILE/4 pods, four lanes per pod, pre-records staged with cp.async.bulk on
+// mbarriers, check_decide_quad); hand-offs are counters in L2.  Partial passes, per-kernel timing and the NCCL fallback run the same tile functions as the three
 // kernels above, chained with programmatic dependent launch (griddepcontrol): k_check matches the pending pods while k_reconcile
 // is still summing, and only its 4-step compare waits for k_finalize.
 #pragma once
@@ -39,9 +38,11 @@ namespace kt {
 #ifndef KT_WAIT_MODE       // how a wait acquires: 0 relaxed polls + acquire fence, 1 relaxed polls + one acquire load, 2 acquire polls
 #define KT_WAIT_MODE 1
 #endif
-#ifndef KT_PASS_THREADS    // resident threads per SM the fused pass is compiled for (register cap = 65536 / this)
-#define KT_PASS_THREADS 768
-#endif
+// Resident threads per SM the fused pass is compiled for (register cap = 65536 / this).  Both are built; launch_pass picks one from
+// the shape: 512 (128 registers, no spills) for passes whose tiles are a few rounds of the grid, where the chain after the last
+// reconcile tile is the time; 768 (80 registers) for passes many rounds deep, whose reconcile tiles stream better with 24 warps
+// per SM than with 16 (C5).
+constexpr int kPassThreadsShallow = 512, kPassThreadsDeep = 768;
 #ifndef KT_SLOT_CAP        // upper bound on the per-CTA accumulator slots (shared memory vs straight-to-HBM atomics)
 #define KT_SLOT_CAP 32
 #endif
@@ -57,13 +58,14 @@ constexpr uint32_t kFull = 0xffffffffu;
 #endif
 constexpr int kStageChunk = KT_STAGE_CHUNK;  // resources whose pre-record values and sums a decide lane requests together
 #ifndef KT_EVAL_PAIR  // 1: a lane's first two words are evaluated with their table gathers interleaved (eval_word2).  Measured
-#define KT_EVAL_PAIR 0  // measured slower at the 80-register cap of a resident pass (spills) -- off
+#define KT_EVAL_PAIR 0  // measured slower at the 80-register cap of the fused pass at 768 threads per SM (spills) -- off
 #endif
 #ifndef KT_DECIDE_UNROLLED
 #define KT_DECIDE_UNROLLED 0
 #endif
 constexpr int kPropose = 4;          // words a warp of a decide tile may propose to its CTA's staging table per round
-constexpr int kTraceRow = 32;        // u64 per CTA of the optional in-kernel trace: {ticket, sm, t_start, t_end, 12 stage stamps (globaltimer ns), 16 cycle counts}
+constexpr int kTraceRow = 32;        // u64 per traced tile of the optional in-kernel trace: {ticket, sm, t_start, t_end, 12 stage stamps (globaltimer ns),
+                                     // 12 cycle counts, CTA, CTA exit}
 
 // Word info of a pod row (k_translate_rows; valid for the tables it was computed with): the words whose namespace mask is
 // non-zero for the pod's namespace are the only ones the pod can match anything in.  Namespace-scoped Throttles give 1-3 of
@@ -200,20 +202,21 @@ __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepc
 __device__ __forceinline__ void pdl_wait_primary() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
 // ---- in-kernel hand-off between the roles of the fused pass (k_pass) ----------------------------------
-// Tiles are handed out by a ticket counter, reconcile tiles first, then finalize, then check tiles: a CTA that
-// waits on a counter can only be waiting for tiles with SMALLER tickets, which are already running on some SM,
-// so the waits cannot deadlock whatever the residency.  Signals are fence + relaxed add (release pattern) by
-// thread 0 after a CTA barrier; waits are relaxed polls + one acquire fence by thread 0 followed by a CTA barrier.
+// Work is handed out by ONE ticket counter: pending-match tiles, reconcile tiles, then the second phase (status tiles and
+// decide sub-tiles).  First-phase tiles never wait.  A second-phase piece waits only for pieces with smaller tickets, which
+// running CTAs have already drawn (a CTA draws its next ticket only once its previous piece is done), or for other GPUs,
+// whose pieces follow the same order -- so the waits cannot deadlock whatever the residency, and correctness does not depend
+// on the grid fitting the device (k_pass sizes it to the device for speed only).  Signals are fence + relaxed add (release
+// pattern) by thread 0 after a CTA barrier; waits are relaxed polls + one acquire by thread 0 followed by a CTA barrier.
 struct PassSync {
   // counters of ONE pass, re-armed by its last CTA (everything before `error`)
-  unsigned ticket;      // next tile
+  unsigned ticket;      // next piece of work
   unsigned rec_done;    // reconcile tiles finished (their REDs are performed at L2)
   unsigned prep_done;   // finalize tiles that have written their throttles' pre-records (nothing to wait for: early)
   unsigned match_done;  // pending-match tiles finished (affectedThrottles rows written)
   unsigned tot_done;    // multi-GPU: finalize tiles of this rank that have written the all-rank totals of their throttles
   unsigned exited;      // CTAs that are done with everything; the last one re-arms the counters
-  unsigned dec_ticket;  // resident pass: next piece of the shared second phase (decide sub-tiles, status tiles)
-  unsigned spare;
+  unsigned spare[2];    // unused: `error` stays at index kPassSyncRearm
   unsigned error;       // a wait gave up (kSpinTimeoutNs): a peer never arrived; the host reports it, the results are void
   unsigned pad[3];
 };
@@ -355,16 +358,13 @@ struct PdlSync {
 struct FlagSync {
   PassSync* s;
   unsigned n_rec, n_fin, n_match;
-  bool own_rows;  // resident pass: a decide tile reads the match rows its own CTA wrote (a CTA barrier orders them)
   __device__ __forceinline__ void wait_reconciled() const { cta_wait_at_least(&s->rec_done, n_rec, &s->error); }
   // the sums of every rank are in px.total
   __device__ __forceinline__ void wait_totals(const PartExchange& px) const {
     if (px.npeers == 0) wait_reconciled();
     else cta_wait_at_least(&s->tot_done, n_fin, &s->error);
   }
-  __device__ __forceinline__ void wait_matched() const {
-    if (!own_rows) cta_wait_at_least(&s->match_done, n_match, &s->error);
-  }
+  __device__ __forceinline__ void wait_matched() const { cta_wait_at_least(&s->match_done, n_match, &s->error); }
   __device__ __forceinline__ void wait_prepped() const { cta_wait_at_least(&s->prep_done, n_fin, &s->error); }
   __device__ __forceinline__ void signal_prepped() const { cta_signal(&s->prep_done); }
   __device__ __forceinline__ void signal_totals() const { cta_signal(&s->tot_done); }
@@ -668,9 +668,6 @@ __device__ __forceinline__ unsigned long long warp_sum_u64(unsigned long long v)
 #ifndef KT_SMEM_ADD32  // 1: 64-bit shared-memory accumulator adds as two native 32-bit atomics with a carry; 0: atomicAdd(u64) (a CAS loop)
 #define KT_SMEM_ADD32 1
 #endif
-#ifndef KT_PASS_RESIDENT  // 1: a pass whose whole grid fits the device keeps its match CTAs on as decide tiles; 2: ... and every CTA that
-#define KT_PASS_RESIDENT 2  // has finished its own tile shares the decide work (check_decide_quad)
-#endif
 __device__ __forceinline__ uint32_t smem_addr(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(unsigned long long* bar, unsigned count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_addr(bar)), "r"(count) : "memory");
@@ -744,7 +741,8 @@ template <int TPC, int B, int RT, bool REG, int TILE = kTileReconcile>
 __device__ __forceinline__ void reconcile_tile(const PodView& pods, const TableView& tb, int L, int R, int S, uint32_t* __restrict__ bitmap,
                                                unsigned long long* __restrict__ part /* [2R+1][M]: used, present, cnt */,
                                                unsigned char* smem_raw, int64_t tile_index, unsigned long long* trace_row = nullptr,
-                                               unsigned long long* row_bar = nullptr /* fresh transaction barrier (count 1, phase 0): stage the rows in bulk */) {
+                                               unsigned long long* row_bar = nullptr /* transaction barrier (count 1): stage the rows in bulk */,
+                                               unsigned* row_parity = nullptr /* with row_bar: its phase parity, advanced by every bulk-staged tile */) {
   // optional stage stamps of warp 0 (kt_enable_trace): [4] the pod rows have landed, [5] first two words evaluated, [6] barrier
   // passed, [7] words + sums done, [8] sweep done
   auto stamp = [&](int k) {
@@ -824,7 +822,8 @@ __device__ __forceinline__ void reconcile_tile(const PodView& pods, const TableV
   }
   if constexpr (KT_BULK_ROWS != 0 && REG && RT > 0) {
     if (bulk) {  // the slices have landed: the lane's own row out of shared memory
-      mbar_wait(row_bar, 0u);
+      mbar_wait(row_bar, *row_parity);
+      *row_parity ^= 1u;
       winfo = s_stage[8 * TILE + tid];
       flags = s_stage[9 * TILE + tid];
       ns = (int)s_stage[10 * TILE + tid];
@@ -1077,7 +1076,6 @@ struct __align__(16) PreHdr {
 constexpr uint32_t kPreLive = 1u, kPreE3 = 2u, kPreOnEqual = 4u, kPreGiven = 8u;
 __host__ __device__ inline size_t pre_record_bytes(int R) { return 16 + 16 * (size_t)R + 16; }
 
-constexpr unsigned kStatusBatch = 1;  // finalize tiles (status halves) per status CTA
 constexpr int kFinPrep = 1, kFinStatus = 2;  // the halves of a finalize tile: the fused pass runs them as separate tiles (prep first, so
                                              // that nobody ever waits for pre-records), the chained k_finalize runs both
 template <class Sync>
@@ -1773,10 +1771,9 @@ __device__ __forceinline__ void check_decide_tile(const PodView& pods, const Tab
 
 
 // ------------------------------------------------------------------------------------------------
-// The SHARED decide tiles of a resident pass.  When every match and reconcile CTA of the grid is on the device at once, the
-// decide work is not left to the P/TILE CTAs that matched the pending pods (one lane per pod walking its words and pairs one
-// after the other while every other SM has gone idle): every CTA that has finished its own tile --
-// match or reconcile -- draws sub-tiles of TILE/4 pending pods from a second ticket counter.  FOUR lanes per pod: lane q
+// The SHARED decide tiles of the fused pass.  The decide work is not left to P/TILE CTAs with one lane per pod (walking its
+// words and pairs one after the other while every other SM has gone idle): every CTA of k_pass that has run out of match and
+// reconcile tiles draws sub-tiles of TILE/4 pending pods from the same ticket counter.  FOUR lanes per pod: lane q
 // fetches the pod's q-th word of the round and claims its staging slot (same-word lanes of a warp elect one claimant; a word
 // that finds no slot -- rows in arrival order -- is checked pair by pair straight from L2), and the pod's pairs are dealt out
 // to its four lanes bit by bit.  Everything before the wait for the sums -- requests, match words, slot claims, the
@@ -2026,11 +2023,12 @@ __global__ void __launch_bounds__(kTileCheck) k_check(PodView pods, TableView tb
 }
 
 // ------------------------------------------------------------------------------------------------
-// k_pass: the whole pass in ONE launch.  Every CTA draws a ticket and becomes a reconcile tile, a finalize
-// tile or a check tile (in that ticket order).  Check tiles match their pending pods while the reconcile
-// tiles are still summing; finalize tiles load thresholds / overrides meanwhile and, with peers, perform the
-// all-reduce themselves by pulling the other ranks' partial sums over NVLink.  One cold start instead of
-// three, and the hand-offs cost a poll of an L2 counter instead of a kernel boundary.
+// k_pass: the whole pass in ONE launch of at most as many CTAs as the device holds at once.  Every CTA draws tickets
+// until none is left: match tiles (which also write the pre-records), reconcile tiles, then the second phase -- status
+// tiles (with peers they perform the all-reduce over NVLink) and decide sub-tiles.  Match tiles hold the first tickets,
+// so the pending pods are matched while the reconcile tiles are still summing, and the CTAs that finish those cheap
+// tiles first take the reconcile tiles that did not fit the first wave.  One cold start instead of three, and the
+// hand-offs cost a poll of an L2 counter instead of a kernel boundary.
 // ------------------------------------------------------------------------------------------------
 struct PassArgs {
   PodView run, pend;
@@ -2048,16 +2046,16 @@ struct PassArgs {
   long long now;
   uint32_t eval_flags;
   int L, R, S, G;
-  unsigned n_chk, n_rec, n_fin;  // tiles per role; tickets: [match (+ prep) n_chk][reconcile n_rec][status n_status][decide n_chk]; a tile only
-                                 // ever waits for SMALLER tickets (status: reconcile; decide: match + prep, reconcile -- with peers the status
-                                 // tiles' totals) or for other GPUs, whose tiles are subject to the same order -- unless the whole grid is
-                                 // resident (below)
-  unsigned n_status;             // CTAs that run the status halves: ceil(n_fin / kStatusBatch)
-  unsigned resident;             // 1: every match and reconcile CTA of the grid is on the device at once; the match CTAs stay on as the decide
-                                 // tiles; 2: ... and every CTA that is through with its own tile shares the decide work (check_decide_quad)
-  unsigned n_sub;                // resident == 2: shared decide sub-tiles of TILE/4 pending pods (the grid has no status CTAs: n_status == 0,
-                                 // the n_fin status tiles are drawn from the same ticket counter as the sub-tiles)
-  unsigned long long* trace;     // optional (kt_enable_trace): per CTA kTraceRow x u64 {ticket, sm, t_start, t_end, stage stamps} in globaltimer ns
+  unsigned quad;                 // 1: decide sub-tiles of TILE/4 pending pods, four lanes per pod (check_decide_quad); 0: decide tiles of
+                                 // TILE pods, one lane per pod (check_decide_tile) -- the host picks (launch_pass)
+  unsigned n_chk, n_rec, n_fin;  // tiles per role; tickets: [match (+ prep) n_chk][reconcile n_rec][second phase: n_fin status tiles and n_sub
+  unsigned n_sub;                // decide (sub-)tiles -- status first with peers (they carry the exchange the decide
+                                 // sub-tiles wait for), last alone (nobody waits for them)]; a piece only ever waits for SMALLER tickets
+                                 // (status: reconcile; decide: match + prep, reconcile -- with peers the status tiles' totals) or for other
+                                 // GPUs, whose pieces are subject to the same order (PassSync)
+  unsigned long long* trace;     // optional (kt_enable_trace): per first-phase ticket, then per status tile, kTraceRow x u64 {ticket, sm, t_start,
+                                 // t_end, stage stamps} in globaltimer ns, [28] the CTA that ran it; a CTA's last first-phase tile also
+                                 // carries its first decide sub-tile's stamps and [29] the time the CTA exited
 };
 __device__ __forceinline__ unsigned long long globaltimer_ns() {
   unsigned long long t;
@@ -2067,120 +2065,96 @@ __device__ __forceinline__ unsigned long long globaltimer_ns() {
 
 // TILE: pods per CTA (= threads).  128 everywhere except ClusterThrottle-heavy tables, where every pod walks a dozen words and a
 // CTA's accumulator slots (one per word, 2 KB each at R = 8) are better shared by twice the pods (measured faster at C3).
-template <int TPC, int B, int RT, bool REG, int TILE = kTileReconcile>
-__global__ void __launch_bounds__(TILE, KT_PASS_THREADS / TILE) k_pass(const __grid_constant__ PassArgs a) {
+template <int TPC, int B, int RT, bool REG, int TILE, int THREADS>
+__global__ void __launch_bounds__(TILE, THREADS / TILE) k_pass(const __grid_constant__ PassArgs a) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
-  __shared__ unsigned s_ticket, s_sub;
+  __shared__ unsigned s_ticket;
+  __shared__ unsigned s_last;                 // trace: this CTA's last first-phase ticket (~0u: none yet)
+  __shared__ unsigned long long s_t_start;    // trace: when the current tile began
   __shared__ __align__(8) unsigned long long s_mbar[kMaxWarps + 1];  // transaction barriers: one per warp (bulk copies of the shared decide tiles), [kMaxWarps] the reconcile tile's rows
-  unsigned long long t_start = 0;
   // Launched with programmatic stream serialization: the NEXT launch in the stream (normally the next pass) may have its CTAs
   // placed while this one still runs -- they sit in the wait below until this grid has completed and flushed, so nothing of
-  // theirs (tickets, counters, sums) can mix with ours; what overlaps is their launch latency.  Every CTA releases the
-  // dependents at once: a grid whose CTAs are not all resident yet cannot be overtaken (the dependents only start when ALL
-  // our CTAs have started), so the tiles we still owe always find an SM.
+  // theirs (tickets, counters, sums) can mix with ours; what overlaps is their launch latency.
   pdl_launch_dependents();
   if (threadIdx.x == 0) {
 #pragma unroll
     for (int i = 0; i < kMaxWarps + 1; ++i) mbar_init(&s_mbar[i], 1u);
     mbar_init_fence();
+    s_last = ~0u;
   }
   pdl_wait_primary();
-  if (threadIdx.x == 0) {
-    s_ticket = atomicAdd(&a.sync->ticket, 1u);
-    if (a.trace) t_start = globaltimer_ns();
-  }
-  __syncthreads();
-  unsigned tile = s_ticket;
-  const FlagSync sync{a.sync, a.n_rec, a.n_fin, a.n_chk, a.resident == 1};
-  unsigned long long* trow = a.trace ? a.trace + (size_t)s_ticket * kTraceRow : nullptr;
-  bool shares_decide = false;  // resident == 2: this CTA goes on to the shared second phase once its own tile is done
-  int own_status = -1;         // a status CTA's tile (passes that are not resident)
-  if (tile < a.n_chk) {  // no dependencies: first tickets
-    // The match tiles also write the pre-records (the prep half of the finalize tiles, spread over them): they hold the first
-    // tickets, so every pre-record exists a few microseconds into the pass and no decide tile ever waits for one -- without
-    // extra CTAs pushing reconcile tiles out of the first wave.
-    for (unsigned ft = tile; ft < a.n_fin; ft += a.n_chk)
-      finalize_tile(a.tv, a.tb.M, a.R, a.G, a.now, a.eval_flags, a.px, a.out, a.pre, (int)ft, sync, nullptr, kFinPrep);
-    // the first match tile also clears the sparse list's counter: every decide tile waits for ALL match tiles before it appends
-    if (tile == 0 && threadIdx.x == 0 && a.sparse.count) *a.sparse.count = 0u;
-    check_match_tile<TPC, B, REG, TILE>(a.pend, a.tb, a.L, a.pend_bitmap, a.codes, smem_raw, tile);
-    cta_signal(&a.sync->match_done);
-    if (KT_PASS_RESIDENT == 1 && a.resident == 1) {
-      // RESIDENT pass (the host found that every CTA of the grid fits on the device at once): the CTA stays and becomes the decide
-      // tile of the same 128 pods -- already placed, its pre-wait work done long before the reconcile tiles finish, instead of a
-      // late CTA that is only launched when somebody else exits.  (It waits for LARGER tickets, which is only safe because all
-      // of them are resident; a grid that does not fit keeps the decide tiles behind the reconcile tiles.)
-      __syncthreads();
-      check_decide_tile<TILE, RT>(a.pend, a.tb, a.R, decide_stage_words(a.R, TILE), a.pre, a.px, a.pend_bitmap, a.codes, a.admit, smem_raw, tile, sync,
-                                        a.sparse, trow);
+  const unsigned n_tiles = a.n_chk + a.n_rec;
+  auto draw = [&]() -> unsigned {
+    __syncthreads();  // everybody has read the previous ticket, and the CTA's shared memory is free again
+    if (threadIdx.x == 0) s_ticket = atomicAdd(&a.sync->ticket, 1u);
+    __syncthreads();
+    return s_ticket;
+  };
+  // (the trace bookkeeping lives in shared memory: nothing of it stays in registers across a tile, which runs at the register cap)
+  auto trace_row = [&](unsigned t) -> unsigned long long* { return a.trace && t != ~0u ? a.trace + (size_t)t * kTraceRow : nullptr; };
+  auto close_row = [&](unsigned long long* row) {  // thread 0, at the end of a traced tile
+    unsigned smid;
+    asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
+    row[0] = s_ticket; row[1] = smid; row[2] = s_t_start; row[3] = globaltimer_ns(); row[28] = blockIdx.x;
+  };
+  unsigned row_parity = 0;  // of s_mbar[kMaxWarps], across this CTA's reconcile tiles
+  unsigned ticket;
+  // ---- first phase: match and reconcile tiles, none of which waits for anything ----
+  while ((ticket = draw()) < n_tiles) {
+    if (a.trace && threadIdx.x == 0) s_t_start = globaltimer_ns();
+    if (ticket < a.n_chk) {
+      const FlagSync sync{a.sync, a.n_rec, a.n_fin, a.n_chk};
+      // The match tiles also write the pre-records (the prep half of the finalize tiles, spread over them): they hold the first
+      // tickets, so every pre-record exists a few microseconds into the pass and no decide sub-tile ever waits for one.
+      for (unsigned ft = ticket; ft < a.n_fin; ft += a.n_chk)
+        finalize_tile(a.tv, a.tb.M, a.R, a.G, a.now, a.eval_flags, a.px, a.out, a.pre, (int)ft, sync, nullptr, kFinPrep);
+      // the first match tile also clears the sparse list's counter: every decide sub-tile waits for ALL match tiles before it appends
+      if (ticket == 0 && threadIdx.x == 0 && a.sparse.count) *a.sparse.count = 0u;
+      check_match_tile<TPC, B, REG, TILE>(a.pend, a.tb, a.L, a.pend_bitmap, a.codes, smem_raw, ticket);
+      cta_signal(&a.sync->match_done);
+    } else {
+      reconcile_tile<TPC, B, RT, REG, TILE>(a.run, a.tb, a.L, a.R, a.S, a.run_bitmap, a.px.mine, smem_raw, ticket - a.n_chk, trace_row(ticket),
+                                            &s_mbar[kMaxWarps], &row_parity);
+      cta_signal(&a.sync->rec_done);
     }
-    shares_decide = KT_PASS_RESIDENT == 2 && a.resident == 2;
-  } else if ((tile -= a.n_chk) < a.n_rec) {
-    reconcile_tile<TPC, B, RT, REG, TILE>(a.run, a.tb, a.L, a.R, a.S, a.run_bitmap, a.px.mine, smem_raw, tile, trow, &s_mbar[kMaxWarps]);
-    cta_signal(&a.sync->rec_done);
-    shares_decide = KT_PASS_RESIDENT == 2 && a.resident == 2;
-  } else if ((tile -= a.n_rec) < a.n_status) {
-    // status tiles of a pass whose grid does not fit the device (off the critical path; nobody on this GPU waits for them, so
-    // they need not be resident from the start: they take the slots the reconcile tiles leave, which is when their work begins
-    // anyway).  Run below, by the one copy of the status code that the shared second phase uses as well.
-    own_status = (int)tile;
-  } else {
-    check_decide_tile<TILE, RT>(a.pend, a.tb, a.R, decide_stage_words(a.R, TILE), a.pre, a.px, a.pend_bitmap, a.codes, a.admit, smem_raw, tile - a.n_status, sync,
-                                      a.sparse, trow);
+    if (a.trace && threadIdx.x == 0) {  // (s_ticket is still this tile's: the next draw begins with a CTA barrier)
+      close_row(trace_row(s_ticket));
+      s_last = s_ticket;
+    }
   }
-  if ((KT_PASS_RESIDENT == 2 && shares_decide) || own_status >= 0) {
-    // RESIDENT pass, shared second phase: every match and reconcile CTA is on the device at once (the host checked), so a CTA
-    // that is through with its own tile may wait for ALL of them.  It draws work from a second ticket counter until none is
-    // left: the decide sub-tiles and the status tiles (the grid of such a pass has no status CTAs of its own).  With peers the
-    // status tiles come first -- they carry the exchange the decide tiles wait for; alone they come last, nobody waits for them.
-    unsigned mbar_phase = 0;
-    bool first = true;
-    const unsigned n_work = a.n_sub + a.n_fin;
-    while (true) {
-      bool is_status;
-      unsigned index;
-      if (own_status >= 0) {  // a status CTA: its one tile
-        is_status = true;
-        index = (unsigned)own_status;
-      } else {
-        __syncthreads();  // the CTA's shared memory is free again (previous role / previous piece of work)
-        if (threadIdx.x == 0) s_sub = atomicAdd(&a.sync->dec_ticket, 1u);
-        __syncthreads();
-        const unsigned work = s_sub;
-        if (work >= n_work) break;
-        const bool status_first = a.px.npeers > 0;
-        is_status = status_first ? work < a.n_fin : work >= a.n_sub;
-        index = status_first ? (is_status ? work : work - a.n_fin) : (is_status ? work - a.n_sub : work);
-      }
-      if (is_status) {
-        finalize_tile(a.tv, a.tb.M, a.R, a.G, a.now, a.eval_flags, a.px, a.out, a.pre, (int)index, sync, own_status >= 0 ? trow : nullptr, kFinStatus);
-        if (own_status >= 0) break;
-      } else {
-        if constexpr (KT_PASS_RESIDENT == 2)
-          check_decide_quad<TILE, RT>(a.pend, a.tb, a.R, decide_stage_words(a.R, TILE), a.pre, a.px, a.pend_bitmap, a.codes, a.admit, smem_raw, index, sync,
-                                      a.sparse, s_mbar, mbar_phase, first ? trow : nullptr);
-        first = false;
-      }
+  // ---- second phase: status tiles and decide sub-tiles, until the counter runs past them ----
+  unsigned mbar_phase = 0;
+  bool first = true;
+  const unsigned n_work = a.n_fin + a.n_sub;
+  const bool status_first = a.px.npeers > 0;
+  for (unsigned work = ticket - n_tiles; work < n_work; work = draw() - n_tiles) {
+    const bool is_status = status_first ? work < a.n_fin : work >= a.n_sub;
+    const unsigned index = status_first ? (is_status ? work : work - a.n_fin) : (is_status ? work - a.n_sub : work);
+    const FlagSync sync{a.sync, a.n_rec, a.n_fin, a.n_chk};
+    if (is_status) {  // traced as row n_tiles + index (after the first-phase tickets' rows)
+      unsigned long long* trow = trace_row(n_tiles + index);
+      if (trow && threadIdx.x == 0) s_t_start = globaltimer_ns();
+      finalize_tile(a.tv, a.tb.M, a.R, a.G, a.now, a.eval_flags, a.px, a.out, a.pre, (int)index, sync, trow, kFinStatus);
+      if (trow && threadIdx.x == 0) close_row(trow);
+    } else if (a.quad) {
+      check_decide_quad<TILE, RT>(a.pend, a.tb, a.R, decide_stage_words(a.R, TILE), a.pre, a.px, a.pend_bitmap, a.codes, a.admit, smem_raw, index, sync,
+                                  a.sparse, s_mbar, mbar_phase, first ? trace_row(s_last) : nullptr);
+      first = false;
+    } else {  // (no trace stamps: they would land on the reconcile tile's)
+      check_decide_tile<TILE, RT>(a.pend, a.tb, a.R, decide_stage_words(a.R, TILE), a.pre, a.px, a.pend_bitmap, a.codes, a.admit, smem_raw, index, sync,
+                                  a.sparse);
     }
   }
   // the last CTA out re-arms the counters for the next launch (stream-ordered after this one)
   __syncthreads();
   if (threadIdx.x == 0) {
-    if (a.trace) {
-      unsigned smid;
-      asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
-      unsigned long long* row = a.trace + (size_t)s_ticket * kTraceRow;
-      row[0] = s_ticket; row[1] = smid; row[2] = t_start; row[3] = globaltimer_ns();
-    }
-    const unsigned total = (a.resident ? 1u : 2u) * a.n_chk + a.n_rec + a.n_status;
-    if (atomicAdd(&a.sync->exited, 1u) == total - 1) {
+    if (unsigned long long* row = trace_row(s_last)) row[29] = globaltimer_ns();
+    if (atomicAdd(&a.sync->exited, 1u) == gridDim.x - 1) {
       a.sync->ticket = 0;
       a.sync->rec_done = 0;
       a.sync->prep_done = 0;
       a.sync->match_done = 0;
       a.sync->tot_done = 0;
-      a.sync->dec_ticket = 0;
-      a.sync->spare = 0;
       a.sync->exited = 0;
     }
   }

@@ -1,5 +1,6 @@
-"""Per-role timeline of the fused pass (k_pass) from the in-kernel trace: when each role's tiles start and end relative to
-the first CTA, the stage stamps of every role (median / p90 / max since pass start) and the slowest tiles of each role.
+"""Per-role timeline of the fused pass (k_pass) from the in-kernel trace: the grid and how many tiles its CTAs ran, when each
+role's tiles start and end relative to the first CTA, the stage stamps of every role (median / p90 / max since pass start),
+the shared decide sub-tiles and the slowest tiles of each role.
 python tools/pass_trace.py [C2] [sorted|unsorted]"""
 import os
 import sys
@@ -22,10 +23,9 @@ s = torch.cuda.Stream()
 eng.set_stream(s.cuda_stream)
 eng.enable_trace(True)
 STAGES = {
-    "match": ["(resident: decide) rows seen", "words + pre staged", "sums seen", "constants done", "decided"],
+    "match": [],
     "reconcile": ["rows landed", "2 words evaluated", "barrier", "words+sums", "sweep"],
-    "finalize": ["pre-records", "reconcile seen", "sums read", "status written"],
-    "decide": ["match rows seen", "words + pre staged", "sums seen", "constants done", "decided"],
+    "status": ["-", "reconcile seen", "sums read", "status written"],
 }
 for it in range(4):
     with torch.cuda.stream(s):
@@ -37,23 +37,35 @@ for it in range(4):
     rows, roles = eng.trace()
     rows = rows.astype(np.float64)
     t0 = rows[:, 2].min()
+    grid = int(roles[3])
+    cta = rows[:, 28].astype(np.int64)
+    per_cta = np.bincount(cta, minlength=grid)
+    exit_ = rows[rows[:, 29] > 0, 29]
+    span = max(rows[:, 3].max(), exit_.max() if len(exit_) else 0.0)
+    print(f"pass {it} ({'cold' if it >= 2 else 'warm'} L2): span {(span - t0) / 1e3:.1f} us, {len(rows)} tiles on {grid} CTAs on {len(set(rows[:, 1]))} SMs; "
+          f"tiles per CTA: " + ", ".join(f"{k}: {int((per_cta == k).sum())} CTAs" for k in range(int(per_cta.max()) + 1) if (per_cta == k).any()))
+    if len(exit_):
+        print(f"  CTA exit  since pass start: med {np.median(exit_ - t0) / 1e3:5.1f}  p90 {np.percentile(exit_ - t0, 90) / 1e3:5.1f}  max {(exit_.max() - t0) / 1e3:5.1f}")
     lo = 0
-    print(f"pass {it} ({'cold' if it >= 2 else 'warm'} L2): span {(rows[:, 3].max() - t0) / 1e3:.1f} us, {len(rows)} CTAs on {len(set(rows[:, 1]))} SMs")
-    for name, n in zip(STAGES, roles):
+    for name, n in zip(STAGES, roles[:3]):
         r = rows[lo:lo + int(n)]
+        tickets = np.arange(lo, lo + int(n))
         lo += int(n)
         if not len(r):
             continue
         st, en = (r[:, 2] - t0) / 1e3, (r[:, 3] - t0) / 1e3
         print(f"  {name:9s} n={int(n):4d}  start {st.min():5.1f}..{st.max():5.1f}  end med {np.median(en):5.1f} p90 {np.percentile(en, 90):5.1f} max {en.max():5.1f}  dur med {np.median(en - st):5.1f}")
+        late = (tickets >= grid) & (name != "status")  # tiles drawn after the first wave: by CTAs that finished an earlier tile
+        if late.any():
+            print(f"            {int(late.sum())} tiles in the leftover round: start {st[late].min():5.1f}..{st[late].max():5.1f}  end max {en[late].max():5.1f}")
         for k, label in enumerate(STAGES[name]):
             x = (r[:, 4 + k] - t0) / 1e3
             x = x[r[:, 4 + k] > 0]
             if len(x):
                 print(f"            {label:18s} since pass start: med {np.median(x):5.1f}  p90 {np.percentile(x, 90):5.1f}  max {x.max():5.1f}")
-        if name in ("match", "reconcile") and (r[:, 9] > 0).any():  # shared decide tiles (resident pass): the CTA's first sub-tile
+        if (r[:, 9] > 0).any():  # a CTA's last tile carries the stamps of its first shared decide sub-tile
             sel = r[:, 9] > 0
-            print(f"            -> {int(sel.sum())} of these CTAs went on to shared decide sub-tiles")
+            print(f"            -> {int(sel.sum())} CTAs whose last tile was one of these went on to shared decide sub-tiles")
             for k, label in enumerate(["rows + pre visible", "slots claimed", "sums seen", "constants done", "decided"]):
                 x = (r[sel, 9 + k] - t0) / 1e3
                 x = x[r[sel, 9 + k] > 0]
@@ -79,5 +91,5 @@ for it in range(4):
             worst = np.argsort(-en)[:4]
             for i in worst:
                 stamps = " ".join(f"{(r[i, 4 + k] - t0) / 1e3:5.1f}" if r[i, 4 + k] > 0 else "    -" for k in range(len(STAGES[name])))
-                print(f"            slowest: tile {i:4d} sm {int(r[i, 1]):3d} start {st[i]:5.1f} end {en[i]:5.1f} | {stamps}")
+                print(f"            slowest: tile {i:4d} sm {int(r[i, 1]):3d} cta {int(r[i, 28]):4d} start {st[i]:5.1f} end {en[i]:5.1f} | {stamps}")
 eng.close()

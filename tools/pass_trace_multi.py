@@ -31,10 +31,12 @@ for it in range(5):
         continue
     t0 = rows[:, 2].min()
     nm, nr, nf = int(roles[0]), int(roles[1]), int(roles[2])
-    rec, fin, dec = rows[nm:nm + nr], rows[nm + nr:nm + nr + nf], rows[nm + nr + nf:]
+    rec, fin = rows[nm:nm + nr], rows[nm + nr:nm + nr + nf]
+    dec = rows[:nm + nr][rows[:nm + nr, 9] > 0]  # a CTA's last match / reconcile row carries its first decide sub-tile's stamps
     us = lambda a: (a.astype(np.float64) - float(t0)) / 1e3
-    print(f"[rank {rank}] pass {it}: launches {eng.timing().launches} span {us(rows[:,3]).max():.1f} us | reconcile end max {us(rec[:,3]).max():.1f} | finalize: pre-records {np.median(us(fin[:,4])):.1f}, "
-          f"own reconcile seen {np.median(us(fin[:,5])):.1f} (max {us(fin[:,5]).max():.1f}), totals of all ranks read {np.median(us(fin[:,6])):.1f} (max {us(fin[:,6]).max():.1f}), done {us(fin[:,3]).max():.1f} | "
-          f"decide: words+pre staged {np.median(us(dec[:,5])):.1f}, sums seen {np.median(us(dec[:,6])):.1f} (max {us(dec[:,6]).max():.1f}), decided {np.median(us(dec[:,8])):.1f}, end max {us(dec[:,3]).max():.1f}", flush=True)
+    med = lambda a: f"{np.median(a):.1f} (max {a.max():.1f})" if len(a) else "-"
+    print(f"[rank {rank}] pass {it}: launches {eng.timing().launches} span {max(us(rows[:, 3]).max(), us(rows[:, 29]).max()):.1f} us on {int(roles[3])} CTAs | "
+          f"reconcile end max {us(rec[:, 3]).max():.1f} | status: own reconcile seen {med(us(fin[:, 5]))}, totals of all ranks read {med(us(fin[:, 6]))}, "
+          f"done {med(us(fin[:, 3]))} | first decide sub-tiles: sums of all ranks seen {med(us(dec[:, 11]))}, decided {med(us(dec[:, 13]))}", flush=True)
 eng.close()
 dist.destroy_process_group()

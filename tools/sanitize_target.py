@@ -1,11 +1,13 @@
 """Small passes through every device path for compute-sanitizer (memcheck / racecheck / synccheck), checked against nothing:
 the tool is the check.
   compute-sanitizer --tool racecheck python tools/sanitize_target.py
-Paths: fused pass (resident: the whole grid fits) and chained kernels (per-kernel timing), fast family (L <= 8) with 128- and
+Paths: fused pass (persistent grid; shared second phase) and chained kernels (per-kernel timing), fast family (L <= 8) with 128- and
 256-row tiles (a ClusterThrottle-heavy table has long per-namespace word lists), general family (L = 12, 6-bit counters), ragged
 R = 1; wide / compact / packed uploads (packed: the fused unpack + translate kernel), row deltas, the one-call step with the
 sparse check result, observed status + the device-side status diff + row getters, GIVEN_STATUS passes, queue admission rounds.
-KT_SANITIZE_BIG=1 adds a 120k-row snapshot whose grid is NOT resident at once (separate decide tiles)."""
+KT_SANITIZE_BIG=1 adds two 120k-row snapshots with more tiles than the device holds CTAs at once, so that CTAs run several tiles
+one after the other in the same shared memory: 4k pending pods (four-lane decide sub-tiles) and 40k (more sub-tiles than two
+rounds of the grid: lane-per-pod decide tiles after reconcile tiles)."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
@@ -14,10 +16,10 @@ from kube_throttler_b200 import abi, synth
 
 cases = [("C3", dict(m=300, n=3000, p=500)), ("C3", dict(m=900, n=2500, p=400)), ("C2", dict(m=200, n=2000, p=300, L=12, q_max=6)),
          ("C2", dict(m=40, n=70, p=33, R=1))]
-if os.environ.get("KT_SANITIZE_SMALL"):  # a quick look at the fused resident pass only (shared second phase; 128- and 256-row tiles)
+if os.environ.get("KT_SANITIZE_SMALL"):  # a quick look at the fused pass only (128- and 256-row tiles)
     cases = [cases[0], cases[3]]
 if os.environ.get("KT_SANITIZE_BIG"):
-    cases.append(("C2", dict(m=500, n=120_000, p=4000)))
+    cases += [("C2", dict(m=500, n=120_000, p=4000)), ("C2", dict(m=500, n=120_000, p=40_000))]
 for cfg, kw in cases:
     snap = synth.generate(cfg, **kw)
     eng = kt.Engine(snap.R, snap.L, snap.LN)
