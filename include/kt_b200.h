@@ -375,6 +375,38 @@ int kt_debug_compile_tables(const kt_limits* limits, int32_t m, const kt_throttl
                             int32_t n_ns, const int64_t* ns_labels, int32_t dims[12], uint32_t* table, uint32_t* need,
                             uint32_t* nsmask, int32_t* nsw_off, int32_t* nsw_idx, uint32_t* keydir, uint32_t* valrow, uint32_t* hash);
 
+/* ---- test seam of the fused pass (diagnostic only, like tracing) ------------------ */
+/* At launch the fused pass picks, from the shape, a residency (the build compiled for 512 or for 768 resident threads per SM)
+ * and a decide mode (four-lane sub-tiles or lane-per-pod tiles), and sizes its grid to what the device holds.  Most shapes
+ * reach only a few of these combinations, so a test forces them here to compare every build and mode with a reference at
+ * small sizes.  This is a test seam, not a tuning option: the automatic choices are the product's, and no product path sets
+ * a plan.
+ *   threads_per_sm  in: 0 automatic, 512 or 768                     out: the build that ran
+ *   decide          in: 0 automatic, 1 quad sub-tiles, 2 per-pod    out: the mode that ran
+ *   max_ctas        in: 0 what the device holds; else a cap on the grid (clamped to 1..capacity of the chosen build), applied
+ *                   before the automatic choices: they see the capped grid.  A grid larger than the device holds is not offered.
+ *   grid, capacity  out: CTAs launched; CTAs the chosen build fits on the device at once (occupancy x SMs)
+ *   tile, tpc, b, rt  out: the kernel variant of the pass (rt 0: the general family)
+ *   n_chk, n_rec, n_fin, n_sub  out: match tiles, reconcile tiles, status tiles, decide pieces
+ * kt_debug_set_pass_plan(NULL) or an all-zero plan restores the automatic choices (the default); KT_ERR_INVALID for other
+ * values.  While a plan is set, a single-GPU fused pass also checks its in-kernel waits: one that timed out makes kt_sync and
+ * the getters return KT_ERR_STATE; and it first fills every output it writes (bitmaps, codes, admit bits, status columns) with
+ * a poison pattern, so that work it skipped cannot hide behind the previous pass's results.  kt_debug_get_pass_plan reports what the last fused pass of the context ran
+ * (KT_ERR_STATE before the first one). */
+typedef struct kt_pass_plan {
+  int32_t threads_per_sm;
+  int32_t decide;
+  uint32_t max_ctas;
+  uint32_t grid;
+  uint32_t capacity;
+  int32_t tile, tpc, b, rt;
+  uint32_t n_chk, n_rec, n_fin, n_sub;
+} kt_pass_plan;
+#define KT_PLAN_DECIDE_QUAD 1
+#define KT_PLAN_DECIDE_PER_POD 2
+int kt_debug_set_pass_plan(kt_ctx* ctx, const kt_pass_plan* plan);
+int kt_debug_get_pass_plan(kt_ctx* ctx, kt_pass_plan* last);
+
 /* ---- multi-GPU (row-sharded snapshot, one context per GPU) --------------------- */
 /* Each context holds a row shard of both pod kinds and a replica of the throttles; the
  * only exchange is one int64 sum all-reduce of the per-throttle partials between the

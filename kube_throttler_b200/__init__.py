@@ -45,7 +45,7 @@ EXPORTS = [
     "kt_enable_trace", "kt_get_trace", "kt_host_alloc", "kt_host_alloc_upload", "kt_host_free", "kt_upload_pods", "kt_upload_pods_compact", "kt_upload_pods_packed", "kt_set_async_uploads", "kt_update_pod_rows", "kt_upload_namespaces",
     "kt_upload_throttles", "kt_upload_status", "kt_set_reserved", "kt_evaluate", "kt_get_reconcile",
     "kt_match_words", "kt_get_match_bitmap", "kt_get_match_rows", "kt_get_check", "kt_set_sparse_check", "kt_get_check_sparse", "kt_get_check_rows", "kt_get_changed", "kt_get_reconcile_rows", "kt_step_submit", "kt_step_wait", "kt_admit_queue", "kt_get_timing", "kt_comm_unique_id",
-    "kt_comm_init", "kt_comm_destroy", "kt_debug_compile_tables",
+    "kt_comm_init", "kt_comm_destroy", "kt_debug_compile_tables", "kt_debug_set_pass_plan", "kt_debug_get_pass_plan",
 ]
 
 
@@ -104,6 +104,8 @@ def lib():
         L.kt_comm_destroy.argtypes = [vp]
         L.kt_debug_compile_tables.argtypes = [C.POINTER(abi.Limits), C.c_int32, C.POINTER(abi.ThrottleCols), C.POINTER(abi.SelectorTable), C.c_int32, vp,
                                               vp, vp, vp, vp, vp, vp, vp, vp, vp]
+        L.kt_debug_set_pass_plan.argtypes = [vp, C.POINTER(abi.PassPlan)]
+        L.kt_debug_get_pass_plan.argtypes = [vp, C.POINTER(abi.PassPlan)]
         _lib = L
     return _lib
 
@@ -185,6 +187,18 @@ class Engine:
 
     def sync(self):
         self._ck(self._L.kt_sync(self._h))
+
+    def set_pass_plan(self, threads: int = 0, decide: int = 0, max_ctas: int = 0):
+        """Test seam: force the fused pass's build (512 / 768 threads per SM), decide mode (abi.PLAN_DECIDE_*) and a cap on its
+        grid; all zero restores the automatic choices.  Diagnostic only (kt_debug_set_pass_plan)."""
+        plan = abi.PassPlan(threads_per_sm=threads, decide=decide, max_ctas=max_ctas)
+        self._ck(self._L.kt_debug_set_pass_plan(self._h, C.byref(plan)))
+
+    def pass_plan(self) -> abi.PassPlan:
+        """What the last fused pass ran: build, decide mode, grid, capacity, kernel variant, pieces per role."""
+        plan = abi.PassPlan()
+        self._ck(self._L.kt_debug_get_pass_plan(self._h, C.byref(plan)))
+        return plan
 
     # -- uploads ------------------------------------------------------------------------------
     def upload_pods(self, kind: int, pods: PodCols):

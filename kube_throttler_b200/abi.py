@@ -76,6 +76,15 @@ class Timing(C.Structure):
                 ("check_ms", C.c_float), ("total_ms", C.c_float), ("launches", C.c_int32)]
 
 
+PLAN_DECIDE_QUAD, PLAN_DECIDE_PER_POD = 1, 2
+
+
+class PassPlan(C.Structure):  # kt_pass_plan (test seam of the fused pass: kt_debug_set_pass_plan / kt_debug_get_pass_plan)
+    _fields_ = [("threads_per_sm", C.c_int32), ("decide", C.c_int32), ("max_ctas", C.c_uint32), ("grid", C.c_uint32),
+                ("capacity", C.c_uint32), ("tile", C.c_int32), ("tpc", C.c_int32), ("b", C.c_int32), ("rt", C.c_int32),
+                ("n_chk", C.c_uint32), ("n_rec", C.c_uint32), ("n_fin", C.c_uint32), ("n_sub", C.c_uint32)]
+
+
 def ptr(a: Optional[np.ndarray]) -> Optional[int]:
     """Raw address of a C-contiguous numpy array (None -> NULL)."""
     if a is None:

@@ -150,6 +150,10 @@ struct kt_ctx {
   bool trace = false;
   uint32_t trace_roles[4] = {0, 0, 0, 0};  // match tiles, reconcile tiles, status tiles, CTAs launched
   PassSync* last_sync = nullptr;  // counters of the last fused pass: its error flag is checked when results are fetched
+  kt_pass_plan plan{};            // kt_debug_set_pass_plan: forced choices of the fused pass (inputs only; all zero: automatic)
+  bool plan_forced = false;
+  kt_pass_plan ran{};             // what the last fused pass launched (kt_debug_get_pass_plan)
+  bool have_ran = false;
   bool fused = true;  // one-launch pass (k_pass) when the whole pass is asked for; three PDL-chained kernels otherwise
   DevBuf d_changed;  // device-side status diff: {count[2] u32 by pass parity, pad to 16 B, idx[M] i32, flag[M] u8}
   unsigned diff_parity = 0;
@@ -481,21 +485,28 @@ cudaError_t launch_pass(kt_ctx* c, const PassArgs& a0) {
   // Persistent grid: as many CTAs as the device holds at once (never more than there are first-phase tiles); each one draws
   // tiles until the ticket counter runs out, so every CTA is placed at the start and the second phase is shared by all of them.
   const unsigned tiles = a.n_chk + a.n_rec;
+  // a forced plan (kt_debug_set_pass_plan) caps the grid before both choices below and may override either of them
+  const kt_pass_plan& fp = c->plan;
+  auto capped = [&](unsigned n) { return fp.max_ctas != 0 && fp.max_ctas < n ? fp.max_ctas : n; };
   unsigned capacity = 0;
   cudaError_t e = pass_capacity<TPC, B, RT, REG, TILE, kPassThreadsShallow>(c, smem, &capacity);
   if (e != cudaSuccess) return e;
-  const bool deep = tiles > kDeepRounds * capacity;
+  const bool deep = fp.threads_per_sm ? fp.threads_per_sm == kPassThreadsDeep : tiles > kDeepRounds * capped(capacity);
   if (deep && (e = pass_capacity<TPC, B, RT, REG, TILE, kPassThreadsDeep>(c, smem, &capacity)) != cudaSuccess) return e;
-  const unsigned grid = tiles < capacity ? tiles : capacity;
+  const unsigned avail = capped(capacity);
+  const unsigned grid = tiles < avail ? tiles : avail;
   // The decide work: four lanes per pod in sub-tiles of TILE/4 pods spread it over every CTA, but each sub-tile stages its own
   // pre-records and finishes its own constants -- a latency chain of several L2 trips.  That pays while the sub-tiles take at
   // most two rounds of the grid (C4: 625 sub-tiles on 528 CTAs, 46 us against 50 us); beyond that (C5: 3125 sub-tiles on 792 CTAs,
   // 185 us against 167 us) the rounds queue up and lane-per-pod tiles of TILE pods do the same work in a quarter of the pieces.  The
   // factor 2 lies between those two shapes (1.2 and 5.9 rounds); where between them the two cross has not been measured.
   const unsigned n_quad = (unsigned)((a.pend.n + TILE / 4 - 1) / (TILE / 4));
-  a.quad = n_quad <= 2 * grid;
+  a.quad = fp.decide ? fp.decide == KT_PLAN_DECIDE_QUAD : n_quad <= 2 * grid;
   a.n_sub = a.quad ? n_quad : a.n_chk;
   if (c->trace) { c->trace_roles[0] = a.n_chk; c->trace_roles[1] = a.n_rec; c->trace_roles[2] = a.n_fin; c->trace_roles[3] = grid; }
+  kt_pass_plan& ran = c->ran;
+  ran = kt_pass_plan{deep ? kPassThreadsDeep : kPassThreadsShallow, a.quad ? KT_PLAN_DECIDE_QUAD : KT_PLAN_DECIDE_PER_POD, fp.max_ctas, grid, capacity,
+                     TILE, TPC, B, RT, a.n_chk, a.n_rec, a.n_fin, a.n_sub};
   return deep ? launch(c, k_pass<TPC, B, RT, REG, TILE, kPassThreadsDeep>, grid, TILE, smem, /*pdl=*/KT_PASS_PDL != 0, a)
               : launch(c, k_pass<TPC, B, RT, REG, TILE, kPassThreadsShallow>, grid, TILE, smem, /*pdl=*/KT_PASS_PDL != 0, a);
 }
@@ -1089,6 +1100,13 @@ static int evaluate_locked(kt_ctx* c, int64_t now, uint32_t flags) {
     }
   }
   if (whole && (!multi || !c->p2p_failed)) {
+    if (c->plan_forced) {
+      // Test seam: every output and pre-record of the pass is poisoned first (the bitmaps and code rows are zero-filled again by
+      // the pass, as after new rows), so that a piece of work a forced plan never ran cannot hide behind the last pass's results.
+      for (DevBuf* b : {&run.bitmap, &pend.bitmap, &c->d_codes, &c->d_admit, &c->d_pre, &c->d_out})
+        if (b->p) KT_CUDA(c, cudaMemsetAsync(b->p, 0xA5, b->cap, c->stream));
+      run.bitmap_clean = pend.bitmap_clean = false;
+    }
     PassArgs a{};
     a.run = pod_view(run); a.pend = pod_view(pend); a.tb = tb; a.tv = tv; a.out = ov; a.px = px;
     a.run_bitmap = run.bitmap.as<uint32_t>(); a.pend_bitmap = pend.bitmap.as<uint32_t>(); a.codes = c->d_codes.as<uint32_t>();
@@ -1105,8 +1123,11 @@ static int evaluate_locked(kt_ctx* c, int64_t now, uint32_t flags) {
       a.trace = c->d_trace.as<unsigned long long>();
     }
     KT_CUDA(c, dispatch_pass(c, a));
+    c->have_ran = true;
     run.bitmap_clean = pend.bitmap_clean = true;  // zero-filled (if need be) and written by this pass: maintained from here on
-    c->last_sync = (multi && !c->p2p_failed) ? a.sync : nullptr;  // only a pass that waits for OTHER ranks can time out
+    // only a pass that waits for OTHER ranks can time out; under a forced plan the waits on its own tiles are checked as well
+    // (a wait on a larger ticket would stall there, on a grid of a few CTAs, and must not pass as void results)
+    c->last_sync = (multi && !c->p2p_failed) || c->plan_forced ? a.sync : nullptr;
     c->last = kt_timing{};
     c->last.launches = 1;
     c->evaluated = true;
@@ -1539,6 +1560,31 @@ int kt_debug_compile_tables(const kt_limits* lim, int32_t m, const kt_throttle_c
   };
   put(table, ht.table); put(need, ht.need); put(nsmask, ht.nsmask); put(nsw_off, ht.nsw_off); put(nsw_idx, ht.nsw_idx);
   put(keydir, ht.keydir); put(valrow, ht.valrow); put(hash, ht.hash);
+  return KT_OK;
+}
+
+int kt_debug_set_pass_plan(kt_ctx* c, const kt_pass_plan* plan) {
+  if (!c) return KT_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(c->mu);
+  kt_pass_plan p{};
+  if (plan) {
+    p.threads_per_sm = plan->threads_per_sm;
+    p.decide = plan->decide;
+    p.max_ctas = plan->max_ctas;
+  }
+  if (p.threads_per_sm != 0 && p.threads_per_sm != kPassThreadsShallow && p.threads_per_sm != kPassThreadsDeep)
+    return fail(c, KT_ERR_INVALID, "threads_per_sm %d: expected 0, %d or %d", p.threads_per_sm, kPassThreadsShallow, kPassThreadsDeep);
+  if (p.decide < 0 || p.decide > KT_PLAN_DECIDE_PER_POD) return fail(c, KT_ERR_INVALID, "decide %d: expected 0, 1 or 2", p.decide);
+  c->plan = p;
+  c->plan_forced = p.threads_per_sm != 0 || p.decide != 0 || p.max_ctas != 0;
+  return KT_OK;
+}
+
+int kt_debug_get_pass_plan(kt_ctx* c, kt_pass_plan* last) {
+  if (!c || !last) return KT_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(c->mu);
+  if (!c->have_ran) return fail(c, KT_ERR_STATE, "kt_debug_get_pass_plan before the first fused pass");
+  *last = c->ran;
   return KT_OK;
 }
 

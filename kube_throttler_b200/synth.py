@@ -115,15 +115,20 @@ def _namespace_set(ns_reqs_of_terms, ns_labels) -> str:
     return "".join(out)
 
 
-def _gen_selectors(rng, m: int, kind: np.ndarray, q_max: int = 0, layout_ns_labels=None):
+def _gen_selectors(rng, m: int, kind: np.ndarray, q_max: int = 0, layout_ns_labels=None, terms=None):
     """CSR selector table: T in {1,2} (80/20), Q in {1,2,3} (60/30/10); 85% equality, 5% each
     In(2-3 values) / NotIn / Exists / DoesNotExist.  ClusterThrottle terms get 0-2 namespace requirements.
+    terms=k: T = 1 for k = 1, else uniform in 1..k with the last throttle at exactly k (so k fixes the table's term planes).
     Requirement pool layout: all podSelector requirements (term order), then all namespaceSelector ones."""
     zp = _zipf_p(V_VALUES)
     term_off = [0]
     pod_reqs, ns_reqs = [], []  # per term: list of (key, op, [vals])
     for t in range(m):
-        T = 1 if rng.random() < 0.8 else 2
+        u = rng.random()
+        if terms is None:
+            T = 1 if u < 0.8 else 2
+        else:
+            T = terms if t == m - 1 else 1 + int(u * terms)
         for _ in range(T):
             Q = int(rng.integers(1, q_max + 1)) if q_max else int(rng.choice([1, 2, 3], p=[0.6, 0.3, 0.1]))
             keys = rng.choice(K_POD_KEYS, size=Q, replace=False)
@@ -336,13 +341,19 @@ def _equality_thresholds(snap: abi.Snapshot, rng, frac: float = 0.12) -> None:
 
 def generate(config: str = "C2", *, seed=None, m=None, n=None, p=None, R=None, n_ns=None, cluster_frac=None,
              override_frac=None, L: int = 8, sort_by_namespace: bool = True, now: int = NOW_2026,
-             calibrate: bool = True, q_max: int = 0, column_layout: bool = False, values=None) -> abi.Snapshot:
+             calibrate: bool = True, q_max: int = 0, column_layout: bool = False, values=None, terms=None) -> abi.Snapshot:
     """Build the snapshot of a BASELINE config (or a scaled variant via keyword overrides).
+
+    terms: None draws one or two selector terms per throttle (80/20); 1 gives every throttle one term (one term plane per
+    table entry); 2, 3 or 4 draw 1..terms terms, with the last throttle at exactly `terms` (3: two plane pairs, one of them a
+    padded empty plane; 4: two full plane pairs).
 
     values: None keeps the requests of the config (cpu milli, memory bytes, ...); "wide", "carry" or "signed" rewrites the
     request columns of the running and pending pods (VALUE_REGIMES, _rewrite_values) before the thresholds are calibrated, within
     the domain the host layer guarantees (per column, sum of |v| over running + pending + reservations + status below 2^62), and
     adds exact-equality thresholds (_equality_thresholds)."""
+    if terms not in (None, 1, 2, 3, 4):
+        raise ValueError(f"terms={terms!r}: expected None or 1..4")
     base = dict(CONFIGS[config])
     for k, v in dict(seed=seed, m=m, n=n, p=p, R=R, n_ns=n_ns, cluster_frac=cluster_frac, override_frac=override_frac).items():
         if v is not None:
@@ -383,7 +394,7 @@ def generate(config: str = "C2", *, seed=None, m=None, n=None, p=None, R=None, n
     thr_flags[rng.random(m) < 0.01] = 0  # 1% belong to another throttler instance
 
     # q_max > 3: terms needing > 3 keys present (6-bit counters); column_layout: ClusterThrottles ordered as kt_host.cc orders them
-    sel = _gen_selectors(rng, m, kind, q_max, layout_ns_labels=ns_labels if column_layout else None)
+    sel = _gen_selectors(rng, m, kind, q_max, layout_ns_labels=ns_labels if column_layout else None, terms=terms)
 
     snap = abi.Snapshot(
         R=R, L=L, LN=LN, running=running, pending=pending, ns_labels=ns_labels, kind=kind, thr_ns=thr_ns,

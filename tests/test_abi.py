@@ -45,6 +45,9 @@ def test_struct_layouts(kt):
     assert C.sizeof(abi.StatusCols) == 8 * 8
     assert C.sizeof(abi.ReconcileOut) == 8 * 8
     assert C.sizeof(abi.Timing) == 24
+    assert C.sizeof(abi.PassPlan) == 13 * 4
+    assert [abi.PassPlan.__dict__[f].offset for f in ("threads_per_sm", "decide", "max_ctas", "grid", "capacity", "tile", "n_chk", "n_sub")] == \
+        [0, 4, 8, 12, 16, 20, 36, 48]
 
 
 def test_library_is_sm90a_cuda(kt):
@@ -60,6 +63,34 @@ def test_library_is_sm90a_cuda(kt):
     sass = subprocess.run([cuobjdump, "-sass", kt.LIB_PATH], capture_output=True, text=True).stdout
     for k in ("k_reconcile", "k_finalize", "k_check"):
         assert k in sass
+
+
+def test_fused_pass_builds_and_their_register_budgets(kt):
+    """The shipped SASS holds all 24 k_pass builds: the 12 kernel variants of dispatch_pass (fast family: TPC 1/2 x R <= 4/8 x
+    128/256-row tiles; general family: TPC 1/2 x B 2/6) for 512 and for 768 resident threads per SM.  What the comment at
+    kPassThreadsShallow claims holds: every 512-thread build fits 128 registers with no stack or local memory (no spills), every
+    768-thread build fits 80 registers (a spill there is tolerated: those builds run the passes many rounds deep)."""
+    import shutil
+    import subprocess
+
+    cuobjdump = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
+    if not os.path.exists(cuobjdump):
+        pytest.skip("cuobjdump not available")
+    out = subprocess.run([cuobjdump, "-res-usage", kt.LIB_PATH], capture_output=True, text=True, check=True).stdout
+    usage = {}
+    for name, res in re.findall(r"Function (_ZN2kt6k_pass\S+):\s*\n\s*(.*)", out):
+        m = re.fullmatch(r"_ZN2kt6k_passILi(\d)ELi(\d)ELi(\d)ELb([01])ELi(\d+)ELi(\d+)EEEvNS_8PassArgsE:?", name)
+        assert m, name
+        usage[tuple(int(x) for x in m.groups())] = {k: int(v) for k, v in re.findall(r"(\w+)(?:\[\d+\])?:(\d+)", res)}
+    fast = [(tpc, 2, rt, 1, tile) for tpc in (1, 2) for rt in (4, 8) for tile in (128, 256)]
+    general = [(tpc, b, 0, 0, 128) for tpc in (1, 2) for b in (2, 6)]
+    want = {v + (threads,) for v in fast + general for threads in (512, 768)}
+    assert set(usage) == want, sorted(set(usage) ^ want)
+    for key, u in usage.items():
+        if key[-1] == 512:
+            assert u["REG"] <= 128 and u["STACK"] == 0 and u["LOCAL"] == 0, (key, u)
+        else:
+            assert u["REG"] <= 80, (key, u)
 
 
 def test_no_gpu_means_error_not_fallback(kt):

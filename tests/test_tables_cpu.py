@@ -117,6 +117,35 @@ def test_compiled_tables_reproduce_the_oracle_relation(kt, oracle, kw):
     np.testing.assert_array_equal(match_bitmap(t, snap.pending, False), want.pend_bitmap)
 
 
+@pytest.mark.parametrize("config,terms,tppad", [
+    ("C2", 1, 1), ("C3", 1, 1),   # one term per throttle: one plane per table entry
+    ("C2", 3, 4), ("C3", 3, 4),   # up to three: two plane pairs, the fourth plane padding
+    ("C2", 4, 4), ("C3", 4, 4),   # up to four: two full plane pairs
+])
+def test_term_planes(kt, oracle, config, terms, tppad):
+    """synth terms=1 / 3 / 4 give the table compiler one plane per entry or two plane pairs; the relation still equals the
+    oracle's, and a plane beyond a throttle's own terms (the padded plane when TP = 3) can match no pod: its namespace mask and
+    its needed counts are zero."""
+    snap = synth.generate(config, m=150, n=900, p=250, terms=terms)
+    nterms = np.diff(snap.term_off)
+    assert nterms.max() == terms and nterms.min() == 1
+    t = compile_tables(kt, snap)
+    assert t["TPpad"] == tppad
+    want = oracle.columnar_evaluate(snap, words_per_row=t["Wp"])
+    np.testing.assert_array_equal(match_bitmap(t, snap.running, True), want.run_bitmap)
+    np.testing.assert_array_equal(match_bitmap(t, snap.pending, False), want.pend_bitmap)
+    w = np.arange(snap.m) >> 5
+    bit = np.uint32(1) << (np.arange(snap.m) & 31).astype(np.uint32)
+    for s in range(tppad):
+        unused = nterms <= s
+        assert not (t["nsmask"][:, w[unused], s] & bit[unused]).any(), f"plane {s}"
+        assert not (t["need"][w[unused], s, :] & bit[unused][:, None]).any(), f"plane {s}"
+        if s < terms:
+            assert t["nsmask"][:, :, s].any(), f"plane {s} is never used"
+    if terms == 3:
+        assert not t["nsmask"][:, :, 3].any() and not t["need"][:, 3, :].any()
+
+
 def test_sparse_ids_take_the_hash(kt, oracle):
     from test_gpu_parity import _remap_label_ids
 

@@ -7,12 +7,34 @@ R = 1; wide / compact / packed uploads (packed: the fused unpack + translate ker
 sparse check result, observed status + the device-side status diff + row getters, GIVEN_STATUS passes, queue admission rounds.
 KT_SANITIZE_BIG=1 adds two 120k-row snapshots with more tiles than the device holds CTAs at once, so that CTAs run several tiles
 one after the other in the same shared memory: 4k pending pods (four-lane decide sub-tiles) and 40k (more sub-tiles than two
-rounds of the grid: lane-per-pod decide tiles after reconcile tiles)."""
+rounds of the grid: lane-per-pod decide tiles after reconcile tiles).
+Forced plans (kt_debug_set_pass_plan) then run every k_pass build (512 and 768 threads per SM) under both decide modes on the
+grid the device holds and on one of a single CTA, for small shapes of 128- and 256-row tiles, the general family and two plane
+pairs per table entry.  KT_SANITIZE_PLANS=1 runs only those."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
 import kube_throttler_b200 as kt
 from kube_throttler_b200 import abi, synth
+
+plan_cases = [("C2", dict(m=40, n=70, p=33, R=1)), ("C3", dict(m=600, n=1500, p=300, terms=2)), ("C2", dict(m=200, n=600, p=300, q_max=6, terms=3))]
+for cfg, kw in plan_cases:
+    snap = synth.generate(cfg, **kw)
+    eng = kt.Engine(snap.R, snap.L, snap.LN)
+    eng.upload_snapshot(snap)
+    eng.set_sparse_check(4 * snap.pending.n + 64)
+    for threads in (512, 768):
+        for decide in (abi.PLAN_DECIDE_QUAD, abi.PLAN_DECIDE_PER_POD):
+            for cap in (0, 1):
+                eng.set_pass_plan(threads, decide, cap)
+                eng.evaluate(snap.now)
+                eng.sync()
+    plan = eng.pass_plan()
+    eng.close()
+    print(cfg, kw, "ok: forced plans, tile", plan.tile, "tpc", plan.tpc, "b", plan.b, "rt", plan.rt, flush=True)
+if os.environ.get("KT_SANITIZE_PLANS"):
+    print("sanitize target done")
+    sys.exit(0)
 
 cases = [("C3", dict(m=300, n=3000, p=500)), ("C3", dict(m=900, n=2500, p=400)), ("C2", dict(m=200, n=2000, p=300, L=12, q_max=6)),
          ("C2", dict(m=40, n=70, p=33, R=1))]
