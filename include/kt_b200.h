@@ -336,6 +336,19 @@ int kt_get_match_bitmap(kt_ctx* ctx, int kind, uint32_t* words /*[n][words_per_r
  * host finds which reserved pods a reconcile has observed (unreserveAffectedPods, throttle_controller.go:135-155)
  * without downloading the whole relation. */
 int kt_get_match_rows(kt_ctx* ctx, int kind, int64_t k, const int64_t* rows, uint32_t* words /*[k][words_per_row]*/);
+/* The same relation from the throttles' side (affectedPods, throttle_controller.go:221-246, clusterthrottle_controller.go:224-270),
+ * for k listed throttles, transposed on the device from what the last pass (or kt_admit_queue) left, exactly as
+ * kt_get_match_bitmap / kt_get_check would deliver it.  For throttle idx[j], the rows whose bit is set, ascending, are
+ * rows[off[j] .. off[j+1]).
+ *   RUNNING: the affectedPods relation as kt_get_match_bitmap defines it (finished pods included: the caller splits them by
+ *            its flags).
+ *   PENDING: the pods the throttle affects; codes[i] = the 2-bit code of (rows[i], idx[j]) that kt_get_check would show.
+ * idx entries must lie in [0, M) (KT_ERR_INVALID otherwise); duplicates each get their own segment; k = 0 is valid.  off[0..k]
+ * is always written; rows / codes only when off[k] <= cap -- otherwise the caller retries with a larger cap.  codes may be NULL
+ * and must be NULL for RUNNING.  Only the words of the listed throttles are read (count, offsets, scan, fill: four launches,
+ * one read of off[], one copy of the rows).  Multi-GPU: each rank answers for its own rows. */
+int kt_get_match_columns(kt_ctx* ctx, int kind, int64_t k, const int32_t* idx, int64_t* off /*[k+1]*/, int64_t* rows /*[cap]*/,
+                         uint8_t* codes /*[cap] or NULL*/, int64_t cap);
 /* codes: 2 bits per (pending pod, throttle), pod-major, 16 codes per uint32:
  *   code(p,t) = (codes[p*2*words_per_row + (t>>4)] >> (2*(t&15))) & 3
  * admit[p] = 1 iff every affected throttle is KT_CHECK_NOT_THROTTLED (plugin.go:177-180).

@@ -125,6 +125,24 @@ const char* kth_unreserve(kth_plugin* p, const char* pod_json);
  * {"amount":{...},"pods":["ns/name",...]} -- reserved_resource_amounts.go:113-126. */
 const char* kth_reserved(kth_plugin* p, int kind, const char* throttle_nn);
 
+/* affectedPods(thr) of one Throttle (ns != "") or ClusterThrottle (ns == ""), read from the device's match relations
+ * (throttle_controller.go:221-246, clusterthrottle_controller.go:224-270), plus the queued pods the throttle holds back:
+ * {"pods":["ns/name",...],"terminatedPods":[...],"queued":[{"pod":"ns/name","status":"active"},...]}
+ *   pods            affectedNonTerminatedPods: counted (shouldCountIn), matching, not finished -- exactly what the next
+ *                   reconcile sums into status.used
+ *   terminatedPods  EVERY matching counted pod that has finished.  A listing, not reconcile's slice: the reference's Throttle
+ *                   controller keeps only the last of them (Q8, DESIGN.md section 5), which stays reproduced in reconcile's
+ *                   un-reservation and is not copied here
+ *   queued          the pods of the resident scheduling queue whose affected throttles include this one, with the
+ *                   CheckThrottleStatus that PreFilter by key would give now (informer status + reservations,
+ *                   isThrottledOnEqual = false): "not-throttled", "active", "insufficient", "pod-requests-exceeds-threshold"
+ * Every list is sorted by namespace, then name (the reference's lister order is unspecified).  Pods of namespaces the lister
+ * does not hold never appear for a ClusterThrottle.  {"error": ...} for an unknown throttle, a throttle whose throttlerName is
+ * not this plugin's, and a podSelector conversion error that some counted pod reaches (the text affectedPods returns; the first
+ * such pod in informer order names it).  No side effects: no status is written, no gauge recorded, nothing un-reserved, and
+ * every other call answers as it would have; a device pass runs only when the state changed since the last one this call ran. */
+const char* kth_affected_pods(kth_plugin* p, const char* ns, const char* name);
+
 /* The controllers' Prometheus gauges in text exposition format (throttle_metrics.go:27-131,
  * clusterthrottle_metrics.go:27-131, metrics_recorder.go:25-67): throttle_* families labelled {name,namespace,resource,uid},
  * clusterthrottle_* families labelled {name,resource,uid}; spec threshold / status.throttled / status.used /

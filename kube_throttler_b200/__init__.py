@@ -44,7 +44,7 @@ EXPORTS = [
     "kt_create", "kt_destroy", "kt_last_error", "kt_version", "kt_set_stream", "kt_sync", "kt_enable_timing",
     "kt_enable_trace", "kt_get_trace", "kt_host_alloc", "kt_host_alloc_upload", "kt_host_free", "kt_upload_pods", "kt_upload_pods_compact", "kt_upload_pods_packed", "kt_set_async_uploads", "kt_update_pod_rows", "kt_upload_namespaces",
     "kt_upload_throttles", "kt_upload_status", "kt_set_reserved", "kt_evaluate", "kt_get_reconcile",
-    "kt_match_words", "kt_get_match_bitmap", "kt_get_match_rows", "kt_get_check", "kt_set_sparse_check", "kt_get_check_sparse", "kt_get_check_rows", "kt_get_changed", "kt_get_reconcile_rows", "kt_step_submit", "kt_step_wait", "kt_admit_queue", "kt_get_timing", "kt_comm_unique_id",
+    "kt_match_words", "kt_get_match_bitmap", "kt_get_match_rows", "kt_get_match_columns", "kt_get_check", "kt_set_sparse_check", "kt_get_check_sparse", "kt_get_check_rows", "kt_get_changed", "kt_get_reconcile_rows", "kt_step_submit", "kt_step_wait", "kt_admit_queue", "kt_get_timing", "kt_comm_unique_id",
     "kt_comm_init", "kt_comm_destroy", "kt_debug_compile_tables", "kt_debug_set_pass_plan", "kt_debug_get_pass_plan",
 ]
 
@@ -97,6 +97,7 @@ def lib():
         L.kt_match_words.argtypes = [vp]
         L.kt_match_words.restype = C.c_int32
         L.kt_get_match_bitmap.argtypes = [vp, C.c_int, vp]
+        L.kt_get_match_columns.argtypes = [vp, C.c_int, C.c_int64, vp, vp, vp, vp, C.c_int64]
         L.kt_get_check.argtypes = [vp, vp, vp]
         L.kt_get_timing.argtypes = [vp, C.POINTER(abi.Timing)]
         L.kt_comm_unique_id.argtypes = [vp]
@@ -338,6 +339,23 @@ class Engine:
         admit = np.zeros(rows.shape[0], np.uint8)
         self._ck(self._L.kt_get_check_rows(self._h, rows.shape[0], abi.ptr(rows), abi.ptr(codes), abi.ptr(admit)))
         return codes, admit
+
+    def match_columns(self, kind: int, idx, cap: Optional[int] = None):
+        """affectedPods from the throttles' side: (off[k+1], rows, codes) with throttle idx[j]'s rows, ascending, in
+        rows[off[j]:off[j+1]]; codes (PENDING only, else None) the 2-bit check code of each (row, idx[j]).  `cap` sizes the
+        first attempt (default: the rows of the kind); a larger relation is fetched again with the exact room."""
+        idx = np.ascontiguousarray(idx, np.int32)
+        k = idx.shape[0]
+        off = np.zeros(k + 1, np.int64)
+        cap = self.n[kind] if cap is None else cap
+        while True:
+            rows = np.zeros(max(cap, 1), np.int64)
+            codes = np.zeros(max(cap, 1), np.uint8) if kind == abi.PODS_PENDING else None
+            self._ck(self._L.kt_get_match_columns(self._h, kind, k, abi.ptr(idx), abi.ptr(off), abi.ptr(rows), abi.ptr(codes), cap))
+            total = int(off[k])
+            if total <= cap:
+                return off, rows[:total], (codes[:total] if codes is not None else None)
+            cap = total
 
     def get_changed(self):
         """(sorted indices of the throttles whose status this pass changes, flags[m]) -- the device-side diff against kt_upload_status."""

@@ -6,7 +6,7 @@
 // without walking the queue pod by pod:
 //
 //   * a throttle's view of the queue is its TOUCHER LIST: the queue positions whose pod it affects, ascending (a CSR built
-//     once from the pending match bitmap);
+//     once from the pending match bitmap: ColumnView below);
 //   * the load pod i sees on throttle t is the sum of the requests of the ADMITTED pods before i in t's list -- an exclusive
 //     prefix sum along the list;
 //   * which pods are admitted is the unknown.  Every pod is Undecided, Admitted or surely-reJected.  One round computes, for
@@ -27,9 +27,111 @@
 
 namespace kt {
 
-constexpr int kAdmitBlock = 1024;  // queue positions per CSR build block
+constexpr int kColBlock = 1024;  // rows per counting block of a row-list build
 constexpr uint8_t kUndecided = 0, kAdmitted = 1, kRejected = 2;
 
+// ---- per-throttle row lists: the match relation transposed ---------------------------------------------------------
+// For k listed throttles (duplicates allowed; idx == nullptr lists 0..k-1), the rows i in [0, count) whose bit of
+// bitmap row first + i is set, ascending, as one CSR: entry j's rows are rows[off[j] .. off[j+1]).  Four launches:
+// per-(block, entry) counts, per-entry block offsets and lengths, an exclusive scan of the lengths, the fill.  A warp
+// walks one block of kColBlock rows for 32 consecutive entries, 32 rows at a time (lane = row): the word of an entry's
+// throttle is loaded once per run of entries that share it, and a ballot per entry counts (and in the fill places)
+// the rows in lane order.  Only the words of the listed throttles are read.  kt_admit_queue builds its toucher lists
+// with it (all throttles over the queue rows), kt_get_match_columns the columns it is asked for (all rows).
+struct ColumnView {
+  const uint32_t* bitmap;  // [n][Wp]
+  int Wp;
+  int64_t first, count;    // the rows walked: [first, first + count); list entries hold i = row - first
+  const int32_t* idx;      // [k] or nullptr
+  int64_t k;
+  int nblk;                // ceil(count / kColBlock)
+  int32_t* cnt;            // [nblk][k] set bits per (block, entry); after k_col_lengths: the block's offset in the entry's list
+  int64_t* off;            // [k + 1]
+  int64_t* rows;           // [off[k]]
+  const uint32_t* codes;   // [n][2Wp] 2-bit codes to gather beside the rows, or nullptr
+  uint8_t* codes_out;      // [off[k]]
+};
+
+template <bool FILL>
+__device__ __forceinline__ void col_walk(const ColumnView& v) {
+  const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  const int64_t groups = (v.k + 31) >> 5;
+  if (warp >= (int64_t)v.nblk * groups) return;
+  const int blk = (int)(warp / groups);
+  const int64_t e0 = (warp % groups) * 32;
+  const int ne = v.k - e0 < 32 ? (int)(v.k - e0) : 32;
+  const int my_t = lane < ne ? (v.idx ? v.idx[e0 + lane] : (int)(e0 + lane)) : 0;
+  const int64_t lo = (int64_t)blk * kColBlock, hi = lo + kColBlock < v.count ? lo + kColBlock : v.count;
+  // count: this lane's entry's set bits so far; fill: where its next row goes
+  int64_t at = 0;
+  if (FILL && lane < ne) at = v.off[e0 + lane] + v.cnt[(size_t)blk * v.k + e0 + lane];
+  const uint32_t below = (1u << lane) - 1u;
+  for (int64_t base = lo; base < hi; base += 32) {
+    const int64_t i = base + lane;
+    const bool on = i < hi;
+    const int64_t p = v.first + i;
+    int wcur = -1;
+    uint32_t x = 0u;
+    for (int e = 0; e < ne; ++e) {
+      const int t = __shfl_sync(kFull, my_t, e);
+      if ((t >> 5) != wcur) {  // uniform: every lane sees the same t
+        wcur = t >> 5;
+        x = on ? __ldg(&v.bitmap[p * v.Wp + wcur]) : 0u;
+      }
+      const bool bit = (x >> (t & 31)) & 1u;
+      const uint32_t m = __ballot_sync(kFull, bit);
+      if (FILL) {
+        const int64_t pos = __shfl_sync(kFull, at, e) + __popc(m & below);
+        if (bit) {
+          v.rows[pos] = i;
+          if (v.codes) v.codes_out[pos] = (uint8_t)((__ldg(&v.codes[p * 2 * v.Wp + (t >> 4)]) >> (2 * (t & 15))) & 3u);
+        }
+      }
+      if (lane == e) at += __popc(m);
+    }
+  }
+  if (!FILL && lane < ne) v.cnt[(size_t)blk * v.k + e0 + lane] = (int32_t)at;
+}
+__global__ void __launch_bounds__(128) k_col_count(ColumnView v) { col_walk<false>(v); }
+// per entry: block counts -> block offsets inside the entry's list, and the list length
+__global__ void __launch_bounds__(256) k_col_lengths(ColumnView v) {
+  const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= v.k) return;
+  int32_t run = 0;
+  for (int b = 0; b < v.nblk; ++b) {
+    const int32_t c = v.cnt[(size_t)b * v.k + j];
+    v.cnt[(size_t)b * v.k + j] = run;
+    run += c;
+  }
+  v.off[j + 1] = run;  // length for now
+}
+__global__ void __launch_bounds__(1024) k_col_starts(ColumnView v) {  // exclusive scan of the lengths, one CTA
+  __shared__ long long s_part[1024];
+  const int tid = threadIdx.x;
+  const int64_t per = (v.k + 1023) / 1024;
+  const int64_t lo = tid * per, hi = lo + per < v.k ? lo + per : v.k;
+  long long sum = 0;
+  for (int64_t j = lo; j < hi; ++j) sum += v.off[j + 1];
+  s_part[tid] = sum;
+  __syncthreads();
+  for (int d = 1; d < 1024; d <<= 1) {
+    const long long x = tid >= d ? s_part[tid - d] : 0;
+    __syncthreads();
+    s_part[tid] += x;
+    __syncthreads();
+  }
+  long long run = tid ? s_part[tid - 1] : 0;
+  if (tid == 0) v.off[0] = 0;
+  for (int64_t j = lo; j < hi; ++j) {
+    run += v.off[j + 1];
+    v.off[j + 1] = run;
+  }
+}
+// the lists themselves: the same walk as k_col_count, each set bit stored at its entry's next position
+__global__ void __launch_bounds__(128) k_col_fill(ColumnView v) { col_walk<true>(v); }
+
+// ---- queue-ordered greedy admission -----------------------------------------------------------------------------------
 struct AdmitView {
   int64_t first, count;            // the queue: pending rows [first, first + count), in row order
   const int64_t* req;              // [R][n] pending request columns
@@ -38,74 +140,14 @@ struct AdmitView {
   int64_t n;                       // rows of the pending table
   int Wp, W, M, R;
   const unsigned char* pre;        // [M] pre-records of a GIVEN_STATUS pass (thresholds, observed used + reserved, flags)
-  int32_t* cnt2;                   // [nblk][M] touchers per (CSR block, throttle); after k_admit_offsets: their offsets
-  int32_t* tl_off;                 // [M + 1]
-  int32_t* tl_pod;                 // [nnz] queue positions, ascending per throttle
+  const int64_t* tl_off;           // [M + 1] toucher lists (ColumnView over the queue, every throttle)
+  const int64_t* tl_pod;           // [nnz] queue positions, ascending per throttle
   uint8_t* state;                  // [count]
   uint32_t* fail;                  // [count] bit 0: some pair fails under the largest load, bit 1: under the smallest
   uint32_t* codes;                 // [n][2Wp] (rows of the pending table)
   unsigned char* admit;            // [n]
   uint32_t* counters;              // [0] undecided pods after the last update, [1] admitted
-  int nblk;
 };
-
-// touchers per (block of kAdmitBlock queue positions, throttle): one warp per (block, word), lane = throttle
-__global__ void __launch_bounds__(128) k_admit_count(AdmitView a) {
-  const int warp = (int)((blockIdx.x * (unsigned)blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
-  if (warp >= a.nblk * a.W) return;
-  const int blk = warp / a.W, w = warp % a.W;
-  const int64_t lo = (int64_t)blk * kAdmitBlock, hi = lo + kAdmitBlock < a.count ? lo + kAdmitBlock : a.count;
-  int c = 0;
-  for (int64_t i = lo; i < hi; ++i) c += (__ldg(&a.bitmap[(a.first + i) * a.Wp + w]) >> lane) & 1;
-  const int t = w * 32 + lane;
-  if (t < a.M) a.cnt2[(size_t)blk * a.M + t] = c;
-}
-// per throttle: block counts -> block offsets inside the throttle's list, and the list length; then (one CTA) the lists' starts
-__global__ void __launch_bounds__(256) k_admit_lengths(AdmitView a) {
-  const int t = blockIdx.x * blockDim.x + threadIdx.x;
-  if (t >= a.M) return;
-  int run = 0;
-  for (int b = 0; b < a.nblk; ++b) {
-    const int c = a.cnt2[(size_t)b * a.M + t];
-    a.cnt2[(size_t)b * a.M + t] = run;
-    run += c;
-  }
-  a.tl_off[t + 1] = run;  // length for now
-}
-__global__ void __launch_bounds__(1024) k_admit_starts(AdmitView a) {  // exclusive scan of the lengths, one CTA
-  __shared__ int s_part[1024];
-  const int tid = threadIdx.x;
-  const int per = (a.M + 1023) / 1024;
-  const int lo = tid * per, hi = lo + per < a.M ? lo + per : a.M;
-  int sum = 0;
-  for (int t = lo; t < hi; ++t) sum += a.tl_off[t + 1];
-  s_part[tid] = sum;
-  __syncthreads();
-  for (int d = 1; d < 1024; d <<= 1) {
-    const int v = tid >= d ? s_part[tid - d] : 0;
-    __syncthreads();
-    s_part[tid] += v;
-    __syncthreads();
-  }
-  int run = tid ? s_part[tid - 1] : 0;
-  if (tid == 0) a.tl_off[0] = 0;
-  for (int t = lo; t < hi; ++t) {
-    const int len = a.tl_off[t + 1];
-    run += len;
-    a.tl_off[t + 1] = run;
-  }
-}
-// the lists themselves: same walk as k_admit_count, lane b appends in queue order
-__global__ void __launch_bounds__(128) k_admit_fill(AdmitView a) {
-  const int warp = (int)((blockIdx.x * (unsigned)blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
-  if (warp >= a.nblk * a.W) return;
-  const int blk = warp / a.W, w = warp % a.W;
-  const int64_t lo = (int64_t)blk * kAdmitBlock, hi = lo + kAdmitBlock < a.count ? lo + kAdmitBlock : a.count;
-  const int t = w * 32 + lane;
-  int at = t < a.M ? a.tl_off[t] + a.cnt2[(size_t)blk * a.M + t] : 0;
-  for (int64_t i = lo; i < hi; ++i)
-    if ((__ldg(&a.bitmap[(a.first + i) * a.Wp + w]) >> lane) & 1) a.tl_pod[at++] = (int32_t)i;
-}
 
 // start of a round: every pod forgets last round's pair verdicts; the code words of its affected throttles are cleared (the
 // pairs OR their codes back in)
@@ -149,7 +191,7 @@ template <int RMAX>
 __global__ void __launch_bounds__(128) k_admit_round(AdmitView a) {
   const int t = (int)((blockIdx.x * (unsigned)blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
   if (t >= a.M) return;
-  const int lo = a.tl_off[t], hi = a.tl_off[t + 1];
+  const int64_t lo = a.tl_off[t], hi = a.tl_off[t + 1];
   if (lo == hi) return;
   const int R = a.R;
   const unsigned char* src = a.pre + (size_t)t * pre_record_bytes(R);
@@ -171,9 +213,9 @@ __global__ void __launch_bounds__(128) k_admit_round(AdmitView a) {
 #pragma unroll
   for (int r = 0; r < RMAX; ++r) run[0][r] = run[1][r] = 0;
 
-  for (int at = lo; at < hi; at += 32) {
+  for (int64_t at = lo; at < hi; at += 32) {
     const bool on = at + lane < hi;
-    const int i = on ? a.tl_pod[at + lane] : 0;
+    const int64_t i = on ? a.tl_pod[at + lane] : 0;
     const int64_t p = a.first + i;
     const uint8_t st = on ? a.state[i] : kRejected;
     const uint32_t present = on ? a.present[p] : 0u;

@@ -158,7 +158,8 @@ struct kt_ctx {
   DevBuf d_changed;  // device-side status diff: {count[2] u32 by pass parity, pad to 16 B, idx[M] i32, flag[M] u8}
   unsigned diff_parity = 0;
   bool have_diff = false;  // the last pass produced a diff (an observed status was uploaded)
-  DevBuf d_adm_cnt2, d_adm_off, d_adm_pod, d_adm_state, d_adm_fail, d_adm_counters;  // kt_admit_queue (kt_admit.cuh)
+  DevBuf d_col_idx, d_col_cnt, d_col_off, d_col_rows;  // per-throttle row lists (kt_admit.cuh ColumnView): kt_admit_queue, kt_get_match_columns
+  DevBuf d_adm_state, d_adm_fail, d_adm_counters;      // kt_admit_queue (kt_admit.cuh)
   DevBuf d_pre;    // [M] pre-records, finalize tiles -> decide tiles (kt_kernels.cuh pre_record_bytes)
   // per-throttle outputs of the reconcile half: ONE device block (and one pinned host mirror) so that kt_get_reconcile
   // is a single D2H copy; o_off[i] = byte offset of {used, used_cnt, calc_thr, calc_cnt, used_present, throttled,
@@ -596,8 +597,8 @@ void kt_destroy(kt_ctx* c) {
                    &c->d_thr_present, &c->d_thr_cnt, &c->d_ovr_off, &c->d_ovr_begin, &c->d_ovr_end, &c->d_ovr_flags, &c->d_ovr_thr,
                    &c->d_ovr_present, &c->d_ovr_cnt, &c->d_st_calculated, &c->d_st_calc_thr, &c->d_st_calc_present, &c->d_st_calc_cnt,
                    &c->d_st_used, &c->d_st_used_present, &c->d_st_used_cnt, &c->d_st_throttled, &c->d_reserved, &c->d_reserved_present,
-                   &c->d_reserved_cnt, &c->d_part, &c->d_sync, &c->d_trace, &c->d_pre, &c->d_changed, &c->d_adm_cnt2, &c->d_adm_off, &c->d_adm_pod,
-                   &c->d_adm_state, &c->d_adm_fail, &c->d_adm_counters, &c->d_out, &c->d_codes, &c->d_admit};
+                   &c->d_reserved_cnt, &c->d_part, &c->d_sync, &c->d_trace, &c->d_pre, &c->d_changed, &c->d_col_idx, &c->d_col_cnt, &c->d_col_off,
+                   &c->d_col_rows, &c->d_adm_state, &c->d_adm_fail, &c->d_adm_counters, &c->d_out, &c->d_codes, &c->d_admit};
   if (c->h_out) cudaFreeHost(c->h_out);
   if (c->h_step) cudaFreeHost(c->h_step);
   if (c->ev_step) cudaEventDestroy(c->ev_step);
@@ -1180,6 +1181,34 @@ static int evaluate_locked(kt_ctx* c, int64_t now, uint32_t flags) {
   return KT_OK;
 }
 
+// ---- per-throttle row lists (kt_admit.cuh ColumnView) ---------------------------------------------------------------
+// Counts, offsets and the scan on the stream, then one read of the total (also the whole off[] when off_host is given); the
+// fill is queued only when `fill_cap` admits the total (a negative fill_cap: always).  v.bitmap, Wp, first, count, idx, k and
+// codes are the caller's; the scratch buffers are the context's grow-only d_col_*, the codes beside the rows.
+static int build_columns(kt_ctx* c, ColumnView& v, int64_t* total, int64_t* off_host, int64_t fill_cap = -1) {
+  v.nblk = (int)((v.count + kColBlock - 1) / kColBlock);
+  KT_CUDA(c, c->d_col_cnt.reserve((size_t)v.nblk * (size_t)v.k * 4 + 16));
+  KT_CUDA(c, c->d_col_off.reserve((size_t)(v.k + 1) * 8 + 16));
+  v.cnt = c->d_col_cnt.as<int32_t>();
+  v.off = c->d_col_off.as<int64_t>();
+  const int64_t warps = (int64_t)v.nblk * ((v.k + 31) / 32);
+  if (warps > 0) k_col_count<<<(unsigned)((warps + 3) / 4), 128, 0, c->stream>>>(v);
+  k_col_lengths<<<(unsigned)((v.k + 255) / 256), 256, 0, c->stream>>>(v);
+  k_col_starts<<<1, 1024, 0, c->stream>>>(v);
+  KT_CUDA(c, cudaGetLastError());
+  if (off_host) KT_CUDA(c, cudaMemcpyAsync(off_host, v.off, (size_t)(v.k + 1) * 8, cudaMemcpyDeviceToHost, c->stream));
+  else KT_CUDA(c, cudaMemcpyAsync(total, v.off + v.k, 8, cudaMemcpyDeviceToHost, c->stream));
+  KT_CUDA(c, cudaStreamSynchronize(c->stream));
+  if (off_host) *total = off_host[v.k];
+  if (fill_cap >= 0 && *total > fill_cap) return KT_OK;
+  KT_CUDA(c, c->d_col_rows.reserve((size_t)*total * (v.codes ? 9 : 8) + 16));
+  v.rows = c->d_col_rows.as<int64_t>();
+  v.codes_out = c->d_col_rows.as<uint8_t>() + (size_t)*total * 8;
+  if (warps > 0 && *total > 0) k_col_fill<<<(unsigned)((warps + 3) / 4), 128, 0, c->stream>>>(v);
+  KT_CUDA(c, cudaGetLastError());
+  return KT_OK;
+}
+
 // ---- queue-ordered greedy admission on the device (kt_admit.cuh) ----------------------------------------------------
 int kt_admit_queue(kt_ctx* c, int64_t first, int64_t count, uint32_t flags, int32_t* rounds_out, int64_t* admitted_out) {
   if (!c || first < 0 || count < 0) return KT_ERR_INVALID;
@@ -1199,27 +1228,18 @@ int kt_admit_queue(kt_ctx* c, int64_t first, int64_t count, uint32_t flags, int3
   AdmitView a{};
   a.first = first; a.count = count; a.req = pend.req.as<int64_t>(); a.present = pend.present.as<uint32_t>(); a.bitmap = pend.bitmap.as<uint32_t>();
   a.n = pend.n; a.Wp = c->ht.Wp; a.W = c->ht.W; a.M = M; a.R = R; a.pre = c->d_pre.as<unsigned char>();
-  a.nblk = (int)((count + kAdmitBlock - 1) / kAdmitBlock);
-  KT_CUDA(c, c->d_adm_cnt2.reserve((size_t)a.nblk * M * 4 + 16));
-  KT_CUDA(c, c->d_adm_off.reserve((size_t)(M + 1) * 4 + 16));
   KT_CUDA(c, c->d_adm_state.reserve((size_t)count + 16));
   KT_CUDA(c, c->d_adm_fail.reserve((size_t)count * 4 + 16));
   KT_CUDA(c, c->d_adm_counters.reserve(16));
-  a.cnt2 = c->d_adm_cnt2.as<int32_t>(); a.tl_off = c->d_adm_off.as<int32_t>(); a.state = c->d_adm_state.as<uint8_t>();
+  a.state = c->d_adm_state.as<uint8_t>();
   a.fail = c->d_adm_fail.as<uint32_t>(); a.counters = c->d_adm_counters.as<uint32_t>();
   a.codes = c->d_codes.as<uint32_t>(); a.admit = c->d_admit.as<unsigned char>();
   // 2. every throttle's toucher list (CSR over the queue, built once)
-  const unsigned warps = (unsigned)a.nblk * (unsigned)a.W;
-  k_admit_count<<<(warps + 3) / 4, 128, 0, c->stream>>>(a);
-  k_admit_lengths<<<(unsigned)((M + 255) / 256), 256, 0, c->stream>>>(a);
-  k_admit_starts<<<1, 1024, 0, c->stream>>>(a);
-  KT_CUDA(c, cudaGetLastError());
-  int32_t nnz = 0;
-  KT_CUDA(c, cudaMemcpyAsync(&nnz, a.tl_off + M, 4, cudaMemcpyDeviceToHost, c->stream));
-  KT_CUDA(c, cudaStreamSynchronize(c->stream));
-  KT_CUDA(c, c->d_adm_pod.reserve((size_t)nnz * 4 + 16));
-  a.tl_pod = c->d_adm_pod.as<int32_t>();
-  k_admit_fill<<<(warps + 3) / 4, 128, 0, c->stream>>>(a);
+  ColumnView v{};
+  v.bitmap = a.bitmap; v.Wp = a.Wp; v.first = first; v.count = count; v.k = M;
+  int64_t nnz = 0;
+  if ((rc = build_columns(c, v, &nnz, nullptr))) return rc;
+  a.tl_off = v.off; a.tl_pod = v.rows;
   KT_CUDA(c, cudaMemsetAsync(a.state, 0, (size_t)count, c->stream));
   // 3. rounds: until a round STARTED with nobody undecided (its loads were exact, and so are the codes it wrote)
   uint32_t counters[2] = {(uint32_t)count, 0};
@@ -1480,6 +1500,34 @@ int kt_get_match_rows(kt_ctx* c, int kind, int64_t k, const int64_t* rows, uint3
   k_gather_rows<<<(unsigned)((k + 7) / 8), 256, 0, c->stream>>>(k, s.t_rows.as<int64_t>(), Wp, s.bitmap.as<uint32_t>(), s.t_words.as<uint32_t>());
   KT_CUDA(c, cudaGetLastError());
   KT_CUDA(c, cudaMemcpyAsync(words, s.t_words.p, (size_t)k * Wp * 4, cudaMemcpyDeviceToHost, c->stream));
+  KT_CUDA(c, cudaStreamSynchronize(c->stream));
+  return KT_OK;
+}
+
+int kt_get_match_columns(kt_ctx* c, int kind, int64_t k, const int32_t* idx, int64_t* off, int64_t* rows, uint8_t* codes, int64_t cap) {
+  if (!c || k < 0 || cap < 0 || !off || (k > 0 && !idx) || (cap > 0 && !rows)) return KT_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(c->mu);
+  if (kind != KT_PODS_RUNNING && kind != KT_PODS_PENDING) return fail(c, KT_ERR_INVALID, "bad pod kind %d", kind);
+  if (kind == KT_PODS_RUNNING && codes) return fail(c, KT_ERR_INVALID, "kt_get_match_columns: codes belong to the pending rows");
+  if (!c->evaluated) return fail(c, KT_ERR_STATE, "kt_get_match_columns before kt_evaluate");
+  for (int64_t j = 0; j < k; ++j)
+    if (idx[j] < 0 || idx[j] >= c->M) return fail(c, KT_ERR_INVALID, "throttle %d out of range [0,%d)", idx[j], c->M);
+  int rc = set_device(c);
+  if (rc) return rc;
+  if ((rc = check_pass_error(c))) return rc;
+  off[0] = 0;
+  if (k == 0) return KT_OK;
+  PodStore& s = c->pods[kind];
+  KT_CUDA(c, c->d_col_idx.reserve((size_t)k * 4 + 16));
+  KT_CUDA(c, cudaMemcpyAsync(c->d_col_idx.p, idx, (size_t)k * 4, cudaMemcpyHostToDevice, c->stream));
+  ColumnView v{};
+  v.bitmap = s.bitmap.as<uint32_t>(); v.Wp = c->ht.Wp; v.first = 0; v.count = s.n; v.idx = c->d_col_idx.as<int32_t>(); v.k = k;
+  v.codes = codes ? c->d_codes.as<uint32_t>() : nullptr;
+  int64_t total = 0;
+  if ((rc = build_columns(c, v, &total, off, cap))) return rc;
+  if (total > cap || total == 0) return KT_OK;  // off[] says how much room the rows need
+  KT_CUDA(c, cudaMemcpyAsync(rows, v.rows, (size_t)total * 8, cudaMemcpyDeviceToHost, c->stream));
+  if (codes) KT_CUDA(c, cudaMemcpyAsync(codes, v.codes_out, (size_t)total, cudaMemcpyDeviceToHost, c->stream));
   KT_CUDA(c, cudaStreamSynchronize(c->stream));
   return KT_OK;
 }

@@ -25,6 +25,11 @@
 #include "kt_json.h"
 #include "kt_quantity.h"
 
+// The host layer is also linked, for CPU tests, against engine test doubles (tests/host_stub) that implement only the calls
+// the rest of this file makes: a weak reference lets such a build load, and kth_affected_pods fails in it.  The product
+// library defines the call in kt_engine.cu, so the reference is always bound there.
+#pragma weak kt_get_match_columns
+
 namespace {
 
 using ktjson::Node;
@@ -1405,22 +1410,8 @@ struct kth_plugin {
     std::vector<char> selector_fails(m, 0);
     for (size_t t = 0; t < m; ++t) {
       const ThrottleObj& o = throttles[t];
-      if (!o.live || o.throttler_name != name || o.selector_error().empty()) continue;
-      // the counted pods a broken term is in the way of: the Throttle's namespace, or -- per term -- the namespaces a
-      // ClusterThrottle term's namespaceSelector matches (clusterthrottle_controller.go:224-270 walks exactly those pods)
-      std::vector<int64_t> ns_rows;
-      std::map<std::string, bool> ns_reaches;
-      for (auto& p : pods) {
-        if (!p.live || !should_count_in(p)) continue;
-        if (o.kind == KT_KIND_THROTTLE) {
-          if (p.ns != o.ns) continue;
-        } else {
-          auto f = ns_reaches.find(p.ns);
-          if (f == ns_reaches.end()) f = ns_reaches.emplace(p.ns, !reachable_selector_error(o, p.ns).empty()).first;
-          if (!f->second) continue;
-        }
-        ns_rows.push_back(p.row);
-      }
+      if (!o.live || o.throttler_name != name) continue;
+      const std::vector<int64_t> ns_rows = selector_error_rows(o);
       if (ns_rows.empty()) continue;  // nobody to ask the selector about: no error
       std::vector<uint32_t> w((size_t)ns_rows.size() * (size_t)Wp);
       check(kt_get_match_rows(ctx, KT_PODS_RUNNING, (int64_t)ns_rows.size(), ns_rows.data(), w.data()), "kt_get_match_rows");
@@ -1515,6 +1506,99 @@ struct kth_plugin {
     return w.out;
   }
 
+  // The counted pods a broken podSelector term of o is in the way of: the Throttle's namespace, or -- per term -- the
+  // namespaces a ClusterThrottle term's namespaceSelector matches (clusterthrottle_controller.go:224-270 walks exactly those
+  // pods).  affectedPods fails when one of them matches none of the valid terms before it (its bit is clear).  Empty when o
+  // has no broken term.
+  std::vector<int64_t> selector_error_rows(const ThrottleObj& o) const {
+    std::vector<int64_t> ns_rows;
+    if (o.selector_error().empty()) return ns_rows;
+    std::map<std::string, bool> ns_reaches;
+    for (auto& p : pods) {
+      if (!p.live || !should_count_in(p)) continue;
+      if (o.kind == KT_KIND_THROTTLE) {
+        if (p.ns != o.ns) continue;
+      } else {
+        auto f = ns_reaches.find(p.ns);
+        if (f == ns_reaches.end()) f = ns_reaches.emplace(p.ns, !reachable_selector_error(o, p.ns).empty()).first;
+        if (!f->second) continue;
+      }
+      ns_rows.push_back(p.row);
+    }
+    return ns_rows;
+  }
+
+  // ---- affectedPods of one throttle (kth_affected_pods) -----------------------------------------------------------
+  // Both relations come from one GIVEN_STATUS pass that reconciles too: the running rows it matches are what a reconcile
+  // would sum, the pending codes are what PreFilter by key would answer.  Its results stay good until some other entry
+  // point runs (every one of them may change the state or run a pass of its own: `epoch`).
+  uint64_t epoch = 1, columns_epoch = 0;
+  void column_of(int kind, int32_t t, std::vector<int64_t>& rows, std::vector<uint8_t>* codes) {
+    if (!kt_get_match_columns) fail("kth_affected_pods: the engine this plugin is linked against has no kt_get_match_columns");
+    int64_t off[2] = {0, 0}, cap = 256;
+    while (true) {
+      rows.resize((size_t)cap);
+      if (codes) codes->resize((size_t)cap);
+      check(kt_get_match_columns(ctx, kind, 1, &t, off, rows.data(), codes ? codes->data() : nullptr, cap), "kt_get_match_columns");
+      if (off[1] <= cap) break;
+      cap = off[1];
+    }
+    rows.resize((size_t)off[1]);
+    if (codes) codes->resize((size_t)off[1]);
+  }
+  std::string affected_pods(const std::string& ns, const std::string& tname) {
+    const std::string key = ns.empty() ? "C:/" + tname : "T:" + ns + "/" + tname;
+    auto it = thr_index.find(key);
+    if (it == thr_index.end()) fail((ns.empty() ? "clusterthrottle " : "throttle ") + ns + "/" + tname + " not found");
+    const ThrottleObj& found = throttles[(size_t)it->second];
+    if (found.throttler_name != name) fail(found.nn() + " belongs to throttler \"" + found.throttler_name + "\", not to \"" + name + "\"");
+    if (columns_epoch != epoch) {
+      run_pending_pass({}, 0, 0);
+      columns_epoch = epoch;
+    }
+    const size_t t = (size_t)thr_index.at(key);  // (the pass may have laid the columns out anew)
+    std::vector<int64_t> run_rows, pend_rows;
+    std::vector<uint8_t> codes;
+    column_of(KT_PODS_RUNNING, (int32_t)t, run_rows, nullptr);
+    column_of(KT_PODS_PENDING, (int32_t)t, pend_rows, &codes);
+    const ThrottleObj& o = throttles[t];
+    // a counted pod that reaches a broken term: affectedPods returns that error (throttle_controller.go:233-236); the first such
+    // pod in informer order names it
+    const std::vector<int64_t> err_rows = selector_error_rows(o);
+    if (!err_rows.empty()) {
+      const PodObj* first = nullptr;
+      for (int64_t r : err_rows)
+        if (!std::binary_search(run_rows.begin(), run_rows.end(), r) && (!first || pods[(size_t)r].seq < first->seq)) first = &pods[(size_t)r];
+      if (first) fail(reachable_selector_error(o, first->ns));
+    }
+    auto by_key = [](const PodObj* a, const PodObj* b) { return a->ns != b->ns ? a->ns < b->ns : a->name < b->name; };
+    std::vector<const PodObj*> running, finished;
+    for (int64_t r : run_rows) {
+      const PodObj& p = pods[(size_t)r];
+      ((pod_flags(p) & KT_POD_NOT_FINISHED) ? running : finished).push_back(&p);
+    }
+    std::vector<std::pair<const PodObj*, uint8_t>> queued;
+    for (size_t i = 0; i < pend_rows.size(); ++i) {
+      const int64_t r = pend_rows[i];
+      // (free queue rows are tombstones, which a selector without requirements still matches on the pending side; scratch
+      // rows hold manifests, not queued pods)
+      if (r < (int64_t)pend_pod.size() && pend_pod[(size_t)r] >= 0) queued.emplace_back(&pods[(size_t)pend_pod[(size_t)r]], codes[i]);
+    }
+    std::sort(running.begin(), running.end(), by_key);
+    std::sort(finished.begin(), finished.end(), by_key);
+    std::sort(queued.begin(), queued.end(), [&](const auto& a, const auto& b) { return by_key(a.first, b.first); });
+    static const char* const kStatus[4] = {"not-throttled", "active", "insufficient", "pod-requests-exceeds-threshold"};
+    Writer w;
+    w.begin_obj().key("pods").begin_arr();
+    for (const PodObj* p : running) w.str(p->nn());
+    w.end_arr().key("terminatedPods").begin_arr();
+    for (const PodObj* p : finished) w.str(p->nn());
+    w.end_arr().key("queued").begin_arr();
+    for (auto& q : queued) w.begin_obj().key("pod").str(q.first->nn()).key("status").str(kStatus[q.second & 3u]).end_obj();
+    w.end_arr().end_obj();
+    return w.out;
+  }
+
   // ---- pending pods: one device pass for a batch ----------------------------------------------------------
   struct RowView {  // one pending pod's share of a pass: affectedThrottles row, 2-bit check codes, admit bit
     const uint32_t* bitmap;
@@ -1579,7 +1663,8 @@ struct kth_plugin {
   }
   // One pass over the PENDING table (queue + scratch rows): PreFilter reads the informer copy of .status; reconcile is a
   // separate event (KT_EVAL_GIVEN_STATUS).  Afterwards the device holds the verdicts of every queue row at this state.
-  void run_pending_pass(const std::vector<PodObj>& batch, uint32_t extra_flags) {
+  // (kth_affected_pods asks for skip = 0: the running relation of the same state as well)
+  void run_pending_pass(const std::vector<PodObj>& batch, uint32_t extra_flags, uint32_t skip = KT_EVAL_SKIP_RECONCILE) {
     const bool tables_change = throttles_dirty || namespaces_dirty;
     sync_all();
     sync_status();
@@ -1587,7 +1672,7 @@ struct kth_plugin {
     if (tables_change) queue.valid = false;
     sync_pending(batch);
     if (throttles.empty()) return;
-    check(kt_evaluate(ctx, 0, KT_EVAL_GIVEN_STATUS | KT_EVAL_SKIP_RECONCILE | extra_flags), "kt_evaluate");
+    check(kt_evaluate(ctx, 0, KT_EVAL_GIVEN_STATUS | skip | extra_flags), "kt_evaluate");
   }
   // Bring the host copy of the queue's verdicts up to date (admit bits, affectedThrottles rows, non-zero check codes).
   void fetch_queue_results() {
@@ -2347,10 +2432,11 @@ struct kth_plugin {
 
 namespace {
 
-template <class F>
+template <bool kReadsOnly = false, class F>
 const char* guarded(kth_plugin* p, F&& f) {
   if (!p) return ret(err_json("null plugin handle"));
   std::lock_guard<std::mutex> lk(p->mu);
+  if (!kReadsOnly) ++p->epoch;  // may change the state or run a pass: kth_affected_pods' last pass no longer answers
   try {
     return ret(f());
   } catch (const std::exception& e) {
@@ -2556,6 +2642,7 @@ int64_t kth_queue_row(kth_plugin* p, const char* ns, const char* name) {
 int64_t kth_pre_filter_queue(kth_plugin* p, uint8_t* verdicts, int64_t cap) {
   if (!p || cap < 0 || (cap > 0 && !verdicts)) return -1;
   std::lock_guard<std::mutex> lk(p->mu);
+  ++p->epoch;
   try {
     return p->pre_filter_queue(verdicts, cap);
   } catch (const std::exception& e) {
@@ -2628,6 +2715,9 @@ const char* kth_unreserve(kth_plugin* p, const char* pod_json) {
 }
 const char* kth_reserved(kth_plugin* p, int kind, const char* throttle_nn) {
   return guarded(p, [&]() { return p->reserved_json(kind, throttle_nn ? throttle_nn : ""); });
+}
+const char* kth_affected_pods(kth_plugin* p, const char* ns, const char* name) {
+  return guarded<true>(p, [&]() { return p->affected_pods(ns ? ns : "", name ? name : ""); });
 }
 const char* kth_metrics(kth_plugin* p) {
   return guarded(p, [&]() -> std::string {

@@ -26,7 +26,7 @@ def _bind(L=None):
     L.kth_free.argtypes = [vp]
     L.kth_free.restype = None
     for name, args in (("kth_apply", [vp, cp]), ("kth_delete", [vp, cp, cp, cp]), ("kth_reconcile_all", [vp, cp]),
-                       ("kth_get_status", [vp, cp, cp]), ("kth_get_status_manifest", [vp, cp, cp]), ("kth_pre_filter", [vp, cp]), ("kth_pre_filter_batch", [vp, cp]),
+                       ("kth_get_status", [vp, cp, cp]), ("kth_get_status_manifest", [vp, cp, cp]), ("kth_affected_pods", [vp, cp, cp]), ("kth_pre_filter", [vp, cp]), ("kth_pre_filter_batch", [vp, cp]),
                        ("kth_admit_queue", [vp, cp]), ("kth_pre_filter_key", [vp, cp, cp]), ("kth_reserve_key", [vp, cp, cp]), ("kth_unreserve_key", [vp, cp, cp]),
                        ("kth_queue_stats", [vp]), ("kth_reserve", [vp, cp]), ("kth_unreserve", [vp, cp]), ("kth_reserved", [vp, C.c_int, cp]), ("kth_metrics", [vp]), ("kth_eval", [cp])):
         fn = getattr(L, name)
@@ -44,7 +44,7 @@ def _bind(L=None):
 
 
 HOST_EXPORTS = ["kth_new_plugin", "kth_new_plugin_error", "kth_free", "kth_apply", "kth_delete", "kth_reconcile_all", "kth_get_status", "kth_get_status_manifest",
-                "kth_pre_filter", "kth_pre_filter_key", "kth_reserve_key", "kth_unreserve_key", "kth_pre_filter_queue", "kth_queue_row", "kth_pod_row", "kth_queue_stats", "kth_last_error", "kth_pre_filter_batch", "kth_admit_queue", "kth_reserve", "kth_unreserve", "kth_reserved", "kth_metrics", "kth_eval"]
+                "kth_pre_filter", "kth_pre_filter_key", "kth_reserve_key", "kth_unreserve_key", "kth_pre_filter_queue", "kth_queue_row", "kth_pod_row", "kth_queue_stats", "kth_last_error", "kth_pre_filter_batch", "kth_admit_queue", "kth_reserve", "kth_unreserve", "kth_reserved", "kth_metrics", "kth_eval", "kth_affected_pods"]
 
 
 def _result(raw):
@@ -104,6 +104,11 @@ class Plugin:
         raw = self._L.kth_get_status_manifest(self._h, namespace.encode(), name.encode()).decode()
         _result(raw.encode())  # raises on {"error": ...}
         return raw
+
+    def affected_pods(self, name, namespace=""):
+        """affectedPods of a Throttle (namespace given) or ClusterThrottle: {"pods": [...], "terminatedPods": [...],
+        "queued": [{"pod": "ns/name", "status": ...}, ...]}, each sorted by namespace, then name."""
+        return _result(self._L.kth_affected_pods(self._h, namespace.encode(), name.encode()))
 
     # plugin
     def prefilter(self, pod):
