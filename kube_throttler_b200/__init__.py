@@ -85,6 +85,7 @@ def lib():
         L.kt_step_wait.argtypes = [vp, C.POINTER(abi.StepResult)]
         L.kt_admit_queue.argtypes = [vp, C.c_int64, C.c_int64, C.c_uint32, C.POINTER(C.c_int32), C.POINTER(C.c_int64)]
         L.kt_get_check_rows.argtypes = [vp, C.c_int64, vp, vp, vp]
+        L.kt_get_match_rows.argtypes = [vp, C.c_int, C.c_int64, vp, vp]
         L.kt_get_changed.argtypes = [vp, vp, C.c_int64, C.POINTER(C.c_int64), vp]
         L.kt_get_reconcile_rows.argtypes = [vp, C.c_int64, vp, C.POINTER(abi.ReconcileOut)]
         L.kt_update_pod_rows.argtypes = [vp, C.c_int, C.c_int64, vp, vp, vp, vp, vp, vp]
@@ -339,6 +340,13 @@ class Engine:
         admit = np.zeros(rows.shape[0], np.uint8)
         self._ck(self._L.kt_get_check_rows(self._h, rows.shape[0], abi.ptr(rows), abi.ptr(codes), abi.ptr(admit)))
         return codes, admit
+
+    def match_rows(self, kind: int, rows: np.ndarray) -> np.ndarray:
+        """words[k][words_per_row]: the match bitmap rows of the listed rows of a kind, gathered on the device."""
+        rows = np.ascontiguousarray(rows, np.int64)
+        words = np.zeros((rows.shape[0], self.words_per_row), np.uint32)
+        self._ck(self._L.kt_get_match_rows(self._h, kind, rows.shape[0], abi.ptr(rows), abi.ptr(words)))
+        return words
 
     def match_columns(self, kind: int, idx, cap: Optional[int] = None):
         """affectedPods from the throttles' side: (off[k+1], rows, codes) with throttle idx[j]'s rows, ascending, in
