@@ -12,6 +12,7 @@
 #include <cstring>
 #include <mutex>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/kt_b200.h"
@@ -154,7 +155,6 @@ struct kt_ctx {
   bool plan_forced = false;
   kt_pass_plan ran{};             // what the last fused pass launched (kt_debug_get_pass_plan)
   bool have_ran = false;
-  bool fused = true;  // one-launch pass (k_pass) when the whole pass is asked for; three PDL-chained kernels otherwise
   DevBuf d_changed;  // device-side status diff: {count[2] u32 by pass parity, pad to 16 B, idx[M] i32, flag[M] u8}
   unsigned diff_parity = 0;
   bool have_diff = false;  // the last pass produced a diff (an observed status was uploaded)
@@ -196,13 +196,6 @@ struct kt_ctx {
   unsigned epoch = 0;         // passes exchanged through the window so far
   bool win_stale = false;     // the throttle set changed: the window's buffers are laid out for another M -> rebuilt (collectively) before the next pass
 };
-
-#ifndef KT_WIDE_TILES  // 1: ClusterThrottle-heavy tables run the pass with 256-pod tiles
-#define KT_WIDE_TILES 1
-#endif
-#ifndef KT_PASS_PDL  // 1: k_pass is launched with programmatic stream serialization (its launch overlaps the previous kernel's tail)
-#define KT_PASS_PDL 1
-#endif
 
 namespace {
 
@@ -428,9 +421,6 @@ cudaError_t launch(kt_ctx* c, void (*kern)(KArgs...), unsigned blocks, unsigned 
   return cudaLaunchKernelEx(&cfg, kern, KArgs(args)...);
 }
 
-// Kernel variant dispatch.  Fast family (label rows in registers): L <= 8 and counter bits B = 2, with the
-// register accumulators sized for R <= 4 / R <= 8.  General family (rows in shared memory, shared-memory
-// accumulation): any L <= 32, R <= 31, B in {2, 6}.  Both come for 1 or 2 term planes per table entry.
 int reconcile_slots(const kt_ctx* c) {
   int s = c->ht.max_ns_words + 2;  // a tile usually spans one or two namespaces
   if (s < 4) s = 4;
@@ -508,48 +498,43 @@ cudaError_t launch_pass(kt_ctx* c, const PassArgs& a0) {
   kt_pass_plan& ran = c->ran;
   ran = kt_pass_plan{deep ? kPassThreadsDeep : kPassThreadsShallow, a.quad ? KT_PLAN_DECIDE_QUAD : KT_PLAN_DECIDE_PER_POD, fp.max_ctas, grid, capacity,
                      TILE, TPC, B, RT, a.n_chk, a.n_rec, a.n_fin, a.n_sub};
-  return deep ? launch(c, k_pass<TPC, B, RT, REG, TILE, kPassThreadsDeep>, grid, TILE, smem, /*pdl=*/KT_PASS_PDL != 0, a)
-              : launch(c, k_pass<TPC, B, RT, REG, TILE, kPassThreadsShallow>, grid, TILE, smem, /*pdl=*/KT_PASS_PDL != 0, a);
+  return deep ? launch(c, k_pass<TPC, B, RT, REG, TILE, kPassThreadsDeep>, grid, TILE, smem, /*pdl=*/true, a)
+              : launch(c, k_pass<TPC, B, RT, REG, TILE, kPassThreadsShallow>, grid, TILE, smem, /*pdl=*/true, a);
+}
+// The kernel variant, chosen here for every launch: TPC term planes per table entry (1 or 2), B counter bits (2 or 6), RT the
+// compile-time bound on R of the register accumulators (0: accumulate in shared memory), REG label rows in registers.  `go`
+// is called with one std::integral_constant per template argument.
+//   Fast family (REG, RT = 4 for R <= 4, else 8): L <= 8, B = 2 and R <= 8.  General family: any L <= 32, R <= 31, B in {2, 6}.
+//   `check`: the check keeps no per-resource registers, so it takes register rows whenever L <= 8 and B = 2, whatever R is --
+//   with R > 8 a register-row check runs beside a general reconcile (RT means nothing to it).
+template <class Go>
+cudaError_t with_variant(const kt_ctx* c, bool check, Go&& go) {
+  using B2 = std::integral_constant<int, 2>;
+  using B6 = std::integral_constant<int, 6>;
+  const bool t1 = c->ht.TPpad == 1, b2 = c->ht.B <= 2;
+  const int R = c->lim.n_resources;
+  auto by_tpc = [&](auto b, auto rt, auto reg) {
+    return t1 ? go(std::integral_constant<int, 1>{}, b, rt, reg) : go(std::integral_constant<int, 2>{}, b, rt, reg);
+  };
+  if (c->lim.label_slots <= 8 && b2 && (check || R <= 8))
+    return R <= 4 ? by_tpc(B2{}, std::integral_constant<int, 4>{}, std::true_type{}) : by_tpc(B2{}, std::integral_constant<int, 8>{}, std::true_type{});
+  return b2 ? by_tpc(B2{}, std::integral_constant<int, 0>{}, std::false_type{}) : by_tpc(B6{}, std::integral_constant<int, 0>{}, std::false_type{});
 }
 cudaError_t dispatch_pass(kt_ctx* c, const PassArgs& a) {
-  const bool t1 = c->ht.TPpad == 1, b2 = c->ht.B <= 2;
-  const int R = c->lim.n_resources;
-  const bool fast = c->lim.label_slots <= 8 && b2 && R <= 8;
   // ClusterThrottle-heavy tables (a namespace's word list is long): 256 pods share a CTA's accumulator slots
-  const bool wide = KT_WIDE_TILES != 0 && a.S >= 8 && kTileReconcile == 128;
-  if (fast) {
-    if (wide) {
-      if (t1) return R <= 4 ? launch_pass<1, 2, 4, true, 256>(c, a) : launch_pass<1, 2, 8, true, 256>(c, a);
-      return R <= 4 ? launch_pass<2, 2, 4, true, 256>(c, a) : launch_pass<2, 2, 8, true, 256>(c, a);
+  const bool wide = a.S >= 8;
+  return with_variant(c, false, [&](auto tpc, auto b, auto rt, auto reg) {
+    if constexpr (reg) {
+      if (wide) return launch_pass<tpc, b, rt, reg, 256>(c, a);
     }
-    if (t1) return R <= 4 ? launch_pass<1, 2, 4, true, kTileReconcile>(c, a) : launch_pass<1, 2, 8, true, kTileReconcile>(c, a);
-    return R <= 4 ? launch_pass<2, 2, 4, true, kTileReconcile>(c, a) : launch_pass<2, 2, 8, true, kTileReconcile>(c, a);
-  }
-  if (t1 && b2) return launch_pass<1, 2, 0, false, kTileReconcile>(c, a);
-  if (t1) return launch_pass<1, 6, 0, false, kTileReconcile>(c, a);
-  if (b2) return launch_pass<2, 2, 0, false, kTileReconcile>(c, a);
-  return launch_pass<2, 6, 0, false, kTileReconcile>(c, a);
+    return launch_pass<tpc, b, rt, reg, kTileReconcile>(c, a);
+  });
 }
 cudaError_t dispatch_reconcile(kt_ctx* c, const PodView& pv, const TableView& tb, unsigned long long* part, unsigned blocks) {
-  const bool t1 = c->ht.TPpad == 1, b2 = c->ht.B <= 2;
-  const int R = c->lim.n_resources;
-  const bool fast = c->lim.label_slots <= 8 && b2 && R <= 8;
-  if (fast) {
-    if (t1) return R <= 4 ? launch_reconcile<1, 2, 4, true>(c, pv, tb, part, blocks) : launch_reconcile<1, 2, 8, true>(c, pv, tb, part, blocks);
-    return R <= 4 ? launch_reconcile<2, 2, 4, true>(c, pv, tb, part, blocks) : launch_reconcile<2, 2, 8, true>(c, pv, tb, part, blocks);
-  }
-  if (t1 && b2) return launch_reconcile<1, 2, 0, false>(c, pv, tb, part, blocks);
-  if (t1) return launch_reconcile<1, 6, 0, false>(c, pv, tb, part, blocks);
-  if (b2) return launch_reconcile<2, 2, 0, false>(c, pv, tb, part, blocks);
-  return launch_reconcile<2, 6, 0, false>(c, pv, tb, part, blocks);
+  return with_variant(c, false, [&](auto tpc, auto b, auto rt, auto reg) { return launch_reconcile<tpc, b, rt, reg>(c, pv, tb, part, blocks); });
 }
 cudaError_t dispatch_check(kt_ctx* c, const PodView& pv, const TableView& tb, const PartExchange& px, unsigned blocks, bool pdl) {
-  const bool t1 = c->ht.TPpad == 1, b2 = c->ht.B <= 2;
-  if (c->lim.label_slots <= 8 && b2) return t1 ? launch_check<1, 2, true>(c, pv, tb, px, blocks, pdl) : launch_check<2, 2, true>(c, pv, tb, px, blocks, pdl);
-  if (t1 && b2) return launch_check<1, 2, false>(c, pv, tb, px, blocks, pdl);
-  if (t1) return launch_check<1, 6, false>(c, pv, tb, px, blocks, pdl);
-  if (b2) return launch_check<2, 2, false>(c, pv, tb, px, blocks, pdl);
-  return launch_check<2, 6, false>(c, pv, tb, px, blocks, pdl);
+  return with_variant(c, true, [&](auto tpc, auto b, auto, auto reg) { return launch_check<tpc, b, reg>(c, pv, tb, px, blocks, pdl); });
 }
 
 }  // namespace
@@ -1073,7 +1058,7 @@ static int evaluate_locked(kt_ctx* c, int64_t now, uint32_t flags) {
   // ---- the whole pass in one launch (k_pass), both halves asked for.  With several ranks the all-reduce happens
   // inside it: finalize tiles add this rank's partial sums into every rank's totals over NVLink (exchange windows). ----
   const bool multi = c->comm && c->nranks > 1;
-  const bool whole = c->fused && !tm && do_rec && do_chk && M > 0 && run.n > 0 && pend.n > 0;
+  const bool whole = !tm && do_rec && do_chk && M > 0 && run.n > 0 && pend.n > 0;
   if (whole && multi) {
     if ((rc = ensure_window(c, (size_t)(2 * R + 1) * M * 8))) return rc;
     if (!c->p2p_failed) {

@@ -31,38 +31,16 @@
 
 namespace kt {
 
-#ifndef KT_TILE_RECONCILE
-#define KT_TILE_RECONCILE 128
-#endif
-// ---- experiment switches (tools/sweep_variants.sh builds one library per setting; A/B on the same box) ----
-#ifndef KT_WAIT_MODE       // how a wait acquires: 0 relaxed polls + acquire fence, 1 relaxed polls + one acquire load, 2 acquire polls
-#define KT_WAIT_MODE 1
-#endif
 // Resident threads per SM the fused pass is compiled for (register cap = 65536 / this).  Both are built; launch_pass picks one from
 // the shape: 512 (128 registers, no spills) for passes whose tiles are a few rounds of the grid, where the chain after the last
 // reconcile tile is the time; 768 (80 registers) for passes many rounds deep, whose reconcile tiles stream better with 24 warps
 // per SM than with 16 (C5).
 constexpr int kPassThreadsShallow = 512, kPassThreadsDeep = 768;
-#ifndef KT_SLOT_CAP        // upper bound on the per-CTA accumulator slots (shared memory vs straight-to-HBM atomics)
-#define KT_SLOT_CAP 32
-#endif
-#ifndef KT_HEAVY_PODS
-#define KT_HEAVY_PODS 6
-#endif
-constexpr int kTileReconcile = KT_TILE_RECONCILE;  // running pods per CTA (one lane per pod)
+constexpr int kTileReconcile = 128;  // running pods per CTA (one lane per pod)
 constexpr int kTileCheck = 64;       // pending pods per CTA
-constexpr int kMaxSlots = KT_SLOT_CAP;        // upper bound on the per-CTA accumulator slots (one per distinct 32-throttle word)
+constexpr int kMaxSlots = 32;        // upper bound on the per-CTA accumulator slots (one per distinct 32-throttle word)
 constexpr uint32_t kFull = 0xffffffffu;
-#ifndef KT_STAGE_CHUNK
-#define KT_STAGE_CHUNK 4
-#endif
-constexpr int kStageChunk = KT_STAGE_CHUNK;  // resources whose pre-record values and sums a decide lane requests together
-#ifndef KT_EVAL_PAIR  // 1: a lane's first two words are evaluated with their table gathers interleaved (eval_word2).  Measured
-#define KT_EVAL_PAIR 0  // measured slower at the 80-register cap of the fused pass at 768 threads per SM (spills) -- off
-#endif
-#ifndef KT_DECIDE_UNROLLED
-#define KT_DECIDE_UNROLLED 0
-#endif
+constexpr int kStageChunk = 4;       // resources whose pre-record values and sums a decide lane requests together
 constexpr int kPropose = 4;          // words a warp of a decide tile may propose to its CTA's staging table per round
 constexpr int kTraceRow = 32;        // u64 per traced tile of the optional in-kernel trace: {ticket, sm, t_start, t_end, 12 stage stamps (globaltimer ns),
                                      // 12 cycle counts, CTA, CTA exit}
@@ -78,7 +56,7 @@ __host__ __device__ inline uint32_t winfo_pack(int cnt, int w0, int w1, int W) {
   if (W > 4096) return kWinfoList << 24;
   return (uint32_t)(w0 & 0xfff) | ((uint32_t)(w1 & 0xfff) << 12) | ((uint32_t)(cnt > 254 ? 254 : cnt) << 24);
 }
-constexpr int kHeavyPods = KT_HEAVY_PODS;        // a throttle matching more pods of a warp than this is summed by the whole warp
+constexpr int kHeavyPods = 6;        // a throttle matching more pods of a warp than this is summed by the whole warp
 
 struct PodView {
   const int64_t* labels;    // [Lpad][n] keyId<<32 | valId (the snapshot as uploaded; re-translated when the tables change)
@@ -122,24 +100,12 @@ struct WordCursor {
       cnt = __ldg(&tb.nsw_off[ns + 1]) - lo;
     }
   }
-  __device__ __forceinline__ int at_inline0() const { return inl > 0 ? w0 : 0x40000000 + lo; }  // a per-namespace key for clustering tests
   __device__ __forceinline__ int at(const TableView& tb, int k) const {
     if (k >= cnt) return 0x7fffffff;
     if (k < inl) return k == 0 ? w0 : w1;
     return __ldg(&tb.nsw_idx[lo + k]);
   }
 };
-
-#ifndef KT_SCATTER_WORDS  // a warp whose lanes start in more distinct words than this takes the per-lane paths
-#define KT_SCATTER_WORDS 32  // 32 = never: measured slower than the rounds at C2 in arrival order; the product keeps rows clustered (kt_host.cc row arenas)
-#endif
-// Do the lanes of this warp live in many different namespaces (rows in arrival order)?  Judged by their first words.
-__device__ __forceinline__ bool warp_is_scattered(const WordCursor& wc) {
-  const int key = wc.cnt > 0 ? wc.at_inline0() : -1;
-  const unsigned same = __match_any_sync(kFull, key);
-  const bool leader = key >= 0 && (__ffs(same) - 1) == (int)(threadIdx.x & 31);
-  return __popc(__ballot_sync(kFull, leader)) > KT_SCATTER_WORDS;
-}
 
 // Per-throttle constants of the 4-step check, produced by k_finalize, gathered per matched pair.
 // Followed in memory by int64 thrv[R] (S1 thresholds) and int64 head[R] (S4: threshold - used - reserved).
@@ -230,34 +196,12 @@ __device__ __forceinline__ unsigned ld_relaxed_gpu(const unsigned* p) {
   asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
   return v;
 }
-__device__ __forceinline__ unsigned ld_relaxed_sys(const unsigned* p) {
-  unsigned v;
-  asm volatile("ld.relaxed.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-  return v;
-}
 __device__ __forceinline__ unsigned ld_acquire_gpu(const unsigned* p) {
   unsigned v;
   asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
   return v;
 }
-__device__ __forceinline__ unsigned ld_acquire_sys(const unsigned* p) {
-  unsigned v;
-  asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-  return v;
-}
 __device__ __forceinline__ void fence_acquire_gpu() { asm volatile("fence.acq_rel.gpu;" ::: "memory"); }
-__device__ __forceinline__ void fence_acquire_sys() { asm volatile("fence.acq_rel.sys;" ::: "memory"); }
-// One poll of a counter, and what closes a successful wait, per KT_WAIT_MODE.
-__device__ __forceinline__ unsigned poll_gpu(const unsigned* p) { return KT_WAIT_MODE == 2 ? ld_acquire_gpu(p) : ld_relaxed_gpu(p); }
-__device__ __forceinline__ unsigned poll_sys(const unsigned* p) { return KT_WAIT_MODE == 2 ? ld_acquire_sys(p) : ld_relaxed_sys(p); }
-__device__ __forceinline__ void acquire_gpu(const unsigned* p) {
-  if (KT_WAIT_MODE == 0) fence_acquire_gpu();
-  else if (KT_WAIT_MODE == 1) (void)ld_acquire_gpu(p);
-}
-__device__ __forceinline__ void acquire_sys(const unsigned* p) {
-  if (KT_WAIT_MODE == 0) fence_acquire_sys();
-  else if (KT_WAIT_MODE == 1) (void)ld_acquire_sys(p);
-}
 __device__ __forceinline__ void cta_signal(unsigned* counter) {
   __syncthreads();
   if (threadIdx.x == 0) {
@@ -290,8 +234,8 @@ __device__ __forceinline__ void spin_until(Done done, unsigned* error_flag, unsi
 }
 __device__ __forceinline__ void cta_wait_at_least(const unsigned* counter, unsigned target, unsigned* error_flag) {
   if (threadIdx.x == 0) {
-    spin_until([&] { return poll_gpu(counter) >= target; }, error_flag, 40);
-    acquire_gpu(counter);  // the counter only grows within a pass: an acquire load here reads a value >= target
+    spin_until([&] { return ld_relaxed_gpu(counter) >= target; }, error_flag, 40);
+    (void)ld_acquire_gpu(counter);  // the counter only grows within a pass: an acquire load here reads a value >= target
   }
   __syncthreads();
 }
@@ -564,80 +508,6 @@ __device__ __forceinline__ uint32_t eval_word(const TableView& tb, const PodRows
   return result;
 }
 
-// The first two words of a lane together: the table gathers of BOTH words for four labels at a time are in flight before any
-// of them is folded -- two words cost the latency of one (eval_word twice serialises them: the second word's loads only issue
-// after the first word's folds have consumed theirs).  Register-row family only (L <= 8).
-template <int TPC, int B>
-__device__ __forceinline__ void eval_word2(const TableView& tb, const PodRows<true>& rows, int ns, int w0, int w1, uint32_t& m0, uint32_t& m1) {
-  const uint32_t row_bytes = (uint32_t)tb.TPpad * 8u;
-  const int ws[2] = {w0, w1};
-  const unsigned char* wbase[2];
-  const uint32_t* nsm[2];
-  const uint32_t* need[2];
-#pragma unroll
-  for (int z = 0; z < 2; ++z) {
-    wbase[z] = reinterpret_cast<const unsigned char*>(tb.table) + (size_t)ws[z] * tb.rows * row_bytes;
-    nsm[z] = tb.nsmask + ((size_t)ns * tb.W + ws[z]) * tb.TPpad;
-    need[z] = tb.need + (size_t)ws[z] * tb.TPpad * B;
-  }
-  uint32_t result[2] = {0u, 0u};
-#pragma unroll 1
-  for (int s0 = 0; s0 < tb.TPpad; s0 += TPC) {
-    uint32_t sat[2][TPC], cnt[2][TPC][B];
-#pragma unroll
-    for (int z = 0; z < 2; ++z)
-#pragma unroll
-      for (int s = 0; s < TPC; ++s) {
-        sat[z][s] = __ldg(&nsm[z][s0 + s]);
-#pragma unroll
-        for (int b = 0; b < B; ++b) cnt[z][s][b] = 0;
-      }
-#pragma unroll
-    for (int half = 0; half < 2; ++half) {
-      uint32_t v[2][4][TPC * 2];
-#pragma unroll
-      for (int z = 0; z < 2; ++z)
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const unsigned char* e = wbase[z] + rows.off[half * 4 + i] + s0 * 8;
-          if constexpr (TPC == 2) {
-            const uint4 q = __ldg(reinterpret_cast<const uint4*>(e));
-            v[z][i][0] = q.x; v[z][i][1] = q.y; v[z][i][2] = q.z; v[z][i][3] = q.w;
-          } else {
-            const uint2 q = __ldg(reinterpret_cast<const uint2*>(e));
-            v[z][i][0] = q.x; v[z][i][1] = q.y;
-          }
-        }
-#pragma unroll
-      for (int z = 0; z < 2; ++z)
-#pragma unroll
-        for (int i = 0; i < 4; ++i)
-#pragma unroll
-          for (int s = 0; s < TPC; ++s) {
-            sat[z][s] &= v[z][i][2 * s];
-            uint32_t carry = v[z][i][2 * s + 1];  // ripple-add one bit into the bit-sliced counter
-#pragma unroll
-            for (int b = 0; b < B; ++b) {
-              const uint32_t t = cnt[z][s][b] & carry;
-              cnt[z][s][b] ^= carry;
-              carry = t;
-            }
-          }
-    }
-#pragma unroll
-    for (int z = 0; z < 2; ++z)
-#pragma unroll
-      for (int s = 0; s < TPC; ++s) {
-        uint32_t m = sat[z][s];
-#pragma unroll
-        for (int b = 0; b < B; ++b) m &= ~(cnt[z][s][b] ^ __ldg(&need[z][(s0 + s) * B + b]));
-        result[z] |= m;
-      }
-  }
-  m0 = result[0];
-  m1 = result[1];
-}
-
 // 32x32 bit-matrix transpose across the warp: in = lane l holds row l; out = lane b holds column b.
 __device__ __forceinline__ uint32_t warp_transpose32(uint32_t x, int lane) {
   uint32_t m = 0x0000ffffu;
@@ -662,12 +532,6 @@ __device__ __forceinline__ unsigned long long warp_sum_u64(unsigned long long v)
 // ---- bulk asynchronous copies (TMA engine, no tensor map: cp.async.bulk) completing on an mbarrier --------------------------
 // One elected lane arms the barrier with the byte count and issues the copies; the data lands in shared memory without passing
 // through anybody's registers and the consumers sleep on the barrier's phase instead of a scoreboard.  SASS: UBLKCP / SYNCS.
-#ifndef KT_BULK_ROWS  // 1: a reconcile tile's column slices (row offsets, requests, flags ...) are staged with bulk copies; 0: per-lane LDG.
-#define KT_BULK_ROWS 0  // measured slower at C2, C2 x10 and C4 (sixteen 0.5-1 KB copies per tile) -- off
-#endif
-#ifndef KT_SMEM_ADD32  // 1: 64-bit shared-memory accumulator adds as two native 32-bit atomics with a carry; 0: atomicAdd(u64) (a CAS loop)
-#define KT_SMEM_ADD32 1
-#endif
 __device__ __forceinline__ uint32_t smem_addr(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(unsigned long long* bar, unsigned count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_addr(bar)), "r"(count) : "memory");
@@ -705,29 +569,21 @@ constexpr int kMaxWarps = 8;  // of a pass CTA (TILE <= 256)
 // loop (ATOMS.CAST.SPIN); two native 32-bit adds do the same mod 2^64: the low add returns the old low word, which tells
 // whether THIS add carried, and the carry travels with the high word.  (The halves are only read together after a barrier.)
 __device__ __forceinline__ void smem_add_u64(unsigned long long* acc, unsigned long long v) {
-  if constexpr (KT_SMEM_ADD32 != 0) {
-    unsigned* w = reinterpret_cast<unsigned*>(acc);
-    const unsigned lo = (unsigned)v;
-    unsigned hi = (unsigned)(v >> 32);
-    if (lo) {
-      const unsigned old = atomicAdd(w, lo);
-      hi += (old + lo) < old ? 1u : 0u;
-    }
-    if (hi) atomicAdd(w + 1, hi);
-  } else {
-    atomicAdd(acc, v);
+  unsigned* w = reinterpret_cast<unsigned*>(acc);
+  const unsigned lo = (unsigned)v;
+  unsigned hi = (unsigned)(v >> 32);
+  if (lo) {
+    const unsigned old = atomicAdd(w, lo);
+    hi += (old + lo) < old ? 1u : 0u;
   }
+  if (hi) atomicAdd(w + 1, hi);
 }
 
 // Shared-memory carve-up of k_reconcile (host and device must agree).  S = accumulator slots.
-constexpr int kStageCols = 12;  // u32 columns of a bulk-staged tile: 8 row offsets, winfo, flags, ns, present
-__host__ __device__ inline size_t reconcile_stage_offset(int L, int R, int S, bool reg_rows, int tile) {
+__host__ __device__ inline size_t reconcile_smem_bytes(int L, int R, int S, bool reg_rows, int tile) {
   const size_t b = (size_t)R * tile * 8 + (size_t)S * R * 32 * 8 + (reg_rows ? 0 : (size_t)((L + 7) & ~7) * tile * 4) + (size_t)tile * 4 + (size_t)S * 32 * 4 * 2 +
                    (size_t)S * 4;
   return (b + 15) & ~(size_t)15;
-}
-__host__ __device__ inline size_t reconcile_smem_bytes(int L, int R, int S, bool reg_rows, int tile) {
-  return reconcile_stage_offset(L, R, S, reg_rows, tile) + (KT_BULK_ROWS != 0 && reg_rows ? (size_t)kStageCols * tile * 4 : 0);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -740,9 +596,7 @@ __host__ __device__ inline size_t reconcile_smem_bytes(int L, int R, int S, bool
 template <int TPC, int B, int RT, bool REG, int TILE = kTileReconcile>
 __device__ __forceinline__ void reconcile_tile(const PodView& pods, const TableView& tb, int L, int R, int S, uint32_t* __restrict__ bitmap,
                                                unsigned long long* __restrict__ part /* [2R+1][M]: used, present, cnt */,
-                                               unsigned char* smem_raw, int64_t tile_index, unsigned long long* trace_row = nullptr,
-                                               unsigned long long* row_bar = nullptr /* transaction barrier (count 1): stage the rows in bulk */,
-                                               unsigned* row_parity = nullptr /* with row_bar: its phase parity, advanced by every bulk-staged tile */) {
+                                               unsigned char* smem_raw, int64_t tile_index, unsigned long long* trace_row = nullptr) {
   // optional stage stamps of warp 0 (kt_enable_trace): [4] the pod rows have landed, [5] first two words evaluated, [6] barrier
   // passed, [7] words + sums done, [8] sweep done
   auto stamp = [&](int k) {
@@ -768,42 +622,21 @@ __device__ __forceinline__ void reconcile_tile(const PodView& pods, const TableV
   const bool valid = p < pods.n;
   const int64_t pc = valid ? p : pods.n - 1;  // clamped: every lane loads, invalid lanes are masked below
   // ---- everything the tile needs of its pod rows is requested at once: ONE trip to HBM, and nothing else is waited for
-  // before the table gathers of the first two words go out.  A full tile of 16-byte aligned columns is fetched by the copy
-  // engine: thread 0 arms a transaction barrier and issues one bulk copy per column slice (8 row offsets, winfo, flags, ns,
-  // present: TILE * 4 bytes each; R request columns: TILE * 8 bytes each, straight into s_req) -- the slices land in shared
-  // memory without occupying anybody's registers or load queue; everybody else sleeps on the barrier.  Ragged tiles and
-  // unaligned tables (n not a multiple of 4) take the per-lane loads.
-  uint32_t* s_stage = reinterpret_cast<uint32_t*>(smem_raw + reconcile_stage_offset(L, R, S, REG, TILE));  // [kStageCols][TILE]
-  const bool bulk = KT_BULK_ROWS != 0 && REG && RT > 0 && row_bar != nullptr && (pods.n & 3) == 0 && tile0 + TILE <= pods.n;  // CTA-uniform
-  if (bulk && tid == 0) {
-    mbar_expect_tx(row_bar, (unsigned)(kStageCols * TILE * 4 + R * TILE * 8));
-#pragma unroll
-    for (int kcol = 0; kcol < 8; ++kcol) bulk_copy_g2s(s_stage + kcol * TILE, pods.roff + (int64_t)kcol * pods.n + tile0, TILE * 4, row_bar);
-    bulk_copy_g2s(s_stage + 8 * TILE, pods.winfo + tile0, TILE * 4, row_bar);
-    bulk_copy_g2s(s_stage + 9 * TILE, pods.flags + tile0, TILE * 4, row_bar);
-    bulk_copy_g2s(s_stage + 10 * TILE, pods.ns + tile0, TILE * 4, row_bar);
-    bulk_copy_g2s(s_stage + 11 * TILE, pods.present + tile0, TILE * 4, row_bar);
-#pragma unroll 1
-    for (int r = 0; r < R; ++r) bulk_copy_g2s(s_req + (size_t)r * TILE, pods.req + (int64_t)r * pods.n + tile0, TILE * 8, row_bar);
-  }
-  uint32_t winfo, flags, present;
-  int ns;
+  // before the table gathers of the first two words go out
+  const uint32_t winfo = __ldg(&pods.winfo[pc]);
+  const uint32_t flags = valid ? __ldg(&pods.flags[pc]) : 0u;
+  const int ns = __ldg(&pods.ns[pc]);
+  const uint32_t present = __ldg(&pods.present[pc]);
   PodRows<REG> rows;
   rows.init(s_rowid, tid, TILE);
+  load_rows<REG>(pods.roff, pods.n, pc, L, rows);
   long long rq[RT > 0 ? RT : 1];
-  if (!bulk) {
-    winfo = __ldg(&pods.winfo[pc]);
-    flags = valid ? __ldg(&pods.flags[pc]) : 0u;
-    ns = __ldg(&pods.ns[pc]);
-    present = __ldg(&pods.present[pc]);
-    load_rows<REG>(pods.roff, pods.n, pc, L, rows);
-    if constexpr (RT > 0) {
-      const int64_t* rp = pods.req + pc;
+  if constexpr (RT > 0) {
+    const int64_t* rp = pods.req + pc;
 #pragma unroll
-      for (int r = 0; r < RT; ++r) {
-        rq[r] = r < R ? __ldg(rp) : 0;
-        rp += pods.n;
-      }
+    for (int r = 0; r < RT; ++r) {
+      rq[r] = r < R ? __ldg(rp) : 0;
+      rp += pods.n;
     }
   }
   // The match bitmap is maintained, not rebuilt: a row can only ever be non-zero in the words of its namespace's list, so a
@@ -820,22 +653,6 @@ __device__ __forceinline__ void reconcile_tile(const PodView& pods, const TableV
     for (int i = tid; i < S * 32; i += TILE) { s_cnt[i] = 0u; s_pres[i] = 0u; }
     if (tid < S) s_key[tid] = -1;
   }
-  if constexpr (KT_BULK_ROWS != 0 && REG && RT > 0) {
-    if (bulk) {  // the slices have landed: the lane's own row out of shared memory
-      mbar_wait(row_bar, *row_parity);
-      *row_parity ^= 1u;
-      winfo = s_stage[8 * TILE + tid];
-      flags = s_stage[9 * TILE + tid];
-      ns = (int)s_stage[10 * TILE + tid];
-      present = s_stage[11 * TILE + tid];
-#pragma unroll
-      for (int kcol = 0; kcol < 8; ++kcol) rows.off[kcol] = s_stage[kcol * TILE + tid];
-      // ResourceAmountOfPod(p) columns are in place; absent keys read as 0 (presence kept separately)
-#pragma unroll 1
-      for (int r = 0; r < R; ++r)
-        if (!((present >> r) & 1)) s_req[r * TILE + tid] = 0;
-    }
-  }
   // shouldCountIn (throttle_controller.go:217-219): schedulerName == target && nodeName != ""
   const bool counted = (flags & (KT_POD_SCHEDULER_MATCH | KT_POD_SCHEDULED)) == (KT_POD_SCHEDULER_MATCH | KT_POD_SCHEDULED) &&
                        (unsigned)ns < (unsigned)tb.NS;
@@ -847,20 +664,13 @@ __device__ __forceinline__ void reconcile_tile(const PodView& pods, const TableV
   // phase 1 -- the lane's first two words, back to back and independent of the other lanes (a match word only needs the
   // lane's own row): their 2 x Lpad table gathers are all in flight together
   uint32_t m0 = 0, m1 = 0;
-  if constexpr (REG && KT_EVAL_PAIR) {
-    if (wc.inl > 1) eval_word2<TPC, B>(tb, rows, ns, wc.w0, wc.w1, m0, m1);
-    else if (wc.inl > 0) m0 = eval_word<TPC, B, REG>(tb, rows, Lpad, ns, wc.w0);
-  } else {
-    if (wc.inl > 0) m0 = eval_word<TPC, B, REG>(tb, rows, Lpad, ns, wc.w0);
-    if (wc.inl > 1) m1 = eval_word<TPC, B, REG>(tb, rows, Lpad, ns, wc.w1);
-  }
+  if (wc.inl > 0) m0 = eval_word<TPC, B, REG>(tb, rows, Lpad, ns, wc.w0);
+  if (wc.inl > 1) m1 = eval_word<TPC, B, REG>(tb, rows, Lpad, ns, wc.w1);
   // ResourceAmountOfPod(p) columns -> shared memory (absent keys read as 0; presence kept separately)
   if constexpr (RT > 0) {
-    if (!bulk) {
 #pragma unroll
-      for (int r = 0; r < RT; ++r)
-        if (r < R) s_req[r * TILE + tid] = ((present >> r) & 1) ? rq[r] : 0;
-    }
+    for (int r = 0; r < RT; ++r)
+      if (r < R) s_req[r * TILE + tid] = ((present >> r) & 1) ? rq[r] : 0;
   } else {
     const int64_t* rp = pods.req + pc;
     for (int r = 0; r < R; ++r) {
@@ -880,35 +690,6 @@ __device__ __forceinline__ void reconcile_tile(const PodView& pods, const TableV
   unsigned long long* part_pres = part + (size_t)R * tb.M;
   unsigned long long* part_cnt = part + (size_t)2 * R * tb.M;
 
-  // Rows in ARRIVAL order (no two lanes of the warp in the same namespace): the word-by-word rounds below would run once per
-  // lane for a handful of matches each.  Such a warp adds its pods' requests straight to the per-throttle sums in L2, one
-  // RED per (matched throttle, resource) -- slower per match than the transposed sums, but no rounds.
-  if (KT_SCATTER_WORDS < 32 && warp_is_scattered(wc)) {
-#pragma unroll 1
-    for (int kk = 0; kk < wc.cnt; ++kk) {
-      const int w = wc.at(tb, kk);
-      uint32_t word;
-      if (kk < wc.inl) {
-        word = kk == 0 ? m0 : m1;
-      } else {
-        word = eval_word<TPC, B, REG>(tb, rows, Lpad, ns, w);
-        bitmap[p * Wp + w] = word;
-      }
-      if (!alive) continue;
-      while (word) {
-        const int t = w * 32 + __ffs(word) - 1;
-        word &= word - 1;
-        atomicAdd(&part_cnt[t], 1ull);
-        for (int r = 0; r < R; ++r)
-          if ((present >> r) & 1) {
-            const unsigned long long v = (unsigned long long)s_req[r * TILE + tid];
-            if (v) atomicAdd(&part_used[(size_t)r * tb.M + t], v);
-            part_pres[(size_t)r * tb.M + t] = 1ull;  // idempotent flag
-          }
-      }
-    }
-    wc.cnt = 0;  // nothing left for the rounds below (the warp still takes part in the CTA's barriers and sweep)
-  }
   // phase 2 -- the segmented sums, word by word in ascending order, warp-uniform: lanes whose namespace has word w bring
   // their match word (already known for their first two), the others idle.  Namespace-clustered rows (the reference's pod
   // informer is namespace-indexed) make this 1-3 rounds.
@@ -1340,13 +1121,8 @@ __device__ __forceinline__ void check_match_tile(const PodView& pods, const Tabl
   WordCursor wc;
   wc.init(tb, winfo, ns, valid && (unsigned)ns < (unsigned)tb.NS);
   uint32_t m0 = 0, m1 = 0;  // the first two words: all their table gathers in flight together
-  if constexpr (REG && KT_EVAL_PAIR) {
-    if (wc.inl > 1) eval_word2<TPC, B>(tb, rows, ns, wc.w0, wc.w1, m0, m1);
-    else if (wc.inl > 0) m0 = eval_word<TPC, B, REG>(tb, rows, Lpad, ns, wc.w0);
-  } else {
-    if (wc.inl > 0) m0 = eval_word<TPC, B, REG>(tb, rows, Lpad, ns, wc.w0);
-    if (wc.inl > 1) m1 = eval_word<TPC, B, REG>(tb, rows, Lpad, ns, wc.w1);
-  }
+  if (wc.inl > 0) m0 = eval_word<TPC, B, REG>(tb, rows, Lpad, ns, wc.w0);
+  if (wc.inl > 1) m1 = eval_word<TPC, B, REG>(tb, rows, Lpad, ns, wc.w1);
   if (pods.zero_fill) __syncthreads();  // zero-fill before the word stores (rows of a tile are zeroed by all its lanes)
   if (wc.inl > 0) bitmap[p * Wp + wc.w0] = m0;
   if (wc.inl > 1) bitmap[p * Wp + wc.w1] = m1;
@@ -1391,33 +1167,18 @@ __device__ __forceinline__ uint2 decide_word_codes(uint32_t word, const unsigned
     uint32_t code;
     bool s1 = hq.w & 1u, s4 = hq.w & 8u;  // the count lane's share of S1 / S4
     const bool ge = hq.w & 16u;
-    if constexpr (RT > 0 && KT_DECIDE_UNROLLED) {
-      // every resource compared, no data-dependent loop -- measured SLOWER than the loops below at C2 (pods ask for one or two
-      // of the throttles' resources; the loops stop at the first hit): kept behind KT_DECIDE_UNROLLED, off
-      // (S1 threshold.IsThrottled(podAmount, false).IsThrottledFor(pod); S4 used + pod + reserved against the threshold)
-#pragma unroll
-      for (int r = 0; r < RT; ++r) {
-        if (r < R) {
-          const long long v = pod.req[r * pod.stride];
-          const bool on = (cand >> r) & 1;
-          s1 = s1 || (on && v > thrv[r]);
-          const long long hd = head[r];
-          s4 = s4 || (on && (ge ? v >= hd : v > hd));
-        }
-      }
-    } else {
-      for (uint32_t c = cand; c && !s1;) {
-        const int r = __ffs(c) - 1;
-        c &= c - 1;
-        s1 = pod.req[r * pod.stride] > thrv[r];
-      }
-      for (uint32_t c = cand; c && !s4;) {
-        const int r = __ffs(c) - 1;
-        c &= c - 1;
-        const long long v = pod.req[r * pod.stride];
-        const long long hd = head[r];
-        s4 = ge ? v >= hd : v > hd;
-      }
+    // S1 threshold.IsThrottled(podAmount, false).IsThrottledFor(pod); S4 used + pod + reserved against the threshold
+    for (uint32_t c = cand; c && !s1;) {
+      const int r = __ffs(c) - 1;
+      c &= c - 1;
+      s1 = pod.req[r * pod.stride] > thrv[r];
+    }
+    for (uint32_t c = cand; c && !s4;) {
+      const int r = __ffs(c) - 1;
+      c &= c - 1;
+      const long long v = pod.req[r * pod.stride];
+      const long long hd = head[r];
+      s4 = ge ? v >= hd : v > hd;
     }
     if (s1) code = KT_CHECK_POD_REQUESTS_EXCEEDS_THRESHOLD;
     else if ((hq.w & 2u) || (nz & hq.y)) code = KT_CHECK_ACTIVE;   // S2 status.throttled.IsThrottledFor(pod)
@@ -1580,10 +1341,6 @@ __device__ __forceinline__ uint2 decide_word_direct_codes(uint32_t word, int w, 
   }
   return make_uint2(c0, c1);
 }
-__device__ __forceinline__ void decide_word_direct(uint32_t word, int w, const unsigned char* __restrict__ pre, const PartExchange& px, size_t rec, int R, int M,
-                                                   int Wp, const DecidePod& pod, uint32_t* __restrict__ codes, const SparseOut& sp, unsigned char& ok) {
-  store_codes(decide_word_direct_codes(word, w, pre, px, rec, R, M, pod), w, Wp, pod.p, codes, sp, ok);
-}
 
 // the same out of line (everything by value: nothing of the caller has to live in local memory for it): the shared decide
 // tiles take this path only for words that found no staging slot, and keep their own code short
@@ -1650,19 +1407,6 @@ __device__ __forceinline__ void check_decide_tile(const PodView& pods, const Tab
   int k = 0;
   int cur = wc.at(tb, 0);
   bool sums_awaited = false;
-
-  // Pending rows in ARRIVAL order (a different namespace in every lane): staging 32-throttle records word by word would take
-  // one round per lane.  Such a warp checks its pairs one by one instead, every constant fetched from L2 -- the same 4 steps,
-  // without the staging (done below, once the sums exist); it proposes no words to the CTA's rounds.
-  const bool scattered = KT_SCATTER_WORDS < 32 && warp_is_scattered(wc);
-  if (scattered) cur = 0x7fffffff;
-  auto decide_scattered = [&]() {
-#pragma unroll 1
-    for (int kk = 0; kk < wc.cnt; ++kk) {
-      const int w = wc.at(tb, kk);
-      decide_word_direct(__ldcg(&bitmap[p * Wp + w]), w, pre, px, rec, R, M, Wp, pod, codes, sp, ok);
-    }
-  };
 
 #pragma unroll 1
   while (true) {
@@ -1753,7 +1497,6 @@ __device__ __forceinline__ void check_decide_tile(const PodView& pods, const Tab
 #pragma unroll
     for (int j = 0; j < 2; ++j)
       if (my_slot[j] >= 0) stage_finish_record(px, s_key[my_slot[j]], s_any[my_slot[j]], s_chk + (size_t)my_slot[j] * 32 * rec, rec, R, M, lane);
-    if (scattered && k == 0) { decide_scattered(); k = 1; }  // (k is otherwise unused by a scattered warp: marks "done")
     __syncthreads();
     stamp(7);
     // 3. every lane decides its own pairs
@@ -1784,11 +1527,8 @@ __device__ __forceinline__ void check_decide_tile(const PodView& pods, const Tab
 // (1) or over and over (2) on whatever the sums hold so far -- results thrown away, the raw pre-records fetched again -- so
 // that the real run finds its instructions in the SM's instruction caches.
 // ------------------------------------------------------------------------------------------------
-#ifndef KT_QUAD_FENCE  // 1: a shared decide tile looks at its three counters with relaxed loads and acquires once, with a fence; 0: three acquire loads
-#define KT_QUAD_FENCE 1
-#endif
-#ifndef KT_QUAD_DRYRUN  // measured: the walk itself costs what it saves -- off
-#define KT_QUAD_DRYRUN 0
+#ifndef KT_QUAD_DRYRUN  // measured: the walk itself costs what it saves -- off.  Not deleted: the compiler keeps the unused dry-run code, and
+#define KT_QUAD_DRYRUN 0  // without it the 768-thread k_pass allocates registers differently and C5 is 1.6% slower (DESIGN section 9)
 #endif
 template <int TILE, int RT>
 __device__ __forceinline__ void check_decide_quad(const PodView& pods, const TableView& tb, int R, int KS, const unsigned char* __restrict__ pre,
@@ -1838,15 +1578,9 @@ __device__ __forceinline__ void check_decide_quad(const PodView& pods, const Tab
   const unsigned sums_target = px.npeers == 0 ? sync.n_rec : sync.n_fin;
   unsigned seen_match = 0, seen_prep = 0, seen_sums = 0;
   if (tid == 0) {
-    if constexpr (KT_QUAD_FENCE != 0) {
-      seen_match = ld_relaxed_gpu(&sync.s->match_done);
-      seen_prep = ld_relaxed_gpu(&sync.s->prep_done);
-      seen_sums = ld_relaxed_gpu(sums_counter);
-    } else {  // three acquire loads: each one invalidates the SM's L1 under the reconcile tiles still working there
-      seen_match = ld_acquire_gpu(&sync.s->match_done);
-      seen_prep = ld_acquire_gpu(&sync.s->prep_done);
-      seen_sums = ld_acquire_gpu(sums_counter);
-    }
+    seen_match = ld_relaxed_gpu(&sync.s->match_done);
+    seen_prep = ld_relaxed_gpu(&sync.s->prep_done);
+    seen_sums = ld_relaxed_gpu(sums_counter);
   }
   const int ns = valid ? __ldg(&pods.ns[pc]) : -1;
   const uint32_t present = __ldg(&pods.present[pc]);
@@ -1868,15 +1602,15 @@ __device__ __forceinline__ void check_decide_quad(const PodView& pods, const Tab
   if (tid == 0) {
     // the match rows of EVERY pending tile (ours came from some other CTA) and the pre-records (early: they depend on nothing)
     if (seen_match < sync.n_match) {
-      spin_until([&] { return poll_gpu(&sync.s->match_done) >= sync.n_match; }, &sync.s->error, 40);
-      acquire_gpu(&sync.s->match_done);
+      spin_until([&] { return ld_relaxed_gpu(&sync.s->match_done) >= sync.n_match; }, &sync.s->error, 40);
+      (void)ld_acquire_gpu(&sync.s->match_done);
     }
     if (seen_prep < sync.n_fin) {
-      spin_until([&] { return poll_gpu(&sync.s->prep_done) >= sync.n_fin; }, &sync.s->error, 40);
-      acquire_gpu(&sync.s->prep_done);
+      spin_until([&] { return ld_relaxed_gpu(&sync.s->prep_done) >= sync.n_fin; }, &sync.s->error, 40);
+      (void)ld_acquire_gpu(&sync.s->prep_done);
     }
     *s_flag = seen_sums >= sums_target ? 1u : 0u;
-    if constexpr (KT_QUAD_FENCE != 0) fence_acquire_gpu();  // ONE acquire for every counter observed so far
+    fence_acquire_gpu();  // ONE acquire for every counter observed so far
   }
   __syncthreads();  // the slot table is initialised, the requests are in shared memory, the counters have been seen
   bool sums_ready = *s_flag != 0u;
@@ -2071,14 +1805,14 @@ __global__ void __launch_bounds__(TILE, THREADS / TILE) k_pass(const __grid_cons
   __shared__ unsigned s_ticket;
   __shared__ unsigned s_last;                 // trace: this CTA's last first-phase ticket (~0u: none yet)
   __shared__ unsigned long long s_t_start;    // trace: when the current tile began
-  __shared__ __align__(8) unsigned long long s_mbar[kMaxWarps + 1];  // transaction barriers: one per warp (bulk copies of the shared decide tiles), [kMaxWarps] the reconcile tile's rows
+  __shared__ __align__(8) unsigned long long s_mbar[kMaxWarps];  // transaction barriers: one per warp (bulk copies of the shared decide tiles)
   // Launched with programmatic stream serialization: the NEXT launch in the stream (normally the next pass) may have its CTAs
   // placed while this one still runs -- they sit in the wait below until this grid has completed and flushed, so nothing of
   // theirs (tickets, counters, sums) can mix with ours; what overlaps is their launch latency.
   pdl_launch_dependents();
   if (threadIdx.x == 0) {
 #pragma unroll
-    for (int i = 0; i < kMaxWarps + 1; ++i) mbar_init(&s_mbar[i], 1u);
+    for (int i = 0; i < kMaxWarps; ++i) mbar_init(&s_mbar[i], 1u);
     mbar_init_fence();
     s_last = ~0u;
   }
@@ -2097,7 +1831,6 @@ __global__ void __launch_bounds__(TILE, THREADS / TILE) k_pass(const __grid_cons
     asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
     row[0] = s_ticket; row[1] = smid; row[2] = s_t_start; row[3] = globaltimer_ns(); row[28] = blockIdx.x;
   };
-  unsigned row_parity = 0;  // of s_mbar[kMaxWarps], across this CTA's reconcile tiles
   unsigned ticket;
   // ---- first phase: match and reconcile tiles, none of which waits for anything ----
   while ((ticket = draw()) < n_tiles) {
@@ -2113,8 +1846,7 @@ __global__ void __launch_bounds__(TILE, THREADS / TILE) k_pass(const __grid_cons
       check_match_tile<TPC, B, REG, TILE>(a.pend, a.tb, a.L, a.pend_bitmap, a.codes, smem_raw, ticket);
       cta_signal(&a.sync->match_done);
     } else {
-      reconcile_tile<TPC, B, RT, REG, TILE>(a.run, a.tb, a.L, a.R, a.S, a.run_bitmap, a.px.mine, smem_raw, ticket - a.n_chk, trace_row(ticket),
-                                            &s_mbar[kMaxWarps], &row_parity);
+      reconcile_tile<TPC, B, RT, REG, TILE>(a.run, a.tb, a.L, a.R, a.S, a.run_bitmap, a.px.mine, smem_raw, ticket - a.n_chk, trace_row(ticket));
       cta_signal(&a.sync->rec_done);
     }
     if (a.trace && threadIdx.x == 0) {  // (s_ticket is still this tile's: the next draw begins with a CTA barrier)
