@@ -172,12 +172,15 @@ __device__ __forceinline__ void pdl_wait_primary() { asm volatile("griddepcontro
 // decide sub-tiles).  First-phase tiles never wait.  A second-phase piece waits only for pieces with smaller tickets, which
 // running CTAs have already drawn (a CTA draws its next ticket only once its previous piece is done), or for other GPUs,
 // whose pieces follow the same order -- so the waits cannot deadlock whatever the residency, and correctness does not depend
-// on the grid fitting the device (k_pass sizes it to the device for speed only).  Signals are fence + relaxed add (release
-// pattern) by thread 0 after a CTA barrier; waits are relaxed polls + one acquire by thread 0 followed by a CTA barrier.
+// on the grid fitting the device (k_pass sizes it to the device for speed only).  A CTA publishes its finished first-phase tiles
+// in runs, when it draws its first ticket past them: match_done at its first reconcile ticket or when it leaves the phase,
+// rec_done when it leaves the phase.  First-phase tiles never wait, so every one of them is published without anything having to
+// wait for it, and before its CTA starts a piece that can wait.  prep_done and tot_done are signalled piece by piece.  Signals are
+// fence + relaxed add (release pattern) by thread 0 after a CTA barrier; waits are relaxed polls + one acquire by thread 0 + a CTA barrier.
 struct PassSync {
   // counters of ONE pass, re-armed by its last CTA (everything before `error`)
   unsigned ticket;      // next piece of work
-  unsigned rec_done;    // reconcile tiles finished (their REDs are performed at L2)
+  unsigned rec_done;    // reconcile tiles finished and published (their REDs are performed at L2)
   unsigned prep_done;   // finalize tiles that have written their throttles' pre-records (nothing to wait for: early)
   unsigned match_done;  // pending-match tiles finished (affectedThrottles rows written)
   unsigned tot_done;    // multi-GPU: finalize tiles of this rank that have written the all-rank totals of their throttles
@@ -1804,6 +1807,7 @@ __global__ void __launch_bounds__(TILE, THREADS / TILE) k_pass(const __grid_cons
   extern __shared__ __align__(16) unsigned char smem_raw[];
   __shared__ unsigned s_ticket;
   __shared__ unsigned s_last;                 // trace: this CTA's last first-phase ticket (~0u: none yet)
+  __shared__ unsigned s_done[2];              // first-phase tiles this CTA has finished and not yet published: match, reconcile
   __shared__ unsigned long long s_t_start;    // trace: when the current tile began
   __shared__ __align__(8) unsigned long long s_mbar[kMaxWarps];  // transaction barriers: one per warp (bulk copies of the shared decide tiles)
   // Launched with programmatic stream serialization: the NEXT launch in the stream (normally the next pass) may have its CTAs
@@ -1815,6 +1819,7 @@ __global__ void __launch_bounds__(TILE, THREADS / TILE) k_pass(const __grid_cons
     for (int i = 0; i < kMaxWarps; ++i) mbar_init(&s_mbar[i], 1u);
     mbar_init_fence();
     s_last = ~0u;
+    s_done[0] = s_done[1] = 0u;
   }
   pdl_wait_primary();
   const unsigned n_tiles = a.n_chk + a.n_rec;
@@ -1833,7 +1838,16 @@ __global__ void __launch_bounds__(TILE, THREADS / TILE) k_pass(const __grid_cons
   };
   unsigned ticket;
   // ---- first phase: match and reconcile tiles, none of which waits for anything ----
+  // Nothing waits for match_done / rec_done before every first-phase ticket has been drawn, so a CTA publishes the tiles it
+  // finished in runs: its match tiles when it draws its first ticket past them (the decide sub-tiles start staging on the match
+  // rows while the last reconcile tiles run), its reconcile tiles when it leaves the phase -- no L2 round trip between two
+  // reconcile tiles.  Each publish follows the CTA barrier that begins the draw: every thread's tiles are complete.
   while ((ticket = draw()) < n_tiles) {
+    if (threadIdx.x == 0 && ticket >= a.n_chk && s_done[0]) {
+      __threadfence();
+      atomicAdd(&a.sync->match_done, s_done[0]);
+      s_done[0] = 0u;
+    }
     if (a.trace && threadIdx.x == 0) s_t_start = globaltimer_ns();
     if (ticket < a.n_chk) {
       const FlagSync sync{a.sync, a.n_rec, a.n_fin, a.n_chk};
@@ -1844,15 +1858,22 @@ __global__ void __launch_bounds__(TILE, THREADS / TILE) k_pass(const __grid_cons
       // the first match tile also clears the sparse list's counter: every decide sub-tile waits for ALL match tiles before it appends
       if (ticket == 0 && threadIdx.x == 0 && a.sparse.count) *a.sparse.count = 0u;
       check_match_tile<TPC, B, REG, TILE>(a.pend, a.tb, a.L, a.pend_bitmap, a.codes, smem_raw, ticket);
-      cta_signal(&a.sync->match_done);
     } else {
       reconcile_tile<TPC, B, RT, REG, TILE>(a.run, a.tb, a.L, a.R, a.S, a.run_bitmap, a.px.mine, smem_raw, ticket - a.n_chk, trace_row(ticket));
-      cta_signal(&a.sync->rec_done);
     }
-    if (a.trace && threadIdx.x == 0) {  // (s_ticket is still this tile's: the next draw begins with a CTA barrier)
-      close_row(trace_row(s_ticket));
-      s_last = s_ticket;
+    if (threadIdx.x == 0) {  // (s_ticket is still this tile's: the next draw begins with a CTA barrier)
+      ++s_done[ticket < a.n_chk ? 0 : 1];
+      if (a.trace) {
+        close_row(trace_row(s_ticket));
+        s_last = s_ticket;
+      }
     }
+  }
+  // the rest, before this CTA starts anything that can wait (release pattern, as cta_signal)
+  if (threadIdx.x == 0 && (s_done[0] | s_done[1])) {
+    __threadfence();
+    if (s_done[0]) atomicAdd(&a.sync->match_done, s_done[0]);
+    if (s_done[1]) atomicAdd(&a.sync->rec_done, s_done[1]);
   }
   // ---- second phase: status tiles and decide sub-tiles, until the counter runs past them ----
   unsigned mbar_phase = 0;

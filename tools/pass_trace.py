@@ -1,6 +1,7 @@
 """Per-role timeline of the fused pass (k_pass) from the in-kernel trace: the grid and how many tiles its CTAs ran, when each
 role's tiles start and end relative to the first CTA, the stage stamps of every role (median / p90 / max since pass start),
-the shared decide sub-tiles and the slowest tiles of each role.
+how long each stage of a reconcile tile takes and how long its CTA takes from the tile's sweep to its next tile, the shared
+decide sub-tiles and the slowest tiles of each role.
 python tools/pass_trace.py [C2] [sorted|unsorted]"""
 import os
 import sys
@@ -63,6 +64,27 @@ for it in range(4):
             x = x[r[:, 4 + k] > 0]
             if len(x):
                 print(f"            {label:18s} since pass start: med {np.median(x):5.1f}  p90 {np.percentile(x, 90):5.1f}  max {x.max():5.1f}")
+        if name == "reconcile":  # how long each stage of a tile takes, and what a CTA spends between a tile's sweep and its next tile
+            cols = [2] + [4 + k for k in range(len(STAGES[name]))] + [3]
+            ok = (r[:, cols] > 0).all(axis=1)
+            labels = STAGES[name] + ["end (signal)"]
+            parts = [f"{labels[k]} {np.median(d):.2f}/{np.percentile(d, 90):.2f}"
+                     for k, d in enumerate((r[ok][:, b] - r[ok][:, a]) / 1e3 for a, b in zip(cols[:-1], cols[1:]))]
+            print("            per tile, us since the previous stamp (median/p90): " + " | ".join(parts))
+            first = rows[:lo]  # every first-phase tile, in ticket order: a CTA's next tile is its next row
+            per_cta_rows = {}
+            for i in np.argsort(first[:, 2], kind="stable"):
+                per_cta_rows.setdefault(int(first[i, 28]), []).append(i)
+            gap_end, gap_sweep = [], []
+            for seq in per_cta_rows.values():
+                for i, j in zip(seq[:-1], seq[1:]):
+                    if lo - int(n) <= i < lo:  # a reconcile tile followed by another first-phase tile on the same CTA
+                        gap_end.append(first[j, 2] - first[i, 3])
+                        gap_sweep.append(first[j, 2] - first[i, 8])
+            if gap_end:
+                ge, gs = np.array(gap_end) / 1e3, np.array(gap_sweep) / 1e3
+                print(f"            {len(ge)} reconcile tiles followed by another tile on their CTA: end -> next start med {np.median(ge):.2f} "
+                      f"p90 {np.percentile(ge, 90):.2f}; sweep -> next start med {np.median(gs):.2f} p90 {np.percentile(gs, 90):.2f} max {gs.max():.2f}")
         if (r[:, 9] > 0).any():  # a CTA's last tile carries the stamps of its first shared decide sub-tile
             sel = r[:, 9] > 0
             print(f"            -> {int(sel.sum())} CTAs whose last tile was one of these went on to shared decide sub-tiles")
