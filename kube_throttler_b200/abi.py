@@ -26,7 +26,7 @@ POD_SCHEDULER_MATCH, POD_SCHEDULED, POD_NOT_FINISHED = 1, 2, 4
 THR_RESPONSIBLE, THR_SELECTOR_ERROR = 1, 2
 KIND_THROTTLE, KIND_CLUSTERTHROTTLE = 0, 1
 OP_IN, OP_NOTIN, OP_EXISTS, OP_DOESNOTEXIST = 0, 1, 2, 3
-TERM_NS_INVALID = 1
+TERM_NS_INVALID, TERM_POD_INVALID = 1, 2
 OVR_PARSE_ERROR = 1
 CHECK_NOT_THROTTLED, CHECK_ACTIVE, CHECK_INSUFFICIENT, CHECK_POD_REQUESTS_EXCEEDS_THRESHOLD = 0, 1, 2, 3
 CHECK_NAMES = ("not-throttled", "active", "insufficient", "pod-requests-exceeds-threshold")
