@@ -107,6 +107,33 @@ func (e *engine) reconcileAll(nowRFC3339 string) (*reconcileResult, error) {
 	return &r, nil
 }
 
+// reconcileKeysResult is what kth_reconcile reports for the listed keys; keys of other throttlers are skipped.
+type reconcileKeysResult struct {
+	reconcileResult
+	Errors   map[string]string `json:"errors"`   // key -> reconcile's error (malformed key, reachable broken podSelector)
+	NotFound []string          `json:"notFound"` // unknown or deleted: the lister's NotFound, reconcile returns nil
+}
+
+// reconcileKeys is reconcile(key) for the listed keys only ("ns/name" for a Throttle, "/name" for a ClusterThrottle), in one
+// device call over the listed throttles and the namespaces they reach.
+func (e *engine) reconcileKeys(keys []string, nowRFC3339 string) (*reconcileKeysResult, error) {
+	js, err := json.Marshal(keys)
+	if err != nil {
+		return nil, err
+	}
+	ck, cs := C.CString(string(js)), C.CString(nowRFC3339)
+	defer C.free(unsafe.Pointer(ck))
+	defer C.free(unsafe.Pointer(cs))
+	runtime.LockOSThread()
+	raw := C.GoString(C.kth_reconcile(e.h, ck, cs))
+	runtime.UnlockOSThread()
+	var r reconcileKeysResult
+	if err := decode(raw, &r); err != nil {
+		return nil, err
+	}
+	return &r, nil
+}
+
 // statusManifest is the `status` subresource as encoding/json would render v1alpha1.ThrottleStatus.
 func (e *engine) statusManifest(ns, name string) ([]byte, error) {
 	cn, cm := C.CString(ns), C.CString(name)

@@ -349,6 +349,19 @@ int kt_get_match_rows(kt_ctx* ctx, int kind, int64_t k, const int64_t* rows, uin
  * one read of off[], one copy of the rows).  Multi-GPU: each rank answers for its own rows. */
 int kt_get_match_columns(kt_ctx* ctx, int kind, int64_t k, const int32_t* idx, int64_t* off /*[k+1]*/, int64_t* rows /*[cap]*/,
                          uint8_t* codes /*[cap] or NULL*/, int64_t cap);
+/* reconcile(key) for k listed throttles (throttle_controller.go:84-211, clusterthrottle_controller.go:87-214), evaluated at
+ * `now` on the running rows as they are now -- uploaded or delta-updated, whether or not a pass has run since.  For entry j:
+ *   - out: what a KT_EVAL_FRESH_STATUS pass would report for column idx[j] (used, presence, pod count, throttled with
+ *     onEqual = true, CalculateThreshold(now), override_active), shaped [R][k] / [k] as kt_get_reconcile_rows fills them
+ *     (any pointer may be NULL);
+ *   - rows[off[j] .. off[j+1]): the rows the throttle matches, ascending -- the RUNNING relation of kt_get_match_columns
+ *     (counted pods, finished ones included).
+ * Arguments as kt_get_match_columns: idx in [0, M) (KT_ERR_INVALID otherwise), duplicates each get their own entry, k = 0 is
+ * valid, off[0..k] is always written and rows only when off[k] <= cap.  Only the listed throttles' words are evaluated, and
+ * only for the rows whose namespace they can reach; the call writes nothing another call reads (every getter answers as
+ * before it).  KT_ERR_STATE before kt_upload_throttles, and with a communicator (single GPU only). */
+int kt_reconcile_throttles(kt_ctx* ctx, int64_t now_unix_ns, int64_t k, const int32_t* idx, const kt_reconcile_out* out,
+                           int64_t* off /*[k+1]*/, int64_t* rows /*[cap] or NULL*/, int64_t cap);
 /* codes: 2 bits per (pending pod, throttle), pod-major, 16 codes per uint32:
  *   code(p,t) = (codes[p*2*words_per_row + (t>>4)] >> (2*(t&15))) & 3
  * admit[p] = 1 iff every affected throttle is KT_CHECK_NOT_THROTTLED (plugin.go:177-180).

@@ -61,6 +61,19 @@ const char* kth_delete(kth_plugin* p, const char* kind, const char* ns, const ch
  * NextOverrideHappensIn (throttle_types.go:37-63), what the reference passes to enqueueAfter (:201-208). */
 const char* kth_reconcile_all(kth_plugin* p, const char* now_rfc3339);
 
+/* reconcile(key) for the listed keys only (throttle_controller.go:84-211, clusterthrottle_controller.go:87-214): the reference's
+ * controllers reconcile one workqueue key at a time, at the cost of the pods of the namespaces the throttle reaches.  keys_json
+ * is a JSON array of names as kth_reconcile_all spells them under "changed": "namespace/name" for a Throttle, "/name" for a
+ * ClusterThrottle.  Each distinct key, in the order given, gets exactly what kth_reconcile_all does for that throttle (status
+ * under Q6 and Semantic.DeepEqual, cached verdicts, gauges, NextOverrideHappensIn, unreserveAffectedPods with Q8, or the
+ * reachable broken-podSelector error that leaves the status and the reservations alone), from ONE device call over the listed
+ * throttles' columns and the rows of the namespaces they reach (kt_reconcile_throttles).  Throttles that are not listed keep
+ * their status, reservations and gauges.  Returns
+ *   {"reconciled":n,"changed":[...],"requeueAfterNanos":{...},"errors":{key: text},"notFound":[...]}
+ * an unknown or deleted key is in "notFound" (the lister's NotFound makes reconcile return nil, :95-101), a key of another
+ * throttler is skipped, a malformed key is an entry of "errors". */
+const char* kth_reconcile(kth_plugin* p, const char* keys_json, const char* now_rfc3339);
+
 /* status of one Throttle (ns != "") or ClusterThrottle (ns == ""):
  * {"calculatedThreshold":{"threshold":{...},"calculatedAtSet":bool,"calculatedAtUnix":sec,"messages":[..]},
  *  "throttled":{"resourceCounts":{"pod":bool},"resourceRequests":{name:bool}},

@@ -30,7 +30,7 @@ class KtError(RuntimeError):
 
 def build(force: bool = False) -> str:
     """Compile csrc/ for sm_90a in-tree (nvcc cross-compiles without a GPU)."""
-    srcs = [os.path.join(_HERE, "csrc", f) for f in ("kt_engine.cu", "kt_tables.cc", "kt_host.cc", "kt_kernels.cuh", "kt_tables.h", "kt_json.h", "kt_quantity.h")]
+    srcs = [os.path.join(_HERE, "csrc", f) for f in ("kt_engine.cu", "kt_tables.cc", "kt_host.cc", "kt_kernels.cuh", "kt_admit.cuh", "kt_keyed.cuh", "kt_tables.h", "kt_json.h", "kt_quantity.h")]
     srcs.append(os.path.join(_HERE, "..", "include", "kt_b200.h"))
     srcs.append(os.path.join(_HERE, "..", "include", "kt_host.h"))
     newest = max(os.path.getmtime(s) for s in srcs)
@@ -44,7 +44,7 @@ EXPORTS = [
     "kt_create", "kt_destroy", "kt_last_error", "kt_version", "kt_set_stream", "kt_sync", "kt_enable_timing",
     "kt_enable_trace", "kt_get_trace", "kt_host_alloc", "kt_host_alloc_upload", "kt_host_free", "kt_upload_pods", "kt_upload_pods_compact", "kt_upload_pods_packed", "kt_set_async_uploads", "kt_update_pod_rows", "kt_upload_namespaces",
     "kt_upload_throttles", "kt_upload_status", "kt_set_reserved", "kt_evaluate", "kt_get_reconcile",
-    "kt_match_words", "kt_get_match_bitmap", "kt_get_match_rows", "kt_get_match_columns", "kt_get_check", "kt_set_sparse_check", "kt_get_check_sparse", "kt_get_check_rows", "kt_get_changed", "kt_get_reconcile_rows", "kt_step_submit", "kt_step_wait", "kt_admit_queue", "kt_get_timing", "kt_comm_unique_id",
+    "kt_match_words", "kt_get_match_bitmap", "kt_get_match_rows", "kt_get_match_columns", "kt_reconcile_throttles", "kt_get_check", "kt_set_sparse_check", "kt_get_check_sparse", "kt_get_check_rows", "kt_get_changed", "kt_get_reconcile_rows", "kt_step_submit", "kt_step_wait", "kt_admit_queue", "kt_get_timing", "kt_comm_unique_id",
     "kt_comm_init", "kt_comm_destroy", "kt_debug_compile_tables", "kt_debug_set_pass_plan", "kt_debug_get_pass_plan",
 ]
 
@@ -99,6 +99,7 @@ def lib():
         L.kt_match_words.restype = C.c_int32
         L.kt_get_match_bitmap.argtypes = [vp, C.c_int, vp]
         L.kt_get_match_columns.argtypes = [vp, C.c_int, C.c_int64, vp, vp, vp, vp, C.c_int64]
+        L.kt_reconcile_throttles.argtypes = [vp, C.c_int64, C.c_int64, vp, C.POINTER(abi.ReconcileOut), vp, vp, C.c_int64]
         L.kt_get_check.argtypes = [vp, vp, vp]
         L.kt_get_timing.argtypes = [vp, C.POINTER(abi.Timing)]
         L.kt_comm_unique_id.argtypes = [vp]
@@ -363,6 +364,25 @@ class Engine:
             total = int(off[k])
             if total <= cap:
                 return off, rows[:total], (codes[:total] if codes is not None else None)
+            cap = total
+
+    def reconcile_throttles(self, now: int, idx, cap: Optional[int] = None):
+        """reconcile(key) of the listed throttles at `now` on the running rows as they are: (status columns shaped for len(idx)
+        throttles as get_reconcile_rows returns them, off[k+1], rows) with throttle idx[j]'s matched rows, ascending, in
+        rows[off[j]:off[j+1]].  `cap` sizes the first attempt (default: the running rows)."""
+        idx = np.ascontiguousarray(idx, np.int32)
+        k, R, z = idx.shape[0], self.R, np.zeros
+        out = PassResult(self.words_per_row, z((R, k), np.int64), z(k, np.uint32), z(k, np.int64), z(k, np.uint32), z((R, k), np.int64), z(k, np.uint32),
+                         z(k, np.int64), z(k, np.uint8), z((0, 1), np.uint32), z((0, 1), np.uint32), z((0, 1), np.uint32), z(0, np.uint8))
+        rec = out.reconcile_out()
+        off = np.zeros(k + 1, np.int64)
+        cap = self.n[abi.PODS_RUNNING] if cap is None else cap
+        while True:
+            rows = np.zeros(max(cap, 1), np.int64)
+            self._ck(self._L.kt_reconcile_throttles(self._h, now, k, abi.ptr(idx), C.byref(rec), abi.ptr(off), abi.ptr(rows), cap))
+            total = int(off[k])
+            if total <= cap:
+                return out, off, rows[:total]
             cap = total
 
     def get_changed(self):

@@ -18,6 +18,7 @@
 #include "../../include/kt_b200.h"
 #include "kt_kernels.cuh"
 #include "kt_admit.cuh"
+#include "kt_keyed.cuh"
 #include "kt_tables.h"
 
 namespace {
@@ -160,6 +161,7 @@ struct kt_ctx {
   bool have_diff = false;  // the last pass produced a diff (an observed status was uploaded)
   DevBuf d_col_idx, d_col_cnt, d_col_off, d_col_rows;  // per-throttle row lists (kt_admit.cuh ColumnView): kt_admit_queue, kt_get_match_columns
   DevBuf d_adm_state, d_adm_fail, d_adm_counters;      // kt_admit_queue (kt_admit.cuh)
+  DevBuf d_key_list, d_key_reach, d_key_scratch, d_key_acc, d_key_out;  // kt_reconcile_throttles (kt_keyed.cuh): scratch of one call
   DevBuf d_pre;    // [M] pre-records, finalize tiles -> decide tiles (kt_kernels.cuh pre_record_bytes)
   // per-throttle outputs of the reconcile half: ONE device block (and one pinned host mirror) so that kt_get_reconcile
   // is a single D2H copy; o_off[i] = byte offset of {used, used_cnt, calc_thr, calc_cnt, used_present, throttled,
@@ -583,7 +585,8 @@ void kt_destroy(kt_ctx* c) {
                    &c->d_ovr_present, &c->d_ovr_cnt, &c->d_st_calculated, &c->d_st_calc_thr, &c->d_st_calc_present, &c->d_st_calc_cnt,
                    &c->d_st_used, &c->d_st_used_present, &c->d_st_used_cnt, &c->d_st_throttled, &c->d_reserved, &c->d_reserved_present,
                    &c->d_reserved_cnt, &c->d_part, &c->d_sync, &c->d_trace, &c->d_pre, &c->d_changed, &c->d_col_idx, &c->d_col_cnt, &c->d_col_off,
-                   &c->d_col_rows, &c->d_adm_state, &c->d_adm_fail, &c->d_adm_counters, &c->d_out, &c->d_codes, &c->d_admit};
+                   &c->d_col_rows, &c->d_adm_state, &c->d_adm_fail, &c->d_adm_counters, &c->d_out, &c->d_codes, &c->d_admit,
+                   &c->d_key_list, &c->d_key_reach, &c->d_key_scratch, &c->d_key_acc, &c->d_key_out};
   if (c->h_out) cudaFreeHost(c->h_out);
   if (c->h_step) cudaFreeHost(c->h_step);
   if (c->ev_step) cudaEventDestroy(c->ev_step);
@@ -1513,6 +1516,104 @@ int kt_get_match_columns(kt_ctx* c, int kind, int64_t k, const int32_t* idx, int
   if (total > cap || total == 0) return KT_OK;  // off[] says how much room the rows need
   KT_CUDA(c, cudaMemcpyAsync(rows, v.rows, (size_t)total * 8, cudaMemcpyDeviceToHost, c->stream));
   if (codes) KT_CUDA(c, cudaMemcpyAsync(codes, v.codes_out, (size_t)total, cudaMemcpyDeviceToHost, c->stream));
+  KT_CUDA(c, cudaStreamSynchronize(c->stream));
+  return KT_OK;
+}
+
+// ---- reconcile(key) for k listed throttles (kt_keyed.cuh) ---------------------------------------------------------------
+int kt_reconcile_throttles(kt_ctx* c, int64_t now, int64_t k, const int32_t* idx, const kt_reconcile_out* o, int64_t* off, int64_t* rows, int64_t cap) {
+  if (!c || !o || !off || k < 0 || cap < 0 || (k > 0 && !idx) || (cap > 0 && !rows)) return KT_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(c->mu);
+  if (c->comm) return fail(c, KT_ERR_STATE, "kt_reconcile_throttles is single-GPU: this context has a communicator");
+  if (!c->have_throttles) return fail(c, KT_ERR_STATE, "kt_reconcile_throttles before kt_upload_throttles");
+  const int M = c->M, R = c->lim.n_resources;
+  for (int64_t e = 0; e < k; ++e)
+    if (idx[e] < 0 || idx[e] >= M) return fail(c, KT_ERR_INVALID, "throttle %d out of range [0,%d)", idx[e], M);
+  off[0] = 0;
+  if (k == 0) return KT_OK;
+  int rc = set_device(c);
+  if (rc) return rc;
+  PodStore& run = c->pods[KT_PODS_RUNNING];
+  if ((rc = ensure_roff(c, run))) return rc;  // rows or tables changed since the offsets were translated (a pure function of both)
+  // the listed words and their listed bits; entry e sums into compact throttle cidx[e] = j * 32 + bit
+  std::vector<int32_t> words;
+  std::vector<uint32_t> masks;
+  std::vector<int32_t> slot((size_t)c->ht.W, -1), cidx((size_t)k);
+  for (int64_t e = 0; e < k; ++e) {
+    const int w = idx[e] >> 5;
+    if (slot[(size_t)w] < 0) { slot[(size_t)w] = (int32_t)words.size(); words.push_back(w); masks.push_back(0u); }
+    masks[(size_t)slot[(size_t)w]] |= 1u << (idx[e] & 31);
+    cidx[(size_t)e] = slot[(size_t)w] * 32 + (idx[e] & 31);
+  }
+  const int nw = (int)words.size(), NC = (nw + 31) / 32, NJ = nw * 32, NS = c->ht.NS;
+  const size_t n = (size_t)run.n;
+  // one upload: words[nw] | masks[nw] | idx[k] | cidx[k]
+  std::vector<int32_t> list;
+  list.reserve((size_t)2 * nw + 2 * (size_t)k);
+  list.insert(list.end(), words.begin(), words.end());
+  for (uint32_t m : masks) list.push_back((int32_t)m);
+  list.insert(list.end(), idx, idx + k);
+  list.insert(list.end(), cidx.begin(), cidx.end());
+  KT_CUDA(c, c->d_key_list.reserve(list.size() * 4 + 16));
+  KT_CUDA(c, cudaMemcpyAsync(c->d_key_list.p, list.data(), list.size() * 4, cudaMemcpyHostToDevice, c->stream));
+  const int32_t* d_words = c->d_key_list.as<int32_t>();
+  const uint32_t* d_masks = c->d_key_list.as<uint32_t>() + nw;
+  const int32_t* d_idx = d_words + 2 * nw;
+  const int32_t* d_cidx = d_idx + k;
+  KT_CUDA(c, c->d_key_reach.reserve((size_t)NS * NC * 4 + 16));
+  KT_CUDA(c, c->d_key_scratch.reserve(n * nw * 4 + 16));
+  const size_t acc_bytes = (size_t)NJ * ((size_t)R * 8 + 8 + 4);
+  KT_CUDA(c, c->d_key_acc.reserve(acc_bytes + 16));
+  if (n) KT_CUDA(c, cudaMemsetAsync(c->d_key_scratch.p, 0, n * nw * 4, c->stream));
+  KT_CUDA(c, cudaMemsetAsync(c->d_key_acc.p, 0, acc_bytes, c->stream));
+  const TableView tb = table_view(c);
+  if (NS > 0) k_keyed_reach<<<(unsigned)(((int64_t)NS * NC + 255) / 256), 256, 0, c->stream>>>(tb, nw, d_words, d_masks, NC, c->d_key_reach.as<uint32_t>());
+  KT_CUDA(c, cudaGetLastError());
+  KeyedArgs a{};
+  a.pods = pod_view(run);
+  a.tb = tb;
+  a.L = c->lim.label_slots; a.R = R; a.nw = nw; a.words = d_words; a.masks = d_masks; a.reach = c->d_key_reach.as<uint32_t>(); a.NC = NC;
+  a.scratch = c->d_key_scratch.as<uint32_t>();
+  a.used = c->d_key_acc.as<unsigned long long>();
+  a.cnt = a.used + (size_t)R * NJ;
+  a.pres = reinterpret_cast<uint32_t*>(a.cnt + NJ);
+  a.smem_acc = keyed_smem_acc_bytes(nw, R) <= kKeyedSmemAcc ? 1 : 0;
+  if (n && NS > 0) {
+    const int64_t tiles = (int64_t)((n + kKeyedTile - 1) / kKeyedTile);
+    const unsigned grid = (unsigned)std::min<int64_t>(tiles, (int64_t)c->sm_count * 8);
+    KT_CUDA(c, with_variant(c, false, [&](auto tpc, auto b, auto rt, auto reg) {
+      const size_t smem = keyed_smem_bytes(nw, R, a.L, reg, a.smem_acc);
+      return launch(c, k_keyed_rows<tpc, b, rt, reg>, grid, kKeyedTile, smem, false, a);
+    }));
+  }
+  // the status of the k columns, shaped as kt_get_reconcile_rows delivers it
+  ThrottleView tv{};
+  tv.flags = c->d_tflags.as<uint8_t>();
+  tv.thr = c->d_thr.as<int64_t>(); tv.thr_present = c->d_thr_present.as<uint32_t>(); tv.thr_cnt = c->d_thr_cnt.as<int64_t>();
+  tv.ovr_off = c->d_ovr_off.as<int32_t>(); tv.ovr_begin = c->d_ovr_begin.as<int64_t>(); tv.ovr_end = c->d_ovr_end.as<int64_t>();
+  tv.ovr_flags = c->d_ovr_flags.as<uint8_t>(); tv.ovr_thr = c->d_ovr_thr.as<int64_t>(); tv.ovr_present = c->d_ovr_present.as<uint32_t>();
+  tv.ovr_cnt = c->d_ovr_cnt.as<int64_t>(); tv.n_ovr = c->n_ovr;
+  const size_t bytes = (size_t)k * ((size_t)2 * R * 8 + 16 + 12 + 1);
+  KT_CUDA(c, c->d_key_out.reserve(bytes + 16));
+  k_keyed_status<<<(unsigned)((k + 127) / 128), 128, 0, c->stream>>>(k, d_idx, d_cidx, R, M, NJ, tv, (long long)now, a.used, a.cnt, a.pres,
+                                                                   c->d_key_out.as<unsigned char>());
+  KT_CUDA(c, cudaGetLastError());
+  std::vector<unsigned char> hb(bytes);
+  KT_CUDA(c, cudaMemcpyAsync(hb.data(), c->d_key_out.p, bytes, cudaMemcpyDeviceToHost, c->stream));
+  // the matched rows: the scratch transposed (ColumnView over the compact words)
+  ColumnView v{};
+  v.bitmap = a.scratch; v.Wp = nw; v.first = 0; v.count = (int64_t)n; v.idx = d_cidx; v.k = k;
+  int64_t total = 0;
+  if ((rc = build_columns(c, v, &total, off, cap))) return rc;  // (synchronises the stream: hb has landed)
+  size_t at = 0;
+  auto take = [&](void* dst, size_t sz) {
+    if (dst) std::memcpy(dst, hb.data() + at, sz);
+    at += sz;
+  };
+  take(o->used, (size_t)R * k * 8); take(o->calc_thr, (size_t)R * k * 8); take(o->used_cnt, (size_t)k * 8); take(o->calc_cnt, (size_t)k * 8);
+  take(o->used_present, (size_t)k * 4); take(o->throttled, (size_t)k * 4); take(o->calc_present, (size_t)k * 4); take(o->override_active, (size_t)k);
+  if (total > cap || total == 0) return KT_OK;  // off[] says how much room the rows need
+  KT_CUDA(c, cudaMemcpyAsync(rows, v.rows, (size_t)total * 8, cudaMemcpyDeviceToHost, c->stream));
   KT_CUDA(c, cudaStreamSynchronize(c->stream));
   return KT_OK;
 }

@@ -26,9 +26,10 @@
 #include "kt_quantity.h"
 
 // The host layer is also linked, for CPU tests, against engine test doubles (tests/host_stub) that implement only the calls
-// the rest of this file makes: a weak reference lets such a build load, and kth_affected_pods fails in it.  The product
-// library defines the call in kt_engine.cu, so the reference is always bound there.
+// the rest of this file makes: weak references let such a build load, and kth_affected_pods / kth_reconcile fail in it.  The product
+// library defines both calls in kt_engine.cu, so the references are always bound there.
 #pragma weak kt_get_match_columns
+#pragma weak kt_reconcile_throttles
 
 namespace {
 
@@ -1323,6 +1324,59 @@ struct kth_plugin {
     return out;
   }
 
+  // What reconcile writes for throttle t from its device status (entry q of columns shaped for k throttles): status.used,
+  // calculatedThreshold (Q6), throttled, compared under Semantic.DeepEqual; records the gauges.  Returns whether the status changed.
+  bool update_status(size_t t, const kt_reconcile_out& ro, size_t k, size_t q, const GoTime& now) {
+    ThrottleObj& o = throttles[t];
+    o.host_dirty = false;
+    ResAmount nu;  // used := ResourceAmount{}; used = used.Add(ResourceAmountOfPod(p)) ...
+    if (ro.used_present[q] & KT_COUNT_BIT) {
+      nu.has_counts = true;
+      nu.pod = ro.used_cnt[q];
+      nu.requests_nil = false;
+      for (int r = 0; r < (int)cols.size(); ++r)
+        if ((ro.used_present[q] >> r) & 1) nu.requests[r] = from_scale(r, ro.used[(size_t)r * k + q]);
+    }
+    ResAmount nc;  // CalculateThreshold(now).Threshold
+    nc.has_counts = ro.calc_present[q] & KT_COUNT_BIT;
+    nc.pod = nc.has_counts ? ro.calc_cnt[q] : 0;
+    nc.requests_nil = false;
+    for (int r = 0; r < (int)cols.size(); ++r)
+      if ((ro.calc_present[q] >> r) & 1) nc.requests[r] = from_scale(r, ro.calc_thr[(size_t)r * k + q]);
+    if (!ro.override_active[q]) nc = o.threshold;  // no active override: spec.threshold itself (keeps nil-ness and spelling)
+    const std::vector<std::string> msgs = override_messages(o);
+    bool status_changed = false;
+    if (!amount_equal(o.st_calc, nc) || o.st_messages != msgs) {  // Q6: otherwise the old calculatedAt is kept
+      o.st_calc = nc;
+      o.st_calc_at_set = true;
+      o.st_calc_at = now.sec;
+      o.st_messages = msgs;
+      status_changed = true;
+    }
+    // newStatus.Throttled = CalculatedThreshold.Threshold.IsThrottled(Used, true): one entry per threshold resource
+    const bool thr_pod = ro.throttled[q] & KT_COUNT_BIT;
+    std::map<int, bool> thr_req;
+    for (auto& kv : o.st_calc.requests) thr_req[kv.first] = (ro.throttled[q] >> kv.first) & 1;
+    const bool thr_nil = o.st_calc.requests.empty();
+    if (thr_pod != o.st_thr_pod || thr_req != o.st_thr_req) status_changed = true;
+    // apiequality.Semantic.DeepEqual (throttle_controller.go:157): an empty map IS a nil map -- a status that differs from the
+    // informer copy in nil-ness only is not written, and the copy keeps its own (found by a third random event stream, with
+    // statuses arriving through the informer: `used: {resourceRequests: {}}` on a throttle that matches no pod)
+    if (!amount_equal(o.st_used, nu)) status_changed = true;
+    if (status_changed) {  // UpdateStatus(newStatus): the whole of it replaces the copy
+      o.st_thr_pod = thr_pod;
+      o.st_thr_req = thr_req;
+      o.st_thr_req_nil = thr_nil;
+      o.st_used = nu;
+    }
+    o.metrics_pending = true;  // both branches of the status comparison record (throttle_controller.go:159,187); see record_metrics
+    if (status_changed) {
+      throttle_state_changed(t);  // PreFilter reads this status: cached verdicts of the pods it affects are void
+      status_dirty = true;
+    }
+    return status_changed;
+  }
+
   std::string reconcile_all(const std::string& now_s) {
     GoTime now;
     std::string e = parse_rfc3339(now_s, &now);
@@ -1431,55 +1485,7 @@ struct kth_plugin {
       if (selector_fails[t]) continue;                      // affectedPods fails -> reconcile returns the error, status untouched
       ++reconciled;
       const int32_t q = pos[t];  // >= 0: the device says its status changes (or the object was applied since its last reconcile)
-      if (q >= 0) {
-      o.host_dirty = false;
-      ResAmount nu;  // used := ResourceAmount{}; used = used.Add(ResourceAmountOfPod(p)) ...
-      if (used_present[q] & KT_COUNT_BIT) {
-        nu.has_counts = true;
-        nu.pod = used_cnt[q];
-        nu.requests_nil = false;
-        for (int r = 0; r < (int)cols.size(); ++r)
-          if ((used_present[q] >> r) & 1) nu.requests[r] = from_scale(r, used[(size_t)r * k + q]);
-      }
-      ResAmount nc;  // CalculateThreshold(now).Threshold
-      nc.has_counts = calc_present[q] & KT_COUNT_BIT;
-      nc.pod = nc.has_counts ? calc_cnt[q] : 0;
-      nc.requests_nil = false;
-      for (int r = 0; r < (int)cols.size(); ++r)
-        if ((calc_present[q] >> r) & 1) nc.requests[r] = from_scale(r, calc_thr[(size_t)r * k + q]);
-      if (!ovr_active[q]) nc = o.threshold;  // no active override: spec.threshold itself (keeps nil-ness and spelling)
-      const std::vector<std::string> msgs = override_messages(o);
-      bool status_changed = false;
-      if (!amount_equal(o.st_calc, nc) || o.st_messages != msgs) {  // Q6: otherwise the old calculatedAt is kept
-        o.st_calc = nc;
-        o.st_calc_at_set = true;
-        o.st_calc_at = now.sec;
-        o.st_messages = msgs;
-        status_changed = true;
-      }
-      // newStatus.Throttled = CalculatedThreshold.Threshold.IsThrottled(Used, true): one entry per threshold resource
-      const bool thr_pod = throttled[q] & KT_COUNT_BIT;
-      std::map<int, bool> thr_req;
-      for (auto& kv : o.st_calc.requests) thr_req[kv.first] = (throttled[q] >> kv.first) & 1;
-      const bool thr_nil = o.st_calc.requests.empty();
-      if (thr_pod != o.st_thr_pod || thr_req != o.st_thr_req) status_changed = true;
-      // apiequality.Semantic.DeepEqual (throttle_controller.go:157): an empty map IS a nil map -- a status that differs from the
-      // informer copy in nil-ness only is not written, and the copy keeps its own (found by a third random event stream, with
-      // statuses arriving through the informer: `used: {resourceRequests: {}}` on a throttle that matches no pod)
-      if (!amount_equal(o.st_used, nu)) status_changed = true;
-      if (status_changed) {  // UpdateStatus(newStatus): the whole of it replaces the copy
-        o.st_thr_pod = thr_pod;
-        o.st_thr_req = thr_req;
-        o.st_thr_req_nil = thr_nil;
-        o.st_used = nu;
-      }
-      o.metrics_pending = true;  // both branches of the status comparison record (throttle_controller.go:159,187); see record_metrics
-      if (status_changed) {
-        changed.push_back(o.nn());
-        throttle_state_changed(t);  // PreFilter reads this status: cached verdicts of the pods it affects are void
-        status_dirty = true;
-      }
-      }  // (q >= 0)
+      if (q >= 0 && update_status(t, ro, k, (size_t)q, now)) changed.push_back(o.nn());
       __int128 after = 0;
       if (next_override_happens_in(o, now, &after)) requeue.emplace_back(o.nn(), (long long)(after > INT64_MAX ? INT64_MAX : after));
       // unreserveAffectedPods: every affected pod the informer has observed leaves the reservation cache -- except, for a
@@ -1595,6 +1601,107 @@ struct kth_plugin {
     for (const PodObj* p : finished) w.str(p->nn());
     w.end_arr().key("queued").begin_arr();
     for (auto& q : queued) w.begin_obj().key("pod").str(q.first->nn()).key("status").str(kStatus[q.second & 3u]).end_obj();
+    w.end_arr().end_obj();
+    return w.out;
+  }
+
+  // ---- reconcile(key) for listed throttles (kth_reconcile) -----------------------------------------------------------
+  // Each distinct key gets what reconcile_all does for its throttle -- status (Q6, Semantic.DeepEqual), cached verdicts, gauges,
+  // NextOverrideHappensIn, unreserveAffectedPods (Q8) or the reachable broken-podSelector error -- from one kt_reconcile_throttles
+  // call over the listed columns only.  Throttles that are not listed are not touched.
+  std::string reconcile_keys(const std::string& keys_json, const std::string& now_s) {
+    GoTime now;
+    std::string e = parse_rfc3339(now_s, &now);
+    if (!e.empty()) fail(e);
+    ktjson::NodePtr keys = ktjson::parse(keys_json.c_str());
+    if (!keys->is(Node::Arr)) fail("reconcile: keys must be a JSON array of \"namespace/name\" (Throttle) or \"/name\" (ClusterThrottle)");
+    if (!kt_reconcile_throttles) fail("kth_reconcile: the engine this plugin is linked against has no kt_reconcile_throttles");
+    sync_all();  // (may lay the throttle columns out anew: keys are resolved after it)
+    std::vector<std::pair<std::string, std::string>> errors;
+    std::vector<std::string> not_found;
+    std::vector<std::pair<std::string, int32_t>> todo;  // key, throttle column
+    std::set<std::string> seen;
+    for (auto& kp : keys->arr) {
+      if (!kp->is(Node::Str)) fail("reconcile: every key must be a string");
+      const std::string key = kp->text;
+      if (!seen.insert(key).second) continue;
+      // cache.SplitMetaNamespaceKey, with "/name" for a ClusterThrottle (controller.go:95-101)
+      const size_t slash = key.find('/');
+      const std::string ns = slash == std::string::npos ? "" : key.substr(0, slash), tname = slash == std::string::npos ? "" : key.substr(slash + 1);
+      if (slash == std::string::npos || tname.empty() || tname.find('/') != std::string::npos) {
+        errors.emplace_back(key, "unexpected key format: \"" + key + "\"");
+        continue;
+      }
+      auto it = thr_index.find(ns.empty() ? "C:/" + tname : "T:" + ns + "/" + tname);
+      if (it == thr_index.end() || !throttles[(size_t)it->second].live) { not_found.push_back(key); continue; }  // the lister's NotFound: nil
+      if (throttles[(size_t)it->second].throttler_name != name) continue;  // only responsible throttles are ever enqueued (:403-425)
+      todo.emplace_back(key, (int32_t)it->second);
+    }
+    const size_t k = todo.size();
+    const int R = lim.n_resources;
+    std::vector<int32_t> idx(k);
+    for (size_t q = 0; q < k; ++q) idx[q] = todo[q].second;
+    std::vector<int64_t> used((size_t)R * std::max<size_t>(k, 1)), used_cnt(k), calc_thr((size_t)R * std::max<size_t>(k, 1)), calc_cnt(k);
+    std::vector<uint32_t> used_present(k), throttled(k), calc_present(k);
+    std::vector<uint8_t> ovr_active(k);
+    kt_reconcile_out ro{used.data(), used_present.data(), used_cnt.data(), throttled.data(), calc_thr.data(), calc_present.data(), calc_cnt.data(), ovr_active.data()};
+    std::vector<int64_t> off(k + 1, 0), rows;
+    int64_t cap = 1024;
+    while (k) {  // the matched rows of every listed throttle, ascending
+      rows.resize((size_t)cap);
+      check(kt_reconcile_throttles(ctx, clamp_ns(now.ns()), (int64_t)k, idx.data(), &ro, off.data(), rows.data(), cap), "kt_reconcile_throttles");
+      if (off[k] <= cap) break;
+      cap = off[k];
+    }
+    int reconciled = 0;
+    std::vector<std::string> changed;
+    std::vector<std::pair<std::string, long long>> requeue;
+    for (size_t q = 0; q < k; ++q) {
+      const size_t t = (size_t)idx[q];
+      ThrottleObj& o = throttles[t];
+      const int64_t* r0 = rows.data() + off[q];
+      const int64_t* r1 = rows.data() + off[q + 1];
+      // a counted pod that reaches a broken term: affectedPods fails, and reconcile with it -- status untouched, nothing
+      // un-reserved (throttle_controller.go:233-236); the first such pod in informer order names the error
+      const std::vector<int64_t> err_rows = selector_error_rows(o);
+      const PodObj* first = nullptr;
+      for (int64_t r : err_rows)
+        if (!std::binary_search(r0, r1, r) && (!first || pods[(size_t)r].seq < first->seq)) first = &pods[(size_t)r];
+      if (first) { errors.emplace_back(todo[q].first, reachable_selector_error(o, first->ns)); continue; }
+      ++reconciled;
+      if (update_status(t, ro, k, q, now)) changed.push_back(o.nn());
+      __int128 after = 0;
+      if (next_override_happens_in(o, now, &after)) requeue.emplace_back(o.nn(), (long long)(after > INT64_MAX ? INT64_MAX : after));
+      // unreserveAffectedPods: every affected pod the informer has observed leaves the reservation cache -- except, for a
+      // Throttle, the finished ones but the last (Q8; "last" is the order of first appearance, as in reconcile_all)
+      auto it = cache[o.kind].by_thr.find(o.nn());
+      if (it == cache[o.kind].by_thr.end()) continue;
+      int64_t last_fin = -1;
+      if (o.kind == KT_KIND_THROTTLE)
+        for (const int64_t* r = r0; r < r1; ++r) {
+          const PodObj& p = pods[(size_t)*r];
+          if (!(pod_flags(p) & KT_POD_NOT_FINISHED) && (last_fin < 0 || p.seq > pods[(size_t)last_fin].seq)) last_fin = *r;
+        }
+      std::vector<std::string> gone;
+      for (auto& pod : it->second) {
+        auto pi = pod_index.find(pod.first);
+        if (pi == pod_index.end() || !std::binary_search(r0, r1, pi->second)) continue;
+        const PodObj& p = pods[(size_t)pi->second];
+        if (o.kind == KT_KIND_THROTTLE && !(pod_flags(p) & KT_POD_NOT_FINISHED) && pi->second != last_fin) continue;
+        gone.push_back(pod.first);
+      }
+      for (auto& g : gone)
+        if (it->second.erase(g)) reservation_changed(t);
+    }
+    Writer w;
+    w.begin_obj().key("reconciled").num(reconciled).key("changed").begin_arr();
+    for (auto& c : changed) w.str(c);
+    w.end_arr().key("requeueAfterNanos").begin_obj();
+    for (auto& r : requeue) w.key(r.first).num(r.second);
+    w.end_obj().key("errors").begin_obj();
+    for (auto& er : errors) w.key(er.first).str(er.second);
+    w.end_obj().key("notFound").begin_arr();
+    for (auto& nf : not_found) w.str(nf);
     w.end_arr().end_obj();
     return w.out;
   }
@@ -2598,6 +2705,9 @@ const char* kth_delete(kth_plugin* p, const char* kind, const char* ns, const ch
 }
 const char* kth_reconcile_all(kth_plugin* p, const char* now_rfc3339) {
   return guarded(p, [&]() { return p->reconcile_all(now_rfc3339 ? now_rfc3339 : ""); });
+}
+const char* kth_reconcile(kth_plugin* p, const char* keys_json, const char* now_rfc3339) {
+  return guarded(p, [&]() { return p->reconcile_keys(keys_json ? keys_json : "", now_rfc3339 ? now_rfc3339 : ""); });
 }
 const char* kth_get_status(kth_plugin* p, const char* ns, const char* name) {
   return guarded(p, [&]() { return p->status_json(ns ? ns : "", name ? name : ""); });

@@ -862,6 +862,36 @@ __host__ __device__ inline size_t pre_record_bytes(int R) { return 16 + 16 * (si
 
 constexpr int kFinPrep = 1, kFinStatus = 2;  // the halves of a finalize tile: the fused pass runs them as separate tiles (prep first, so
                                              // that nobody ever waits for pre-records), the chained k_finalize runs both
+
+// CalculateThreshold(now) of throttle t for resource r (is_res) or the pod count: merged active overrides REPLACE
+// spec.threshold; per resource name the first active override wins (throttle_types.go:65-106).  mybit is r's presence bit
+// (KT_COUNT_BIT for the count), col = r * M + t.  The finalize tiles and the keyed reconcile (kt_keyed.cuh) share it.
+struct CalcThreshold {
+  bool spec_has, calc_has, active;
+  long long spec_val, calc_val;
+};
+__device__ __forceinline__ CalcThreshold calculate_threshold(const ThrottleView& tv, int t, int r, bool is_res, uint32_t mybit, size_t col, long long now) {
+  CalcThreshold ct;
+  ct.spec_has = tv.thr_present[t] & mybit;
+  ct.spec_val = is_res ? tv.thr[col] : tv.thr_cnt[t];
+  ct.active = false;
+  bool ov_has = false;
+  long long ov_val = 0;
+  const int o_lo = tv.ovr_off[t], o_hi = tv.ovr_off[t + 1];
+  for (int i = o_lo; i < o_hi; ++i) {
+    if (tv.ovr_flags[i] & KT_OVR_PARSE_ERROR) continue;               // skipped, reported in Messages by the host
+    if (!(tv.ovr_begin[i] <= now && now <= tv.ovr_end[i])) continue;  // IsActive: inclusive both ends
+    ct.active = true;
+    if (!ov_has && (tv.ovr_present[i] & mybit)) {
+      ov_has = true;
+      ov_val = is_res ? tv.ovr_thr[(size_t)r * tv.n_ovr + i] : tv.ovr_cnt[i];
+    }
+  }
+  ct.calc_has = ct.active ? ov_has : ct.spec_has;
+  ct.calc_val = ct.active ? ov_val : ct.spec_val;
+  return ct;
+}
+
 template <class Sync>
 __device__ __forceinline__ void finalize_tile(const ThrottleView& tv, int M, int R, int G, long long now, uint32_t eval_flags, const PartExchange& px,
                                               const ReconcileView& out, unsigned char* __restrict__ pre /* [M][pre_record_bytes(R)] */, int tile_index,
@@ -898,29 +928,13 @@ __device__ __forceinline__ void finalize_tile(const ThrottleView& tv, int M, int
     }
   }
 
-  // ---- CalculateThreshold(now): merged active overrides REPLACE spec.threshold; per resource name the first active
-  // override wins (throttle_types.go:65-106) ----
   uint32_t tflags = 0;
   bool spec_has = false, calc_has = false, active_found = false;
   long long spec_val = 0, calc_val = 0;
   if (is_res || is_cnt) {
     tflags = tv.flags[t];
-    spec_has = tv.thr_present[t] & mybit;
-    spec_val = is_res ? tv.thr[col] : tv.thr_cnt[t];
-    bool ov_has = false;
-    long long ov_val = 0;
-    const int o_lo = tv.ovr_off[t], o_hi = tv.ovr_off[t + 1];
-    for (int i = o_lo; i < o_hi; ++i) {
-      if (tv.ovr_flags[i] & KT_OVR_PARSE_ERROR) continue;               // skipped, reported in Messages by the host
-      if (!(tv.ovr_begin[i] <= now && now <= tv.ovr_end[i])) continue;  // IsActive: inclusive both ends
-      active_found = true;
-      if (!ov_has && (tv.ovr_present[i] & mybit)) {
-        ov_has = true;
-        ov_val = is_res ? tv.ovr_thr[(size_t)r * tv.n_ovr + i] : tv.ovr_cnt[i];
-      }
-    }
-    calc_has = active_found ? ov_has : spec_has;
-    calc_val = active_found ? ov_val : spec_val;
+    const CalcThreshold ct = calculate_threshold(tv, t, r, is_res, mybit, col, now);
+    spec_has = ct.spec_has; spec_val = ct.spec_val; calc_has = ct.calc_has; calc_val = ct.calc_val; active_found = ct.active;
   }
   // the threshold CheckThrottledFor compares with (throttle_types.go:128-132): this pass's, or -- GIVEN_STATUS, what
   // PreFilter sees -- the informer copy's status.calculatedThreshold when calculatedAt is set, else spec.threshold

@@ -1,0 +1,220 @@
+// kt_keyed.cuh -- reconcile(key) for k listed throttles on the device (kt_reconcile_throttles).
+//
+// The reference reconciles one key at a time (throttle_controller.go:84-211, clusterthrottle_controller.go:87-214): a key costs
+// the pods of the namespaces its throttle reaches (affectedPods, :221-246), not the whole snapshot.  Here the listed throttles'
+// 32-throttle words ("listed words", with a mask of the listed bits of each) are evaluated for the running rows whose namespace
+// can reach a listed bit, and for nothing else:
+//   1. k_keyed_reach     namespace -> which listed words it reaches (the tables' nsmask AND the listed bits), one bit per word
+//   2. k_keyed_rows      a warp reads ns / flags of 32 rows (the only O(N) traffic, 8 B per row); rows that are not counted or
+//                        whose namespace reaches nothing listed stop there.  The others evaluate the words they reach with the
+//                        pass's own word evaluation (eval_word), AND the listed mask, store the non-zero words in a compact
+//                        scratch [n][nw] and add the not-finished rows' requests into per-CTA accumulators (one warp reduction
+//                        per matched throttle, one global add per CTA and throttle)
+//   3. ColumnView        the scratch transposed into the CSR of matched rows (kt_admit.cuh: count, offsets, scan, fill)
+//   4. k_keyed_status    per listed entry: CalculateThreshold(now) (the finalize tiles' code), IsThrottled(used, true)
+// Nothing here writes a buffer another call reads: the match bitmaps, their clean flags, the partial-sum halves and the status
+// block of the last pass are left as they are.
+#pragma once
+#include "kt_kernels.cuh"
+
+namespace kt {
+
+constexpr int kKeyedTile = 128;            // rows per CTA iteration (one lane per row)
+constexpr size_t kKeyedSmemAcc = 96 * 1024;  // per-CTA accumulators up to this size; beyond it the warps add into HBM directly
+
+struct KeyedArgs {
+  PodView pods;              // the running rows (roff current)
+  TableView tb;
+  int L, R;
+  int nw;                    // listed words
+  const int32_t* words;      // [nw] word index of listed word j
+  const uint32_t* masks;     // [nw] listed bits of word j
+  const uint32_t* reach;     // [NS][NC] bit j%32 of reach[ns * NC + j/32]: namespace ns reaches a listed bit of word j
+  int NC;                    // (nw + 31) / 32
+  uint32_t* scratch;         // [n][nw] the listed bits each row matches (zeroed before the launch; counted rows only)
+  unsigned long long* used;  // [R][nw * 32] sums of the not-finished matched rows (compact throttle j * 32 + b)
+  unsigned long long* cnt;   // [nw * 32]
+  uint32_t* pres;            // [nw * 32] presence bits of those rows' requests
+  int smem_acc;              // 1: per-CTA accumulators in shared memory
+};
+
+__host__ __device__ inline size_t keyed_smem_acc_bytes(int nw, int R) { return (size_t)nw * 32 * ((size_t)R * 8 + 8 + 4); }
+__host__ __device__ inline size_t keyed_smem_bytes(int nw, int R, int L, bool reg_rows, bool smem_acc) {
+  const size_t b = (smem_acc ? keyed_smem_acc_bytes(nw, R) : 0) + (reg_rows ? 0 : (size_t)((L + 7) & ~7) * kKeyedTile * 4);
+  return (b + 15) & ~(size_t)15;
+}
+
+__global__ void __launch_bounds__(256) k_keyed_reach(const TableView tb, int nw, const int32_t* __restrict__ words, const uint32_t* __restrict__ masks,
+                                                     int NC, uint32_t* __restrict__ reach) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (int64_t)tb.NS * NC) return;
+  const int ns = (int)(i / NC), c = (int)(i % NC);
+  uint32_t bits = 0;
+  for (int jj = 0; jj < 32 && c * 32 + jj < nw; ++jj) {
+    const int j = c * 32 + jj;
+    const uint32_t* nsm = tb.nsmask + ((size_t)ns * tb.W + words[j]) * tb.TPpad;
+    uint32_t any = 0;
+    for (int s = 0; s < tb.TPpad; ++s) any |= nsm[s];
+    if (any & masks[j]) bits |= 1u << jj;
+  }
+  reach[i] = bits;
+}
+
+template <int TPC, int B, int RT, bool REG>
+__global__ void __launch_bounds__(kKeyedTile) k_keyed_rows(const KeyedArgs a) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  const int tid = threadIdx.x, lane = tid & 31;
+  const int R = a.R, NJ = a.nw * 32;
+  const int Lpad = (a.L + 7) & ~7;
+  const PodView& pods = a.pods;
+  unsigned long long* s_used = reinterpret_cast<unsigned long long*>(smem_raw);  // [R][NJ]
+  unsigned long long* s_cnt = s_used + (size_t)R * NJ;                           // [NJ]
+  uint32_t* s_pres = reinterpret_cast<uint32_t*>(s_cnt + NJ);                    // [NJ]
+  int32_t* s_rowid = reinterpret_cast<int32_t*>(smem_raw + (a.smem_acc ? keyed_smem_acc_bytes(a.nw, R) : 0));  // [Lpad][TILE] (!REG)
+  if (a.smem_acc) {
+    for (int i = tid; i < R * NJ; i += kKeyedTile) s_used[i] = 0ull;
+    for (int i = tid; i < NJ; i += kKeyedTile) { s_cnt[i] = 0ull; s_pres[i] = 0u; }
+    __syncthreads();
+  }
+  PodRows<REG> rows;
+  rows.init(s_rowid, tid, kKeyedTile);
+  const int64_t tiles = (pods.n + kKeyedTile - 1) / kKeyedTile;
+#pragma unroll 1
+  for (int64_t tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+    const int64_t p = tile * kKeyedTile + tid;
+    const bool valid = p < pods.n;
+    const int64_t pc = valid ? p : pods.n - 1;
+    const uint32_t flags = valid ? __ldg(&pods.flags[pc]) : 0u;
+    const int ns = __ldg(&pods.ns[pc]);
+    // shouldCountIn (throttle_controller.go:217-219), and a namespace that reaches a listed throttle at all
+    const bool counted = (flags & (KT_POD_SCHEDULER_MATCH | KT_POD_SCHEDULED)) == (KT_POD_SCHEDULER_MATCH | KT_POD_SCHEDULED) &&
+                         (unsigned)ns < (unsigned)a.tb.NS;
+    const uint32_t* my_reach = a.reach + (size_t)(counted ? ns : 0) * a.NC;
+    uint32_t any_reach = 0;
+    if (counted)
+      for (int c = 0; c < a.NC; ++c) any_reach |= __ldg(&my_reach[c]);
+    const bool on = counted && any_reach != 0u;
+    if (!__any_sync(kFull, on)) continue;
+    const bool alive = on && (flags & KT_POD_NOT_FINISHED);  // isNotFinished (pod_util.go:26-28)
+    const uint32_t present = on ? __ldg(&pods.present[pc]) & ~KT_COUNT_BIT : 0u;
+    long long rq[RT > 0 ? RT : 1];
+    if constexpr (RT > 0) {
+#pragma unroll
+      for (int r = 0; r < RT; ++r) rq[r] = (alive && r < R && ((present >> r) & 1)) ? __ldg(&pods.req[(int64_t)r * pods.n + pc]) : 0;
+    }
+    if (on) load_rows<REG>(pods.roff, pods.n, pc, a.L, rows);
+#pragma unroll 1
+    for (int c = 0; c < a.NC; ++c) {
+      const uint32_t bits = on ? __ldg(&my_reach[c]) : 0u;
+      uint32_t u = __reduce_or_sync(kFull, bits);
+#pragma unroll 1
+      while (u) {
+        const int j = c * 32 + __ffs(u) - 1;
+        u &= u - 1;
+        uint32_t word = 0;
+        if ((bits >> (j & 31)) & 1u) {
+          word = eval_word<TPC, B, REG>(a.tb, rows, Lpad, ns, __ldg(&a.words[j])) & __ldg(&a.masks[j]);
+          if (word) a.scratch[p * a.nw + j] = word;
+        }
+        // used = used.Add(ResourceAmountOfPod(p)) over the not-finished matched rows: lane b owns throttle (j, b) and the
+        // set of this warp's rows that matched it; each matched throttle is summed by the whole warp
+        const uint32_t T = warp_transpose32(alive ? word : 0u, lane);
+        uint32_t hit = __ballot_sync(kFull, T != 0u);
+#pragma unroll 1
+        while (hit) {
+          const int b = __ffs(hit) - 1;
+          hit &= hit - 1;
+          const uint32_t m = __shfl_sync(kFull, T, b);
+          const bool in = (m >> lane) & 1u;
+          const uint32_t pr = __reduce_or_sync(kFull, in ? present : 0u);
+          const int cj = j * 32 + b;
+          if (lane == 0) {
+            if (a.smem_acc) {
+              smem_add_u64(&s_cnt[cj], (unsigned long long)__popc(m));
+              atomicOr(&s_pres[cj], pr);
+            } else {
+              atomicAdd(&a.cnt[cj], (unsigned long long)__popc(m));
+              atomicOr(&a.pres[cj], pr);
+            }
+          }
+          for (int r = 0; r < R; ++r) {
+            long long v;
+            if constexpr (RT > 0) {
+              v = 0;
+#pragma unroll
+              for (int q = 0; q < RT; ++q)
+                if (q == r) v = rq[q];
+            } else {
+              v = (alive && ((present >> r) & 1)) ? __ldg(&pods.req[(int64_t)r * pods.n + pc]) : 0;
+            }
+            const unsigned long long s = warp_sum_u64(in ? (unsigned long long)v : 0ull);
+            if (lane == (r & 31) && s) {
+              if (a.smem_acc) smem_add_u64(&s_used[(size_t)r * NJ + cj], s);
+              else atomicAdd(&a.used[(size_t)r * NJ + cj], s);
+            }
+          }
+        }
+      }
+    }
+  }
+  if (a.smem_acc) {  // CTA accumulators -> HBM: one add per (throttle, resource) this CTA touched
+    __syncthreads();
+    for (int i = tid; i < NJ; i += kKeyedTile) {
+      if (s_cnt[i] == 0ull) continue;
+      atomicAdd(&a.cnt[i], s_cnt[i]);
+      atomicOr(&a.pres[i], s_pres[i]);
+      for (int r = 0; r < R; ++r)
+        if (s_used[(size_t)r * NJ + i]) atomicAdd(&a.used[(size_t)r * NJ + i], s_used[(size_t)r * NJ + i]);
+    }
+  }
+}
+
+// Status of listed entry e (throttle idx[e], compact accumulator cidx[e]): what a FRESH_STATUS pass reports for that column,
+// written into one packed block shaped as kt_get_reconcile_rows delivers it:
+//   {used[R][k], calc_thr[R][k], used_cnt[k], calc_cnt[k], used_present[k], throttled[k], calc_present[k], override_active[k]}
+__global__ void __launch_bounds__(128) k_keyed_status(int64_t k, const int32_t* __restrict__ idx, const int32_t* __restrict__ cidx, int R, int M, int NJ,
+                                                      const ThrottleView tv, long long now, const unsigned long long* __restrict__ used,
+                                                      const unsigned long long* __restrict__ cnt, const uint32_t* __restrict__ pres, unsigned char* __restrict__ out) {
+  const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= k) return;
+  const int t = idx[e], cj = cidx[e];
+  int64_t* o_used = reinterpret_cast<int64_t*>(out);
+  int64_t* o_calc = o_used + (size_t)R * k;
+  int64_t* o_used_cnt = o_calc + (size_t)R * k;
+  int64_t* o_calc_cnt = o_used_cnt + k;
+  uint32_t* o_used_present = reinterpret_cast<uint32_t*>(o_calc_cnt + k);
+  uint32_t* o_throttled = o_used_present + k;
+  uint32_t* o_calc_present = o_throttled + k;
+  uint8_t* o_active = reinterpret_cast<uint8_t*>(o_calc_present + k);
+  const uint32_t tflags = tv.flags[t];
+  const bool live = (tflags & KT_THR_RESPONSIBLE) && !(tflags & KT_THR_SELECTOR_ERROR);
+  const uint32_t p = pres[cj];
+  uint32_t m_used = 0, m_thr = 0, m_calc = 0;
+  bool active = false;
+  for (int r = 0; r <= R; ++r) {  // r == R: the pod count
+    const bool is_res = r < R;
+    const uint32_t mybit = is_res ? (1u << r) : KT_COUNT_BIT;
+    const CalcThreshold ct = calculate_threshold(tv, t, r, is_res, mybit, (size_t)r * M + t, now);
+    const long long used_val = (long long)(is_res ? used[(size_t)r * NJ + cj] : cnt[cj]);
+    const bool used_has = is_res ? ((p >> r) & 1u) != 0u : used_val > 0;  // Counts stays nil with zero counted pods (Q3)
+    // status.throttled = calculatedThreshold.IsThrottled(used, onEqual=true) (throttle_controller.go:133)
+    const bool throttled = live && ct.calc_has && used_has && used_val >= ct.calc_val;
+    if (used_has) m_used |= mybit;
+    if (throttled) m_thr |= mybit;
+    if (ct.calc_has) m_calc |= mybit;
+    active = ct.active;
+    if (is_res) {
+      o_used[(size_t)r * k + e] = used_val;
+      o_calc[(size_t)r * k + e] = ct.calc_val;
+    } else {
+      o_used_cnt[e] = used_val;
+      o_calc_cnt[e] = ct.calc_val;
+    }
+  }
+  o_used_present[e] = m_used;
+  o_throttled[e] = m_thr;
+  o_calc_present[e] = m_calc;
+  o_active[e] = active;
+}
+
+}  // namespace kt
