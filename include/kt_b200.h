@@ -433,6 +433,28 @@ typedef struct kt_pass_plan {
 int kt_debug_set_pass_plan(kt_ctx* ctx, const kt_pass_plan* plan);
 int kt_debug_get_pass_plan(kt_ctx* ctx, kt_pass_plan* last);
 
+/* ---- row order of the pod tables ------------------------------------------------------ */
+/* A pass costs far more when the 32 rows of a warp belong to many namespaces than when they share one.  So the engine may STORE
+ * the rows of a kind in another order than the caller uploaded them: sorted by namespace id (stable: rows of one namespace keep
+ * the caller's order; rows whose ns lies outside [0, n_ns) form one group at the end).  Every row number that crosses this ABI,
+ * in either direction, stays the caller's, and no result changes; only where each row sits in HBM does.
+ * The rule, applied on every full upload (kt_upload_pods, _compact, _packed, and so kt_step_submit): the host reads a strided
+ * sample of at most 64 groups of 32 consecutive rows from the caller's ns / meta column.  A group is mixed when its rows with
+ * flags != 0 hold more than one namespace (empty and deleted rows carry any ns).  When more than one sampled group in four is
+ * mixed the rows are laid out by namespace, otherwise as given (rows already sorted by namespace are mixed only at namespace
+ * boundaries).  The sample costs no device round trip and no synchronisation.  Row deltas (kt_update_pod_rows) never change
+ * the layout: a row that moves to another namespace stays in its slot (correct, only slower) until the next full upload.
+ * Test seam, like kt_debug_set_pass_plan: no product path sets a row order.
+ *   kt_debug_set_row_order   mode KT_ROW_ORDER_*, applies from the next full upload of the kind (KT_ERR_INVALID for a bad kind
+ *                            or mode).
+ *   kt_debug_get_row_order   the layout now resident: *clustered = 1 when laid out by namespace; dev_row[i] (NULL or [n]) = the
+ *                            device row of caller row i (i itself when as given). */
+#define KT_ROW_ORDER_AUTO 0
+#define KT_ROW_ORDER_AS_GIVEN 1
+#define KT_ROW_ORDER_BY_NAMESPACE 2
+int kt_debug_set_row_order(kt_ctx* ctx, int kind, int mode);
+int kt_debug_get_row_order(kt_ctx* ctx, int kind, int64_t* dev_row /*[n] or NULL*/, int32_t* clustered);
+
 /* ---- multi-GPU (row-sharded snapshot, one context per GPU) --------------------- */
 /* Each context holds a row shard of both pod kinds and a replica of the throttles; the
  * only exchange is one int64 sum all-reduce of the per-throttle partials between the

@@ -30,7 +30,7 @@ class KtError(RuntimeError):
 
 def build(force: bool = False) -> str:
     """Compile csrc/ for sm_90a in-tree (nvcc cross-compiles without a GPU)."""
-    srcs = [os.path.join(_HERE, "csrc", f) for f in ("kt_engine.cu", "kt_tables.cc", "kt_host.cc", "kt_kernels.cuh", "kt_admit.cuh", "kt_keyed.cuh", "kt_tables.h", "kt_json.h", "kt_quantity.h")]
+    srcs = [os.path.join(_HERE, "csrc", f) for f in ("kt_engine.cu", "kt_tables.cc", "kt_host.cc", "kt_kernels.cuh", "kt_admit.cuh", "kt_keyed.cuh", "kt_order.cuh", "kt_tables.h", "kt_json.h", "kt_quantity.h")]
     srcs.append(os.path.join(_HERE, "..", "include", "kt_b200.h"))
     srcs.append(os.path.join(_HERE, "..", "include", "kt_host.h"))
     newest = max(os.path.getmtime(s) for s in srcs)
@@ -46,6 +46,7 @@ EXPORTS = [
     "kt_upload_throttles", "kt_upload_status", "kt_set_reserved", "kt_evaluate", "kt_get_reconcile",
     "kt_match_words", "kt_get_match_bitmap", "kt_get_match_rows", "kt_get_match_columns", "kt_reconcile_throttles", "kt_get_check", "kt_set_sparse_check", "kt_get_check_sparse", "kt_get_check_rows", "kt_get_changed", "kt_get_reconcile_rows", "kt_step_submit", "kt_step_wait", "kt_admit_queue", "kt_get_timing", "kt_comm_unique_id",
     "kt_comm_init", "kt_comm_destroy", "kt_debug_compile_tables", "kt_debug_set_pass_plan", "kt_debug_get_pass_plan",
+    "kt_debug_set_row_order", "kt_debug_get_row_order",
 ]
 
 
@@ -109,6 +110,8 @@ def lib():
                                               vp, vp, vp, vp, vp, vp, vp, vp, vp]
         L.kt_debug_set_pass_plan.argtypes = [vp, C.POINTER(abi.PassPlan)]
         L.kt_debug_get_pass_plan.argtypes = [vp, C.POINTER(abi.PassPlan)]
+        L.kt_debug_set_row_order.argtypes = [vp, C.c_int, C.c_int]
+        L.kt_debug_get_row_order.argtypes = [vp, C.c_int, vp, C.POINTER(C.c_int32)]
         _lib = L
     return _lib
 
@@ -202,6 +205,20 @@ class Engine:
         plan = abi.PassPlan()
         self._ck(self._L.kt_debug_get_pass_plan(self._h, C.byref(plan)))
         return plan
+
+    def set_row_order(self, kind: int, mode: int):
+        """Test seam: store the rows of `kind` as given (abi.ROW_ORDER_AS_GIVEN), by namespace (abi.ROW_ORDER_BY_NAMESPACE) or as
+        the engine chooses from the rows (abi.ROW_ORDER_AUTO, the default), from the next full upload on (kt_debug_set_row_order)."""
+        self._ck(self._L.kt_debug_set_row_order(self._h, kind, mode))
+
+    def row_order(self, kind: int):
+        """(clustered, dev_row[n]) of the resident rows of `kind`: whether they are laid out by namespace, and the device row of
+        every caller row (kt_debug_get_row_order)."""
+        n = self.n[kind] if kind in (abi.PODS_RUNNING, abi.PODS_PENDING) else 0
+        dev_row = np.zeros(max(n, 1), np.int64)
+        clustered = C.c_int32(0)
+        self._ck(self._L.kt_debug_get_row_order(self._h, kind, abi.ptr(dev_row), C.byref(clustered)))
+        return bool(clustered.value), dev_row[:n]
 
     # -- uploads ------------------------------------------------------------------------------
     def upload_pods(self, kind: int, pods: PodCols):

@@ -77,6 +77,7 @@ class Timing(C.Structure):
 
 
 PLAN_DECIDE_QUAD, PLAN_DECIDE_PER_POD = 1, 2
+ROW_ORDER_AUTO, ROW_ORDER_AS_GIVEN, ROW_ORDER_BY_NAMESPACE = 0, 1, 2  # kt_debug_set_row_order (test seam of the row layout)
 
 
 class PassPlan(C.Structure):  # kt_pass_plan (test seam of the fused pass: kt_debug_set_pass_plan / kt_debug_get_pass_plan)

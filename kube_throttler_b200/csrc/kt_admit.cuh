@@ -50,6 +50,7 @@ struct ColumnView {
   int64_t* rows;           // [off[k]]
   const uint32_t* codes;   // [n][2Wp] 2-bit codes to gather beside the rows, or nullptr
   uint8_t* codes_out;      // [off[k]]
+  const uint32_t* rowmap;  // caller row -> bitmap row of a table laid out by namespace (kt_order.cuh), or nullptr: the same row
 };
 
 template <bool FILL>
@@ -70,7 +71,7 @@ __device__ __forceinline__ void col_walk(const ColumnView& v) {
   for (int64_t base = lo; base < hi; base += 32) {
     const int64_t i = base + lane;
     const bool on = i < hi;
-    const int64_t p = v.first + i;
+    const int64_t p = !v.rowmap ? v.first + i : on ? (int64_t)__ldg(&v.rowmap[v.first + i]) : 0;
     int wcur = -1;
     uint32_t x = 0u;
     for (int e = 0; e < ne; ++e) {
@@ -147,7 +148,10 @@ struct AdmitView {
   uint32_t* codes;                 // [n][2Wp] (rows of the pending table)
   unsigned char* admit;            // [n]
   uint32_t* counters;              // [0] undecided pods after the last update, [1] admitted
+  const uint32_t* rowmap;          // caller row -> row of the pending columns when they are laid out by namespace, or nullptr
 };
+// the pending row of queue position i: the queue is in caller rows
+__device__ __forceinline__ int64_t admit_row(const AdmitView& a, int64_t i) { return a.rowmap ? (int64_t)a.rowmap[a.first + i] : a.first + i; }
 
 // start of a round: every pod forgets last round's pair verdicts; the code words of its affected throttles are cleared (the
 // pairs OR their codes back in)
@@ -155,7 +159,7 @@ __global__ void __launch_bounds__(256) k_admit_begin(AdmitView a) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= a.count) return;
   a.fail[i] = 0u;
-  const int64_t p = a.first + i;
+  const int64_t p = admit_row(a, i);
   for (int w = 0; w < a.W; ++w)
     if (a.bitmap[p * a.Wp + w]) *reinterpret_cast<uint2*>(&a.codes[p * 2 * a.Wp + 2 * w]) = make_uint2(0u, 0u);
   if (i == 0) { a.counters[0] = 0u; a.counters[1] = 0u; }
@@ -216,7 +220,7 @@ __global__ void __launch_bounds__(128) k_admit_round(AdmitView a) {
   for (int64_t at = lo; at < hi; at += 32) {
     const bool on = at + lane < hi;
     const int64_t i = on ? a.tl_pod[at + lane] : 0;
-    const int64_t p = a.first + i;
+    const int64_t p = admit_row(a, i);
     const uint8_t st = on ? a.state[i] : kRejected;
     const uint32_t present = on ? a.present[p] : 0u;
     long long v[RMAX];
@@ -295,7 +299,7 @@ __global__ void __launch_bounds__(256) k_admit_update(AdmitView a) {
   }
   if (st == kUndecided) atomicAdd(&a.counters[0], 1u);
   if (st == kAdmitted) atomicAdd(&a.counters[1], 1u);
-  a.admit[a.first + i] = st == kAdmitted;
+  a.admit[admit_row(a, i)] = st == kAdmitted;
 }
 
 }  // namespace kt

@@ -19,6 +19,7 @@
 #include "kt_kernels.cuh"
 #include "kt_admit.cuh"
 #include "kt_keyed.cuh"
+#include "kt_order.cuh"
 #include "kt_tables.h"
 
 namespace {
@@ -62,9 +63,18 @@ struct PodStore {
   // and nothing else.  Whatever can leave a stale non-zero word outside those lists -- new rows, a row delta, new tables, a
   // buffer that was just allocated -- clears this flag; the next pass zeroes the buffers once before it runs.
   bool bitmap_clean = false;
+  // Row order (kt_order.cuh): with `clustered` the columns above hold the caller's rows sorted by namespace, o_caller[device
+  // row] = caller row and o_dev[caller row] = device row; without it no map exists and device row == caller row.
+  bool clustered = false;
+  int order_mode = 0;                        // kt_debug_set_row_order: 0 automatic, 1 as given, 2 by namespace
+  DevBuf o_caller, o_dev, o_scratch;         // the maps; sort keys, ping-pong buffers and digit histograms
+  DevBuf g_labels, g_req, g_present, g_flags, g_ns;  // the other half of each column: a re-layout gathers into it and swaps
   void release() {
     labels.release(); req.release(); present.release(); flags.release(); ns.release(); bitmap.release(); roff.release(); winfo.release();
+    o_caller.release(); o_dev.release(); o_scratch.release();
+    g_labels.release(); g_req.release(); g_present.release(); g_flags.release(); g_ns.release();
     roff_valid = false;
+    clustered = false;
     c_labels.release(); c_req.release(); c_meta.release(); c_pairs.release(); c_dict.release();
     t_rows.release(); t_labels.release(); t_req.release(); t_present.release(); t_flags.release(); t_ns.release(); t_words.release();
   }
@@ -310,6 +320,115 @@ int ensure_roff(kt_ctx* c, PodStore& s) {
   int rc = translate_rows(c, s, s.n, nullptr);
   if (rc) return rc;
   s.roff_valid = true;
+  return KT_OK;
+}
+
+// ---- row order (kt_order.cuh) --------------------------------------------------------------------------------------
+// The layout of a full upload, chosen on the host from the caller's own arrays, with no device round trip: a strided sample of
+// at most kOrderSampleGroups groups of 32 consecutive rows.  A group is mixed when its rows with flags != 0 hold more than one
+// namespace (empty and deleted rows carry arbitrary namespaces).  More than one sampled group in kOrderMixedDiv mixed: the rows
+// are laid out by namespace; otherwise as given.  Rows sorted by namespace are mixed only where one namespace ends and the
+// next begins.
+constexpr int64_t kOrderSampleGroups = 64;
+constexpr int64_t kOrderMixedDiv = 4;
+// row(i, &ns) stores row i's namespace and says whether its flags are non-zero
+template <class Row>
+bool choose_clustered(const PodStore& s, int64_t n, Row row) {
+  if (n <= 0 || s.order_mode == 1) return false;
+  if (s.order_mode == 2) return true;
+  const int64_t groups = n / 32;
+  if (groups == 0) return false;
+  const int64_t sample = std::min(groups, kOrderSampleGroups), stride = groups / sample;
+  int64_t mixed = 0;
+  for (int64_t g = 0; g < sample; ++g) {
+    const int64_t r0 = g * stride * 32;
+    bool seen = false, mix = false;
+    int32_t first = 0;
+    for (int j = 0; j < 32 && !mix; ++j) {
+      int32_t ns;
+      if (!row(r0 + j, &ns)) continue;
+      if (!seen) first = ns;
+      mix = seen && ns != first;
+      seen = true;
+    }
+    mixed += mix ? 1 : 0;
+  }
+  return mixed * kOrderMixedDiv > sample;
+}
+
+// The n rows just landed in the store's columns (caller order, queued on the stream) -> sorted by namespace: the maps, then
+// every row column gathered into its other half.  ns_limit bounds the namespace ids the transfer format can carry, so that
+// the radix passes cover only the digits a key can have.
+int order_rows(kt_ctx* c, PodStore& s, int64_t n, int64_t ns_limit) {
+  if (n > (int64_t)UINT32_MAX) return fail(c, KT_ERR_LIMIT, "%lld rows: a table laid out by namespace holds at most 2^32 - 1", (long long)n);
+  const int L = c->lim.label_slots, R = c->lim.n_resources, Lpad = (L + 7) & ~7;
+  const int64_t max_key = std::min<int64_t>(c->n_ns, ns_limit - 1);
+  int passes = 0;
+  while (passes < 4 && (max_key >> (8 * passes)) != 0) ++passes;
+  const int nblk = (int)((n + kOrderTile - 1) / kOrderTile);
+  const size_t hist_len = (size_t)kOrderDigits * nblk;
+  KT_CUDA(c, s.o_caller.reserve((size_t)n * 4 + 16));
+  KT_CUDA(c, s.o_dev.reserve((size_t)n * 4 + 16));
+  KT_CUDA(c, s.o_scratch.reserve(((size_t)3 * n + hist_len) * 4 + 16));
+  uint32_t* sc = s.o_scratch.as<uint32_t>();
+  uint32_t* keys[2] = {sc, sc + n};
+  uint32_t* vals[2] = {s.o_caller.as<uint32_t>(), sc + 2 * n};
+  uint32_t* hist = sc + 3 * n;
+  int cur = passes & 1;  // so that the last pass leaves the permutation in o_caller
+  const unsigned g = (unsigned)((n + 255) / 256);
+  k_order_keys<<<g, 256, 0, c->stream>>>(n, s.ns.as<int32_t>(), (uint32_t)c->n_ns, keys[cur], vals[cur]);
+  for (int d = 0; d < passes; ++d, cur ^= 1) {
+    k_order_hist<<<nblk, kOrderThreads, 0, c->stream>>>(n, keys[cur], 8 * d, hist, nblk);
+    k_order_scan<<<1, 1024, 0, c->stream>>>(hist, (int64_t)hist_len);
+    k_order_scatter<<<nblk, kOrderThreads, 0, c->stream>>>(n, keys[cur], vals[cur], 8 * d, hist, nblk, keys[cur ^ 1], vals[cur ^ 1]);
+  }
+  const uint32_t* caller_of = s.o_caller.as<uint32_t>();
+  k_order_invert<<<g, 256, 0, c->stream>>>(n, caller_of, s.o_dev.as<uint32_t>());
+  KT_CUDA(c, cudaGetLastError());
+  auto gather = [&](DevBuf& col, DevBuf& other, int cols, auto elem) -> int {
+    using T = decltype(elem);
+    KT_CUDA(c, other.reserve((size_t)cols * n * sizeof(T) + 16));
+    const int64_t e = (int64_t)cols * n;
+    k_order_gather_cols<T><<<(unsigned)((e + 255) / 256), 256, 0, c->stream>>>(n, cols, caller_of, col.as<T>(), other.as<T>());
+    KT_CUDA(c, cudaGetLastError());
+    std::swap(col, other);
+    return KT_OK;
+  };
+  int rc;
+  if ((rc = gather(s.labels, s.g_labels, Lpad, int64_t{})) || (rc = gather(s.req, s.g_req, R, int64_t{})) ||
+      (rc = gather(s.present, s.g_present, 1, uint32_t{})) || (rc = gather(s.flags, s.g_flags, 1, uint32_t{})) || (rc = gather(s.ns, s.g_ns, 1, int32_t{})))
+    return rc;
+  s.clustered = true;
+  return KT_OK;
+}
+// caller row -> device row, or nullptr when the rows are stored as given
+const uint32_t* dev_of(const PodStore& s) { return s.clustered ? s.o_dev.as<uint32_t>() : nullptr; }
+// n per-row results of `W` u32 words (bitmap rows, code rows; W = 0: one byte per row) gathered into caller order in the
+// store's staging buffer; returns it
+template <class T>
+const T* to_caller_order(kt_ctx* c, PodStore& s, const T* src, int W, size_t staging_at = 0) {
+  const int64_t e = s.n * (W ? W : 1);
+  T* dst = reinterpret_cast<T*>(s.t_words.as<unsigned char>() + staging_at);
+  if (W) k_order_gather_rows<<<(unsigned)((e + 255) / 256), 256, 0, c->stream>>>(s.n, W, s.o_dev.as<uint32_t>(), (const uint32_t*)src, (uint32_t*)dst);
+  else k_order_gather_cols<T><<<(unsigned)((e + 255) / 256), 256, 0, c->stream>>>(s.n, 1, s.o_dev.as<uint32_t>(), src, dst);
+  return dst;
+}
+// The admit bits of the last pass in caller order: d_admit itself, or gathered into the pending store's staging buffer at byte `at`.
+int admit_in_caller_order(kt_ctx* c, const unsigned char** out, size_t at = 0) {
+  PodStore& pend = c->pods[KT_PODS_PENDING];
+  *out = c->d_admit.as<unsigned char>();
+  if (!pend.clustered) return KT_OK;
+  KT_CUDA(c, pend.t_words.reserve(at + (size_t)pend.n + 16));
+  *out = to_caller_order(c, pend, *out, 0, at);
+  return KT_OK;
+}
+// the pass's sparse check entries name device rows: rewritten to caller rows once, on the stream right after the pass
+int sparse_to_caller(kt_ctx* c) {
+  const PodStore& pend = c->pods[KT_PODS_PENDING];
+  if (!c->sparse_cap || !pend.clustered || pend.n == 0) return KT_OK;
+  k_order_sparse_rows<<<(unsigned)c->sm_count * 2, 256, 0, c->stream>>>(c->d_sparse.as<uint32_t>(), c->sparse_cap, c->d_sparse.as<uint32_t>() + 4,
+                                                                       pend.o_caller.as<uint32_t>());
+  KT_CUDA(c, cudaGetLastError());
   return KT_OK;
 }
 
@@ -686,6 +805,8 @@ int kt_upload_pods(kt_ctx* c, int kind, int64_t n, const int64_t* labels, const 
   if ((rc = upload(c, s.present, present, (size_t)n))) return rc;
   if ((rc = upload(c, s.flags, flags, (size_t)n))) return rc;
   if ((rc = upload(c, s.ns, ns_id, (size_t)n))) return rc;
+  s.clustered = false;
+  if (choose_clustered(s, n, [&](int64_t i, int32_t* ns) { *ns = ns_id[i]; return flags[i] != 0; }) && (rc = order_rows(c, s, n, (int64_t)1 << 31))) return rc;
   s.n = n;
   s.roff_valid = s.bitmap_clean = false;
   c->evaluated = false;
@@ -721,6 +842,10 @@ int kt_upload_pods_compact(kt_ctx* c, int kind, int64_t n, int32_t val_bits, con
                                                                       s.flags.as<uint32_t>(), s.ns.as<int32_t>());
     KT_CUDA(c, cudaGetLastError());
   }
+  s.clustered = false;
+  if (choose_clustered(s, n, [&](int64_t i, int32_t* ns) { *ns = (int32_t)(meta[i] & 0x1fffffffu); return (meta[i] >> 29) != 0; }) &&
+      (rc = order_rows(c, s, n, (int64_t)1 << 29)))
+    return rc;
   s.n = n;
   s.roff_valid = s.bitmap_clean = false;
   c->evaluated = false;
@@ -766,6 +891,12 @@ static int upload_pods_packed_locked(kt_ctx* c, int kind, int64_t n, const kt_pa
   int err = set_device(c);
   if (err) return err;
   PodStore& s = c->pods[kind];
+  const uint32_t ns_mask = (1u << pk->ns_bits) - 1u;
+  const bool cluster = choose_clustered(s, n, [&](int64_t i, int32_t* ns) {
+    const uint32_t m = pk->meta[i];
+    *ns = (int32_t)(m & ns_mask);
+    return ((m >> pk->ns_bits) & 7u) != 0;
+  });
   KT_CUDA(c, s.labels.reserve((size_t)Lpad * n * 8 + 16));
   KT_CUDA(c, s.req.reserve((size_t)R * n * 8 + 16));
   KT_CUDA(c, s.present.reserve((size_t)n * 4 + 16));
@@ -824,8 +955,8 @@ static int upload_pods_packed_locked(kt_ctx* c, int kind, int64_t n, const kt_pa
     if (!coded)
       for (int r = 0; r < R; ++r) sh.s[r] = (unsigned char)pk->req_shift[r];
     // with tables in place the rows are translated (labels -> table row offsets, namespace -> word info) in the same kernel:
-    // one launch and one read of the labels less per upload
-    const bool fuse = c->have_throttles;
+    // one launch and one read of the labels less per upload (rows laid out by namespace are translated after the move)
+    const bool fuse = c->have_throttles && !cluster;
     if (fuse) {
       KT_CUDA(c, s.roff.reserve((size_t)Lpad * n * 4 + 16));
       KT_CUDA(c, s.winfo.reserve((size_t)n * 4 + 16));
@@ -835,11 +966,14 @@ static int upload_pods_packed_locked(kt_ctx* c, int kind, int64_t n, const kt_pa
                                                                         s.req.as<int64_t>(), s.present.as<uint32_t>(), s.flags.as<uint32_t>(), s.ns.as<int32_t>(),
                                                                         fuse ? 1 : 0, fuse ? table_view(c) : TableView{}, s.roff.as<uint32_t>(), s.winfo.as<uint32_t>());
     KT_CUDA(c, cudaGetLastError());
+    s.clustered = false;
+    if (cluster && (err = order_rows(c, s, n, (int64_t)1 << pk->ns_bits))) return err;
     s.n = n;
     s.roff_valid = fuse;
     s.bitmap_clean = false;
   } else {
     s.n = n;
+    s.clustered = false;
     s.roff_valid = s.bitmap_clean = false;
   }
   c->evaluated = false;
@@ -864,6 +998,7 @@ int kt_update_pod_rows(kt_ctx* c, int kind, int64_t k, const int64_t* rows, cons
   if ((rc = upload(c, s.t_rows, rows, (size_t)k)) || (rc = upload(c, s.t_labels, labels, (size_t)L * k)) || (rc = upload(c, s.t_req, req, (size_t)R * k)) ||
       (rc = upload(c, s.t_present, present, (size_t)k)) || (rc = upload(c, s.t_flags, flags, (size_t)k)) || (rc = upload(c, s.t_ns, ns_id, (size_t)k)))
     return rc;
+  if (s.clustered) k_order_map_rows<<<(unsigned)((k + 255) / 256), 256, 0, c->stream>>>(k, s.o_dev.as<uint32_t>(), s.t_rows.as<int64_t>());  // the layout stays
   k_scatter_rows<<<(unsigned)((k + 255) / 256), 256, 0, c->stream>>>(k, s.t_rows.as<int64_t>(), L, R, s.n, s.t_labels.as<int64_t>(), s.t_req.as<int64_t>(),
                                                                      s.t_present.as<uint32_t>(), s.t_flags.as<uint32_t>(), s.t_ns.as<int32_t>(),
                                                                      s.labels.as<int64_t>(), s.req.as<int64_t>(), s.present.as<uint32_t>(),
@@ -1112,6 +1247,7 @@ static int evaluate_locked(kt_ctx* c, int64_t now, uint32_t flags) {
       a.trace = c->d_trace.as<unsigned long long>();
     }
     KT_CUDA(c, dispatch_pass(c, a));
+    if ((rc = sparse_to_caller(c))) return rc;
     c->have_ran = true;
     run.bitmap_clean = pend.bitmap_clean = true;  // zero-filled (if need be) and written by this pass: maintained from here on
     // only a pass that waits for OTHER ranks can time out; under a forced plan the waits on its own tiles are checked as well
@@ -1163,6 +1299,7 @@ static int evaluate_locked(kt_ctx* c, int64_t now, uint32_t flags) {
     ++launches;
   }
   if (tm) KT_CUDA(c, cudaEventRecord(c->ev[4], c->stream));
+  if (do_chk && (rc = sparse_to_caller(c))) return rc;  // after the timed kernels: delivering results is not the pass
   c->last = kt_timing{};
   c->last.launches = launches;
   c->evaluated = true;
@@ -1221,10 +1358,10 @@ int kt_admit_queue(kt_ctx* c, int64_t first, int64_t count, uint32_t flags, int3
   KT_CUDA(c, c->d_adm_counters.reserve(16));
   a.state = c->d_adm_state.as<uint8_t>();
   a.fail = c->d_adm_fail.as<uint32_t>(); a.counters = c->d_adm_counters.as<uint32_t>();
-  a.codes = c->d_codes.as<uint32_t>(); a.admit = c->d_admit.as<unsigned char>();
+  a.codes = c->d_codes.as<uint32_t>(); a.admit = c->d_admit.as<unsigned char>(); a.rowmap = dev_of(pend);
   // 2. every throttle's toucher list (CSR over the queue, built once)
   ColumnView v{};
-  v.bitmap = a.bitmap; v.Wp = a.Wp; v.first = first; v.count = count; v.k = M;
+  v.bitmap = a.bitmap; v.Wp = a.Wp; v.first = first; v.count = count; v.k = M; v.rowmap = a.rowmap;
   int64_t nnz = 0;
   if ((rc = build_columns(c, v, &nnz, nullptr))) return rc;
   a.tl_off = v.off; a.tl_pod = v.rows;
@@ -1279,7 +1416,11 @@ int kt_step_submit(kt_ctx* c, int64_t n_running, const kt_packed_pods* running, 
   if (!c->ev_step) KT_CUDA(c, cudaEventCreateWithFlags(&c->ev_step, cudaEventDisableTiming));
   unsigned char* hb = reinterpret_cast<unsigned char*>(c->h_step);
   if (c->out_bytes) KT_CUDA(c, cudaMemcpyAsync(hb, c->d_out.p, c->out_bytes, cudaMemcpyDeviceToHost, c->stream));
-  if (P > 0) KT_CUDA(c, cudaMemcpyAsync(hb + off_admit, c->d_admit.p, (size_t)P, cudaMemcpyDeviceToHost, c->stream));
+  if (P > 0) {
+    const unsigned char* src;
+    if ((rc = admit_in_caller_order(c, &src))) return rc;
+    KT_CUDA(c, cudaMemcpyAsync(hb + off_admit, src, (size_t)P, cudaMemcpyDeviceToHost, c->stream));
+  }
   int64_t first = c->sparse_guess < c->sparse_cap ? c->sparse_guess : c->sparse_cap;
   if (P == 0) first = 0;
   // the count and the entries sit next to each other on the device ({count, pad to 16 B, entries}): one copy
@@ -1447,6 +1588,7 @@ int kt_get_check_rows(kt_ctx* c, int64_t k, const int64_t* rows, uint32_t* codes
   KT_CUDA(c, s.t_rows.reserve((size_t)k * 8));
   KT_CUDA(c, s.t_words.reserve((size_t)k * Wc * 4 + (size_t)k + 64));
   KT_CUDA(c, cudaMemcpyAsync(s.t_rows.p, rows, (size_t)k * 8, cudaMemcpyHostToDevice, c->stream));
+  if (s.clustered) k_order_map_rows<<<(unsigned)((k + 255) / 256), 256, 0, c->stream>>>(k, s.o_dev.as<uint32_t>(), s.t_rows.as<int64_t>());
   unsigned char* adm = s.t_words.as<unsigned char>() + (size_t)k * Wc * 4;
   k_gather_rows<<<(unsigned)((k + 7) / 8), 256, 0, c->stream>>>(k, s.t_rows.as<int64_t>(), Wc, c->d_codes.as<uint32_t>(), s.t_words.as<uint32_t>());
   k_gather_bytes<<<(unsigned)((k + 255) / 256), 256, 0, c->stream>>>(k, s.t_rows.as<int64_t>(), c->d_admit.as<unsigned char>(), adm);
@@ -1465,7 +1607,12 @@ int kt_get_match_bitmap(kt_ctx* c, int kind, uint32_t* words) {
   int rc = set_device(c);
   if (rc) return rc;
   PodStore& s = c->pods[kind];
-  if (s.n > 0) KT_CUDA(c, cudaMemcpyAsync(words, s.bitmap.p, (size_t)s.n * c->ht.Wp * 4, cudaMemcpyDeviceToHost, c->stream));
+  const uint32_t* src = s.bitmap.as<uint32_t>();
+  if (s.clustered && s.n > 0) {
+    KT_CUDA(c, s.t_words.reserve((size_t)s.n * c->ht.Wp * 4 + 16));
+    src = to_caller_order(c, s, src, c->ht.Wp);
+  }
+  if (s.n > 0) KT_CUDA(c, cudaMemcpyAsync(words, src, (size_t)s.n * c->ht.Wp * 4, cudaMemcpyDeviceToHost, c->stream));
   KT_CUDA(c, cudaStreamSynchronize(c->stream));
   return KT_OK;
 }
@@ -1485,6 +1632,7 @@ int kt_get_match_rows(kt_ctx* c, int kind, int64_t k, const int64_t* rows, uint3
   KT_CUDA(c, s.t_rows.reserve((size_t)k * 8));
   KT_CUDA(c, s.t_words.reserve((size_t)k * Wp * 4));
   KT_CUDA(c, cudaMemcpyAsync(s.t_rows.p, rows, (size_t)k * 8, cudaMemcpyHostToDevice, c->stream));
+  if (s.clustered) k_order_map_rows<<<(unsigned)((k + 255) / 256), 256, 0, c->stream>>>(k, s.o_dev.as<uint32_t>(), s.t_rows.as<int64_t>());
   k_gather_rows<<<(unsigned)((k + 7) / 8), 256, 0, c->stream>>>(k, s.t_rows.as<int64_t>(), Wp, s.bitmap.as<uint32_t>(), s.t_words.as<uint32_t>());
   KT_CUDA(c, cudaGetLastError());
   KT_CUDA(c, cudaMemcpyAsync(words, s.t_words.p, (size_t)k * Wp * 4, cudaMemcpyDeviceToHost, c->stream));
@@ -1511,6 +1659,7 @@ int kt_get_match_columns(kt_ctx* c, int kind, int64_t k, const int32_t* idx, int
   ColumnView v{};
   v.bitmap = s.bitmap.as<uint32_t>(); v.Wp = c->ht.Wp; v.first = 0; v.count = s.n; v.idx = c->d_col_idx.as<int32_t>(); v.k = k;
   v.codes = codes ? c->d_codes.as<uint32_t>() : nullptr;
+  v.rowmap = dev_of(s);
   int64_t total = 0;
   if ((rc = build_columns(c, v, &total, off, cap))) return rc;
   if (total > cap || total == 0) return KT_OK;  // off[] says how much room the rows need
@@ -1603,6 +1752,7 @@ int kt_reconcile_throttles(kt_ctx* c, int64_t now, int64_t k, const int32_t* idx
   // the matched rows: the scratch transposed (ColumnView over the compact words)
   ColumnView v{};
   v.bitmap = a.scratch; v.Wp = nw; v.first = 0; v.count = (int64_t)n; v.idx = d_cidx; v.k = k;
+  v.rowmap = dev_of(run);  // the scratch is indexed by device row; the lists come out in caller rows
   int64_t total = 0;
   if ((rc = build_columns(c, v, &total, off, cap))) return rc;  // (synchronises the stream: hb has landed)
   size_t at = 0;
@@ -1625,9 +1775,20 @@ int kt_get_check(kt_ctx* c, uint32_t* codes, uint8_t* admit) {
   int rc = set_device(c);
   if (rc) return rc;
   if ((rc = check_pass_error(c))) return rc;
-  const int64_t P = c->pods[KT_PODS_PENDING].n;
-  if (codes && P > 0) KT_CUDA(c, cudaMemcpyAsync(codes, c->d_codes.p, (size_t)P * 2 * c->ht.Wp * 4, cudaMemcpyDeviceToHost, c->stream));
-  if (admit && P > 0) KT_CUDA(c, cudaMemcpyAsync(admit, c->d_admit.p, (size_t)P, cudaMemcpyDeviceToHost, c->stream));
+  PodStore& pend = c->pods[KT_PODS_PENDING];
+  const int64_t P = pend.n;
+  const size_t code_bytes = (size_t)P * 2 * c->ht.Wp * 4;
+  const uint32_t* src_codes = c->d_codes.as<uint32_t>();
+  if (codes && P > 0 && pend.clustered) {  // caller order through the staging buffer: codes, then admit behind them
+    KT_CUDA(c, pend.t_words.reserve(code_bytes + (size_t)P + 16));
+    src_codes = to_caller_order(c, pend, src_codes, 2 * c->ht.Wp);
+  }
+  if (codes && P > 0) KT_CUDA(c, cudaMemcpyAsync(codes, src_codes, code_bytes, cudaMemcpyDeviceToHost, c->stream));
+  if (admit && P > 0) {
+    const unsigned char* src;
+    if ((rc = admit_in_caller_order(c, &src, codes ? code_bytes : 0))) return rc;
+    KT_CUDA(c, cudaMemcpyAsync(admit, src, (size_t)P, cudaMemcpyDeviceToHost, c->stream));
+  }
   KT_CUDA(c, cudaStreamSynchronize(c->stream));
   return KT_OK;
 }
@@ -1661,7 +1822,11 @@ int kt_get_check_sparse(kt_ctx* c, uint8_t* admit, uint32_t* entries, int64_t ca
   // one round trip in the common case: the count and as many entries as the last pass produced (plus slack) together
   int64_t first = c->sparse_guess < room ? c->sparse_guess : room;
   if (P == 0) first = 0;
-  if (admit && P > 0) KT_CUDA(c, cudaMemcpyAsync(admit, c->d_admit.p, (size_t)P, cudaMemcpyDeviceToHost, c->stream));
+  if (admit && P > 0) {
+    const unsigned char* src;
+    if ((rc = admit_in_caller_order(c, &src))) return rc;
+    KT_CUDA(c, cudaMemcpyAsync(admit, src, (size_t)P, cudaMemcpyDeviceToHost, c->stream));
+  }
   KT_CUDA(c, cudaMemcpyAsync(c->h_sparse_count, c->d_sparse.p, 4, cudaMemcpyDeviceToHost, c->stream));
   if (first > 0) KT_CUDA(c, cudaMemcpyAsync(entries, c->d_sparse.as<uint32_t>() + 4, (size_t)first * 12, cudaMemcpyDeviceToHost, c->stream));
   KT_CUDA(c, cudaStreamSynchronize(c->stream));
@@ -1719,6 +1884,35 @@ int kt_debug_get_pass_plan(kt_ctx* c, kt_pass_plan* last) {
   std::lock_guard<std::mutex> lk(c->mu);
   if (!c->have_ran) return fail(c, KT_ERR_STATE, "kt_debug_get_pass_plan before the first fused pass");
   *last = c->ran;
+  return KT_OK;
+}
+
+int kt_debug_set_row_order(kt_ctx* c, int kind, int mode) {
+  if (!c) return KT_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(c->mu);
+  if (kind != KT_PODS_RUNNING && kind != KT_PODS_PENDING) return fail(c, KT_ERR_INVALID, "bad pod kind %d", kind);
+  if (mode < KT_ROW_ORDER_AUTO || mode > KT_ROW_ORDER_BY_NAMESPACE) return fail(c, KT_ERR_INVALID, "row order %d: expected 0, 1 or 2", mode);
+  c->pods[kind].order_mode = mode;
+  return KT_OK;
+}
+
+int kt_debug_get_row_order(kt_ctx* c, int kind, int64_t* dev_row, int32_t* clustered) {
+  if (!c) return KT_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(c->mu);
+  if (kind != KT_PODS_RUNNING && kind != KT_PODS_PENDING) return fail(c, KT_ERR_INVALID, "bad pod kind %d", kind);
+  const PodStore& s = c->pods[kind];
+  if (clustered) *clustered = s.clustered ? 1 : 0;
+  if (!dev_row || s.n == 0) return KT_OK;
+  if (!s.clustered) {
+    for (int64_t i = 0; i < s.n; ++i) dev_row[i] = i;
+    return KT_OK;
+  }
+  int rc = set_device(c);
+  if (rc) return rc;
+  std::vector<uint32_t> map((size_t)s.n);
+  KT_CUDA(c, cudaMemcpyAsync(map.data(), s.o_dev.p, (size_t)s.n * 4, cudaMemcpyDeviceToHost, c->stream));
+  KT_CUDA(c, cudaStreamSynchronize(c->stream));
+  for (int64_t i = 0; i < s.n; ++i) dev_row[i] = map[(size_t)i];
   return KT_OK;
 }
 

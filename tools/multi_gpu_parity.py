@@ -1,5 +1,6 @@
 """Multi-GPU parity: one process per GPU (torchrun), row-sharded snapshot, ONE NCCL all-reduce per pass.
-  python -m torch.distributed.run --nnodes=1 --nproc-per-node 2 --master-addr 127.0.0.1 --master-port 29511 tools/multi_gpu_parity.py [C3] [m n p]
+  python -m torch.distributed.run --nnodes=1 --nproc-per-node 2 --master-addr 127.0.0.1 --master-port 29511 tools/multi_gpu_parity.py [C3] [m n p [arrival]]
+"arrival": the pod rows in arrival order, which every rank lays out by namespace (kt_debug_set_row_order) for its own shard.
 Rank 0 compares the stacked per-rank results with the oracle's evaluation of the WHOLE snapshot, bit for bit, and every
 rank checks that its per-throttle results equal rank 0's (they come out of the same all-reduced partials)."""
 import os
@@ -20,13 +21,18 @@ torch.cuda.set_device(local)
 dist.init_process_group("nccl", device_id=torch.device("cuda", local))
 cfg = sys.argv[1] if len(sys.argv) > 1 else "C3"
 kw = dict(m=int(sys.argv[2]), n=int(sys.argv[3]), p=int(sys.argv[4])) if len(sys.argv) > 4 else dict(m=1000, n=20011, p=2003)
-full = synth.generate(cfg, **kw)
+arrival = len(sys.argv) > 5 and sys.argv[5] == "arrival"
+full = synth.generate(cfg, **kw, sort_by_namespace=not arrival)
 mine = shard.shard_snapshot(full, rank, world)
 eng = kt.Engine(full.R, full.L, full.LN, device=local)
+if arrival:
+    for kind in (abi.PODS_RUNNING, abi.PODS_PENDING):
+        eng.set_row_order(kind, abi.ROW_ORDER_BY_NAMESPACE)
 uid = [kt.Engine.comm_unique_id() if rank == 0 else None]
 dist.broadcast_object_list(uid, src=0)
 eng.comm_init(uid[0], world, rank)
 eng.upload_snapshot(mine)
+assert not arrival or all(eng.row_order(kind)[0] for kind in (abi.PODS_RUNNING, abi.PODS_PENDING))
 results = []
 for flags in (abi.EVAL_FRESH_STATUS, abi.EVAL_ON_EQUAL):
     eng.evaluate(full.now, flags)
@@ -66,7 +72,7 @@ if rank == 0:
         if not np.array_equal(getattr(first, f), getattr(second, f)):
             ok = False
             print(f"second pass differs on {f}")
-    print(f"multi-gpu parity world={world} config={cfg} {kw}: {'OK' if ok else 'FAILED'}")
+    print(f"multi-gpu parity world={world} config={cfg} {kw} arrival={arrival}: {'OK' if ok else 'FAILED'}")
 flag = torch.tensor([1 if ok else 0], device="cuda")
 dist.broadcast(flag, src=0)
 dist.destroy_process_group()
