@@ -166,6 +166,20 @@ func (e *engine) preFilter(pod interface{}) (*preFilterResult, error) {
 	return &r, err
 }
 
+// preFilterKeysEntry is one entry of kth_pre_filter_keys: a PreFilter result, or Error for an unknown pod or a malformed key.
+type preFilterKeysEntry struct {
+	preFilterResult
+	Error string `json:"error"`
+}
+
+// preFilterKeys is PreFilter by key for pods the informer already delivered ("namespace/name"), one entry per key in order, in
+// one device call over the listed rows only.
+func (e *engine) preFilterKeys(keys []string) ([]preFilterKeysEntry, error) {
+	var r []preFilterKeysEntry
+	err := e.call(func(p *C.char) *C.char { return C.kth_pre_filter_keys(e.h, p) }, keys, &r)
+	return r, err
+}
+
 type reserveResult struct {
 	Code    string   `json:"code"`
 	Reasons []string `json:"reasons"`

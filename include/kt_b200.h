@@ -380,6 +380,17 @@ int kt_get_check_sparse(kt_ctx* ctx, uint8_t* admit /*[p]*/, uint32_t* entries /
 /* The check result of k listed pending rows only (a PreFilter caller that wants the reasons of ONE rejected pod after a pass
  * over the whole queue): codes[i][2*words_per_row] and admit[i] of rows[i].  Either output may be NULL. */
 int kt_get_check_rows(kt_ctx* ctx, int64_t k, const int64_t* rows, uint32_t* codes /*[k][2*words_per_row]*/, uint8_t* admit /*[k]*/);
+/* PreFilter for k listed pending rows (plugin.go:148-215), evaluated on the rows, tables, observed status and reservations as
+ * they are now -- uploaded or delta-updated, whether or not a pass has run since -- without a pass over the pending table.
+ * For entry i the outputs are bit for bit what kt_evaluate(ctx, 0, KT_EVAL_GIVEN_STATUS | KT_EVAL_SKIP_RECONCILE | flags)
+ * followed by kt_get_match_rows(KT_PODS_PENDING) (words) and kt_get_check_rows (codes, admit) would deliver for rows[i].
+ * flags is 0 or KT_EVAL_ON_EQUAL (KT_ERR_INVALID otherwise); a given-status check reads no clock.  rows are caller rows in
+ * [0, n) (KT_ERR_INVALID otherwise), duplicates are allowed, k = 0 is valid; any output may be NULL.  Only the listed rows are
+ * evaluated, each over the words of its own namespace; the call writes nothing another call reads (every getter answers as
+ * before it, and one that fails before kt_evaluate still fails).  KT_ERR_STATE before kt_upload_throttles, before
+ * kt_upload_status, and with a communicator (single GPU only). */
+int kt_check_pending_rows(kt_ctx* ctx, uint32_t flags, int64_t k, const int64_t* rows, uint32_t* words /*[k][words_per_row] or NULL*/,
+                          uint32_t* codes /*[k][2*words_per_row] or NULL*/, uint8_t* admit /*[k] or NULL*/);
 
 /* Device-side status diff (replaces the apiequality.Semantic.DeepEqual(thr.Status, *newStatus) of every reconcile,
  * throttle_controller.go:157 / clusterthrottle_controller.go:160): when an observed status is uploaded (kt_upload_status) every

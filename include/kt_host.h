@@ -109,6 +109,16 @@ const char* kth_pre_filter_batch(kth_plugin* p, const char* pods_json);
 const char* kth_pre_filter_key(kth_plugin* p, const char* ns, const char* name);
 const char* kth_reserve_key(kth_plugin* p, const char* ns, const char* name);
 const char* kth_unreserve_key(kth_plugin* p, const char* ns, const char* name);
+/* PreFilter by key for a list of pods, checked on the device row by row (kt_check_pending_rows): the cost follows the listed
+ * pods' own namespaces, not the length of the queue.  keys_json is a JSON array of "namespace/name" strings; the result is a
+ * JSON array with one entry per key, in the order given:
+ *   a queued pod                      exactly what kth_pre_filter_key returns at this moment (reasons in Q10 order, event,
+ *                                     affected lists, controller errors);
+ *   a pod the informer holds, not queued   the same, checked in a scratch row of the same call;
+ *   an unknown pod / a malformed key  {"error": ...}.
+ * All listed pods take one device call after the state sync every entry point does.  The cached queue verdicts are neither
+ * consulted nor refreshed (kth_queue_stats' passes and hits stay as they are); nothing is reserved and no status written. */
+const char* kth_pre_filter_keys(kth_plugin* p, const char* keys_json);
 /* PreFilter of EVERY queued pod in (at most) one device pass, no JSON: verdicts[row] = 0 free row, 1 Success,
  * 2 UnschedulableAndUnresolvable, 3 Error, for rows [0, min(cap, rows)); returns the number of queue rows (or -1, see
  * kth_last_error).  kth_queue_row gives the row of a queued pod (-1: not queued); rows are stable while the pod stays queued. */

@@ -172,6 +172,7 @@ struct kt_ctx {
   DevBuf d_col_idx, d_col_cnt, d_col_off, d_col_rows;  // per-throttle row lists (kt_admit.cuh ColumnView): kt_admit_queue, kt_get_match_columns
   DevBuf d_adm_state, d_adm_fail, d_adm_counters;      // kt_admit_queue (kt_admit.cuh)
   DevBuf d_key_list, d_key_reach, d_key_scratch, d_key_acc, d_key_out;  // kt_reconcile_throttles (kt_keyed.cuh): scratch of one call
+  DevBuf d_chk_rows, d_chk_pre, d_chk_out;  // kt_check_pending_rows (kt_keyed.cuh): scratch of one call
   DevBuf d_pre;    // [M] pre-records, finalize tiles -> decide tiles (kt_kernels.cuh pre_record_bytes)
   // per-throttle outputs of the reconcile half: ONE device block (and one pinned host mirror) so that kt_get_reconcile
   // is a single D2H copy; o_off[i] = byte offset of {used, used_cnt, calc_thr, calc_cnt, used_present, throttled,
@@ -286,6 +287,26 @@ TableView table_view(const kt_ctx* c) {
   tb.nsw_idx = c->d_nsw_idx.as<int32_t>();
   tb.M = c->ht.M; tb.W = c->ht.W; tb.Wp = c->ht.Wp; tb.TPpad = c->ht.TPpad; tb.B = c->ht.B; tb.rows = c->ht.rows; tb.NS = c->ht.NS;
   return tb;
+}
+
+ThrottleView throttle_view(const kt_ctx* c) {
+  ThrottleView tv{};
+  tv.kind = c->d_kind.as<uint8_t>(); tv.flags = c->d_tflags.as<uint8_t>();
+  tv.thr = c->d_thr.as<int64_t>(); tv.thr_present = c->d_thr_present.as<uint32_t>(); tv.thr_cnt = c->d_thr_cnt.as<int64_t>();
+  tv.ovr_off = c->d_ovr_off.as<int32_t>(); tv.ovr_begin = c->d_ovr_begin.as<int64_t>(); tv.ovr_end = c->d_ovr_end.as<int64_t>();
+  tv.ovr_flags = c->d_ovr_flags.as<uint8_t>(); tv.ovr_thr = c->d_ovr_thr.as<int64_t>(); tv.ovr_present = c->d_ovr_present.as<uint32_t>();
+  tv.ovr_cnt = c->d_ovr_cnt.as<int64_t>(); tv.n_ovr = c->n_ovr;
+  if (c->have_status) {  // GIVEN_STATUS reads it as the check's input; any reconciling pass diffs its outputs against it
+    tv.st_calculated = c->d_st_calculated.as<uint8_t>(); tv.st_calc_thr = c->d_st_calc_thr.as<int64_t>();
+    tv.st_calc_present = c->d_st_calc_present.as<uint32_t>(); tv.st_calc_cnt = c->d_st_calc_cnt.as<int64_t>();
+    tv.st_used = c->d_st_used.as<int64_t>(); tv.st_used_present = c->d_st_used_present.as<uint32_t>();
+    tv.st_used_cnt = c->d_st_used_cnt.as<int64_t>(); tv.st_throttled = c->d_st_throttled.as<uint32_t>();
+  }
+  if (c->have_reserved) {
+    tv.reserved = c->d_reserved.as<int64_t>(); tv.reserved_present = c->d_reserved_present.as<uint32_t>();
+    tv.reserved_cnt = c->d_reserved_cnt.as<int64_t>();
+  }
+  return tv;
 }
 
 PodView pod_view(const PodStore& s) {
@@ -705,7 +726,7 @@ void kt_destroy(kt_ctx* c) {
                    &c->d_st_used, &c->d_st_used_present, &c->d_st_used_cnt, &c->d_st_throttled, &c->d_reserved, &c->d_reserved_present,
                    &c->d_reserved_cnt, &c->d_part, &c->d_sync, &c->d_trace, &c->d_pre, &c->d_changed, &c->d_col_idx, &c->d_col_cnt, &c->d_col_off,
                    &c->d_col_rows, &c->d_adm_state, &c->d_adm_fail, &c->d_adm_counters, &c->d_out, &c->d_codes, &c->d_admit,
-                   &c->d_key_list, &c->d_key_reach, &c->d_key_scratch, &c->d_key_acc, &c->d_key_out};
+                   &c->d_key_list, &c->d_key_reach, &c->d_key_scratch, &c->d_key_acc, &c->d_key_out, &c->d_chk_rows, &c->d_chk_pre, &c->d_chk_out};
   if (c->h_out) cudaFreeHost(c->h_out);
   if (c->h_step) cudaFreeHost(c->h_step);
   if (c->ev_step) cudaEventDestroy(c->ev_step);
@@ -1154,22 +1175,7 @@ static int evaluate_locked(kt_ctx* c, int64_t now, uint32_t flags) {
   int launches = 0;
   const bool tm = c->timing;
 
-  ThrottleView tv{};
-  tv.kind = c->d_kind.as<uint8_t>(); tv.flags = c->d_tflags.as<uint8_t>();
-  tv.thr = c->d_thr.as<int64_t>(); tv.thr_present = c->d_thr_present.as<uint32_t>(); tv.thr_cnt = c->d_thr_cnt.as<int64_t>();
-  tv.ovr_off = c->d_ovr_off.as<int32_t>(); tv.ovr_begin = c->d_ovr_begin.as<int64_t>(); tv.ovr_end = c->d_ovr_end.as<int64_t>();
-  tv.ovr_flags = c->d_ovr_flags.as<uint8_t>(); tv.ovr_thr = c->d_ovr_thr.as<int64_t>(); tv.ovr_present = c->d_ovr_present.as<uint32_t>();
-  tv.ovr_cnt = c->d_ovr_cnt.as<int64_t>(); tv.n_ovr = c->n_ovr;
-  if (c->have_status) {  // GIVEN_STATUS reads it as the check's input; any reconciling pass diffs its outputs against it
-    tv.st_calculated = c->d_st_calculated.as<uint8_t>(); tv.st_calc_thr = c->d_st_calc_thr.as<int64_t>();
-    tv.st_calc_present = c->d_st_calc_present.as<uint32_t>(); tv.st_calc_cnt = c->d_st_calc_cnt.as<int64_t>();
-    tv.st_used = c->d_st_used.as<int64_t>(); tv.st_used_present = c->d_st_used_present.as<uint32_t>();
-    tv.st_used_cnt = c->d_st_used_cnt.as<int64_t>(); tv.st_throttled = c->d_st_throttled.as<uint32_t>();
-  }
-  if (c->have_reserved) {
-    tv.reserved = c->d_reserved.as<int64_t>(); tv.reserved_present = c->d_reserved_present.as<uint32_t>();
-    tv.reserved_cnt = c->d_reserved_cnt.as<int64_t>();
-  }
+  const ThrottleView tv = throttle_view(c);
   unsigned char* ob = c->d_out.as<unsigned char>();
   ReconcileView ov{reinterpret_cast<int64_t*>(ob + c->o_off[0]), reinterpret_cast<uint32_t*>(ob + c->o_off[4]), reinterpret_cast<int64_t*>(ob + c->o_off[1]),
                    reinterpret_cast<uint32_t*>(ob + c->o_off[5]), reinterpret_cast<int64_t*>(ob + c->o_off[2]), reinterpret_cast<uint32_t*>(ob + c->o_off[6]),
@@ -1570,6 +1576,62 @@ int kt_get_reconcile_rows(kt_ctx* c, int64_t k, const int32_t* idx, const kt_rec
   };
   take(o->used, (size_t)R * k * 8); take(o->calc_thr, (size_t)R * k * 8); take(o->used_cnt, (size_t)k * 8); take(o->calc_cnt, (size_t)k * 8);
   take(o->used_present, (size_t)k * 4); take(o->throttled, (size_t)k * 4); take(o->calc_present, (size_t)k * 4); take(o->override_active, (size_t)k);
+  return KT_OK;
+}
+
+// ---- PreFilter for k listed pending rows (kt_keyed.cuh) -------------------------------------------------------------
+int kt_check_pending_rows(kt_ctx* c, uint32_t flags, int64_t k, const int64_t* rows, uint32_t* words, uint32_t* codes, uint8_t* admit) {
+  if (!c || k < 0 || (k > 0 && !rows)) return KT_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(c->mu);
+  if (flags & ~KT_EVAL_ON_EQUAL) return fail(c, KT_ERR_INVALID, "kt_check_pending_rows: flags must be 0 or KT_EVAL_ON_EQUAL, not %u", flags);
+  if (c->comm) return fail(c, KT_ERR_STATE, "kt_check_pending_rows is single-GPU: this context has a communicator");
+  if (!c->have_throttles) return fail(c, KT_ERR_STATE, "kt_check_pending_rows before kt_upload_throttles");
+  if (!c->have_status) return fail(c, KT_ERR_STATE, "kt_check_pending_rows checks against the observed status: kt_upload_status first");
+  PodStore& pend = c->pods[KT_PODS_PENDING];
+  for (int64_t i = 0; i < k; ++i)
+    if (rows[i] < 0 || rows[i] >= pend.n) return fail(c, KT_ERR_INVALID, "row %lld out of range [0,%lld)", (long long)rows[i], (long long)pend.n);
+  if (k == 0) return KT_OK;
+  int rc = set_device(c);
+  if (rc) return rc;
+  if ((rc = ensure_roff(c, pend))) return rc;  // rows or tables changed since the offsets were translated (what the next pass does first)
+  const int M = c->M, R = c->lim.n_resources, Wp = c->ht.Wp;
+  const uint32_t eval_flags = KT_EVAL_GIVEN_STATUS | KT_EVAL_SKIP_RECONCILE | flags;
+  // the output block: admit[k] (padded to 16 B) | codes[k][2 Wp] | words[k][Wp] -- one copy fetches the prefix the caller asked for
+  const size_t adm_bytes = ((size_t)k + 15) & ~(size_t)15, code_bytes = (size_t)k * 2 * Wp * 4, word_bytes = (size_t)k * Wp * 4;
+  const size_t out_bytes = adm_bytes + code_bytes + word_bytes;
+  const size_t fetch = words ? out_bytes : codes ? adm_bytes + code_bytes : adm_bytes;
+  KT_CUDA(c, c->d_chk_rows.reserve((size_t)k * 8 + 16));
+  KT_CUDA(c, c->d_chk_out.reserve(out_bytes + 16));
+  KT_CUDA(c, cudaMemcpyAsync(c->d_chk_rows.p, rows, (size_t)k * 8, cudaMemcpyHostToDevice, c->stream));
+  KT_CUDA(c, cudaMemsetAsync(c->d_chk_out.p, 0, adm_bytes + code_bytes + word_bytes, c->stream));
+  if (M > 0) {  // the pre-records of every throttle (the pass's prep half, GIVEN_STATUS: no clock is read)
+    KT_CUDA(c, c->d_chk_pre.reserve((size_t)M * pre_record_bytes(R) + 16));
+    int G = 1;
+    while (G < R + 1) G <<= 1;
+    const long long lanes = (long long)M * G;
+    k_rows_prep<<<(unsigned)((lanes + 127) / 128), 128, 0, c->stream>>>(throttle_view(c), M, R, G, eval_flags, c->d_chk_pre.as<unsigned char>());
+    KT_CUDA(c, cudaGetLastError());
+  }
+  unsigned char* ob = c->d_chk_out.as<unsigned char>();
+  RowsArgs a{};
+  a.pods = pod_view(pend);
+  a.tb = table_view(c);
+  a.L = c->lim.label_slots; a.R = R; a.k = k;
+  a.rows = c->d_chk_rows.as<int64_t>();
+  a.dev_of = dev_of(pend);
+  a.pre = c->d_chk_pre.as<unsigned char>();
+  a.admit = ob;
+  a.codes = reinterpret_cast<uint32_t*>(ob + adm_bytes);
+  a.words = reinterpret_cast<uint32_t*>(ob + adm_bytes + code_bytes);
+  KT_CUDA(c, with_variant(c, true, [&](auto tpc, auto b, auto, auto reg) {
+    return launch(c, k_check_rows<tpc, b, reg>, (unsigned)((k + kRowsTile - 1) / kRowsTile), kRowsTile, rows_smem_bytes(a.L, R, reg), false, a);
+  }));
+  std::vector<unsigned char> hb(fetch);
+  KT_CUDA(c, cudaMemcpyAsync(hb.data(), ob, fetch, cudaMemcpyDeviceToHost, c->stream));
+  KT_CUDA(c, cudaStreamSynchronize(c->stream));
+  if (admit) std::memcpy(admit, hb.data(), (size_t)k);
+  if (codes) std::memcpy(codes, hb.data() + adm_bytes, code_bytes);
+  if (words) std::memcpy(words, hb.data() + adm_bytes + code_bytes, word_bytes);
   return KT_OK;
 }
 

@@ -26,10 +26,11 @@
 #include "kt_quantity.h"
 
 // The host layer is also linked, for CPU tests, against engine test doubles (tests/host_stub) that implement only the calls
-// the rest of this file makes: weak references let such a build load, and kth_affected_pods / kth_reconcile fail in it.  The product
-// library defines both calls in kt_engine.cu, so the references are always bound there.
+// the rest of this file makes: weak references let such a build load, and kth_affected_pods / kth_reconcile / kth_pre_filter_keys
+// fail in it.  The product library defines these calls in kt_engine.cu, so the references are always bound there.
 #pragma weak kt_get_match_columns
 #pragma weak kt_reconcile_throttles
+#pragma weak kt_check_pending_rows
 
 namespace {
 
@@ -2070,6 +2071,69 @@ struct kth_plugin {
     }
     return w.out;
   }
+  // PreFilter for a list of keys in ONE kt_check_pending_rows call over the listed rows only: each entry is what pre_filter_key
+  // would return at this moment, but nothing is read from or written to the cached queue verdicts (no pass, no hit).  Pods the
+  // informer holds that are not queued take scratch rows of the same call.
+  std::string pre_filter_keys(const std::string& keys_json) {
+    ktjson::NodePtr keys = ktjson::parse(keys_json.c_str());
+    if (!keys->is(Node::Arr)) fail("pre_filter_keys: keys must be a JSON array of \"namespace/name\" strings");
+    if (!kt_check_pending_rows) fail("kth_pre_filter_keys: the engine this plugin is linked against has no kt_check_pending_rows");
+    const size_t n = keys->arr.size();
+    std::vector<std::string> err(n), key(n);
+    std::vector<int64_t> scratch_of(n, -1);  // index into `batch` of a pod that is not queued
+    std::vector<PodObj> batch;
+    for (size_t i = 0; i < n; ++i) {
+      const Node& kp = *keys->arr[i];
+      if (!kp.is(Node::Str)) { err[i] = "pre_filter_keys: every key must be a string"; continue; }
+      key[i] = kp.text;
+      const size_t slash = key[i].find('/');
+      if (slash == std::string::npos || slash + 1 == key[i].size() || key[i].find('/', slash + 1) != std::string::npos) {
+        err[i] = "unexpected key format: \"" + key[i] + "\"";
+        continue;
+      }
+      auto it = pod_index.find(key[i]);
+      if (it == pod_index.end()) { err[i] = "pod " + key[i] + " is not in the informer cache"; continue; }
+      const PodObj& pod = pods[(size_t)it->second];
+      if (pod.pend_row < 0) { scratch_of[i] = (int64_t)batch.size(); batch.push_back(pod); }  // (value copy: the sync may re-pack)
+    }
+    // the state sync every entry point does (it may void cached verdicts, as anywhere else), then the rows as they are now
+    const bool tables_change = throttles_dirty || namespaces_dirty;
+    sync_all();
+    sync_status();
+    sync_reserved();
+    if (tables_change) queue.valid = false;
+    sync_pending(batch);
+    std::vector<int64_t> rows, at(n, -1);
+    std::vector<PodObj> who;
+    for (size_t i = 0; i < n; ++i) {
+      if (!err[i].empty()) continue;
+      at[i] = (int64_t)rows.size();
+      if (scratch_of[i] >= 0) {
+        rows.push_back(pend_capacity + scratch_of[i]);
+        who.push_back(batch[(size_t)scratch_of[i]]);
+      } else {
+        const PodObj& pod = pods[(size_t)pod_index.at(key[i])];
+        rows.push_back(pod.pend_row);
+        who.push_back(pod);
+      }
+    }
+    const size_t k = rows.size();
+    PendingResult r;
+    r.Wp = kt_match_words(ctx);
+    r.bitmap.assign(k * (size_t)r.Wp, 0);
+    r.codes.assign(k * 2 * (size_t)r.Wp, 0);
+    r.admit.assign(k, 1);
+    if (!throttles.empty() && k)  // PreFilter passes isThrottledOnEqual = false
+      check(kt_check_pending_rows(ctx, 0, (int64_t)k, rows.data(), r.bitmap.data(), r.codes.data(), r.admit.data()), "kt_check_pending_rows");
+    Writer w;
+    w.begin_arr();
+    for (size_t i = 0; i < n; ++i) {
+      if (at[i] < 0) w.begin_obj().key("error").str(err[i]).end_obj();
+      else prefilter_json(w, who[(size_t)at[i]], r, (size_t)at[i]);
+    }
+    w.end_arr();
+    return w.out;
+  }
   std::string reserve_key(const std::string& ns, const std::string& pname, bool reserve) {
     const PodObj pod = informer_pod(ns, pname);
     // which throttles the pod affects does not depend on statuses or reservations: the cached row serves as long as the pod's
@@ -2730,6 +2794,9 @@ const char* kth_pre_filter(kth_plugin* p, const char* pod_json) {
 }
 const char* kth_pre_filter_key(kth_plugin* p, const char* ns, const char* name) {
   return guarded(p, [&]() { return p->pre_filter_key(ns ? ns : "", name ? name : ""); });
+}
+const char* kth_pre_filter_keys(kth_plugin* p, const char* keys_json) {
+  return guarded(p, [&]() { return p->pre_filter_keys(keys_json ? keys_json : ""); });
 }
 const char* kth_reserve_key(kth_plugin* p, const char* ns, const char* name) {
   return guarded(p, [&]() { return p->reserve_key(ns ? ns : "", name ? name : "", true); });

@@ -1,4 +1,5 @@
-// kt_keyed.cuh -- reconcile(key) for k listed throttles on the device (kt_reconcile_throttles).
+// kt_keyed.cuh -- reconcile(key) for k listed throttles on the device (kt_reconcile_throttles), and PreFilter for k listed
+// pending rows (kt_check_pending_rows, at the end of this file).
 //
 // The reference reconciles one key at a time (throttle_controller.go:84-211, clusterthrottle_controller.go:87-214): a key costs
 // the pods of the namespaces its throttle reaches (affectedPods, :221-246), not the whole snapshot.  Here the listed throttles'
@@ -215,6 +216,100 @@ __global__ void __launch_bounds__(128) k_keyed_status(int64_t k, const int32_t* 
   o_throttled[e] = m_thr;
   o_calc_present[e] = m_calc;
   o_active[e] = active;
+}
+
+// ------------------------------------------------------------------------------------------------
+// PreFilter by key: the GIVEN_STATUS check of k listed pending rows (kt_check_pending_rows).
+//
+// PreFilter sees the informer copy of .status plus the reservations (plugin.go:148-215), so nothing it decides depends on the
+// running rows: the check of one pod costs the words of its own namespace, not a pass over the queue.
+//   1. k_rows_prep   the pass's finalize tile, prep half only (kFinPrep), into this call's own pre-records [M]: the threshold
+//                    CheckThrottledFor compares with and the given used + reserved.  In GIVEN_STATUS mode the prep half reads
+//                    no clock (status.calculatedThreshold or spec.threshold), so `now` is 0 as in the host's queue passes.
+//   2. k_check_rows  one lane per listed row (listed rows share no namespace locality): its row offsets, the words of its
+//                    namespace's list with the pass's eval_word, and each non-zero word decided pair by pair from the
+//                    pre-records (decide_word_direct_codes; in GIVEN_STATUS mode it reads no sums).
+// Outputs go to the call's own block [k][Wp] words | [k][2 Wp] codes | [k] admit, zeroed before the launch, so that every word
+// outside the row's namespace list reads 0 as in the pass's maintained rows.
+// ------------------------------------------------------------------------------------------------
+struct NoSync {  // finalize_tile's prep half signals nobody: the rows kernel is the next launch in the stream
+  __device__ __forceinline__ void wait_reconciled() const {}
+  __device__ __forceinline__ void wait_totals(const PartExchange&) const {}
+  __device__ __forceinline__ void wait_matched() const {}
+  __device__ __forceinline__ void wait_prepped() const {}
+  __device__ __forceinline__ void signal_prepped() const {}
+  __device__ __forceinline__ void signal_totals() const {}
+  __device__ __forceinline__ unsigned* error_flag() const { return nullptr; }
+};
+
+__global__ void __launch_bounds__(128) k_rows_prep(const ThrottleView tv, int M, int R, int G, uint32_t eval_flags, unsigned char* __restrict__ pre) {
+  finalize_tile(tv, M, R, G, 0, eval_flags, PartExchange{}, ReconcileView{}, pre, blockIdx.x, NoSync{}, nullptr, kFinPrep);
+}
+
+constexpr int kRowsTile = 64;  // listed rows per CTA (one lane per row)
+
+struct RowsArgs {
+  PodView pods;                  // the pending rows (roff / winfo current)
+  TableView tb;
+  int L, R;
+  int64_t k;
+  const int64_t* rows;           // [k] caller rows
+  const uint32_t* dev_of;        // caller row -> device row, or null (rows stored as given)
+  const unsigned char* pre;      // [M][pre_record_bytes(R)] from k_rows_prep
+  uint32_t* words;               // [k][Wp]
+  uint32_t* codes;               // [k][2 Wp]
+  unsigned char* admit;          // [k]
+};
+
+__host__ __device__ inline size_t rows_smem_bytes(int L, int R, bool reg_rows) {
+  return (size_t)R * kRowsTile * 8 + (reg_rows ? 0 : (size_t)((L + 7) & ~7) * kRowsTile * 4);
+}
+
+template <int TPC, int B, bool REG>
+__global__ void __launch_bounds__(kRowsTile) k_check_rows(const RowsArgs a) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  const int tid = threadIdx.x;
+  const int64_t i = (int64_t)blockIdx.x * kRowsTile + tid;
+  if (i >= a.k) return;  // (no barrier and no warp collective below: each lane works alone)
+  const int R = a.R, Wp = a.tb.Wp, Lpad = (a.L + 7) & ~7;
+  const PodView& pods = a.pods;
+  long long* s_req = reinterpret_cast<long long*>(smem_raw);                                   // [R][TILE]
+  int32_t* s_rowid = reinterpret_cast<int32_t*>(smem_raw + (size_t)R * kRowsTile * 8);        // [Lpad][TILE] (!REG)
+  const int64_t cr = __ldg(&a.rows[i]);
+  const int64_t p = a.dev_of ? (int64_t)__ldg(&a.dev_of[cr]) : cr;
+  const int ns = __ldg(&pods.ns[p]);
+  const uint32_t present = __ldg(&pods.present[p]);
+  const uint32_t winfo = __ldg(&pods.winfo[p]);
+  // ResourceAmountOfPod(pod): the non-zero requests are the only ones IsThrottledFor looks at (Q5)
+  uint32_t nz = 0;
+  for (int r = 0; r < R; ++r) {
+    long long v = __ldg(&pods.req[(int64_t)r * pods.n + p]);
+    if (!((present >> r) & 1)) v = 0;
+    s_req[r * kRowsTile + tid] = v;
+    if (v != 0) nz |= 1u << r;
+  }
+  const DecidePod pod{s_req + tid, kRowsTile, nz, p};
+  PodRows<REG> rows;
+  rows.init(s_rowid, tid, kRowsTile);
+  load_rows<REG>(pods.roff, pods.n, p, a.L, rows);
+  WordCursor wc;
+  wc.init(a.tb, winfo, ns, (unsigned)ns < (unsigned)a.tb.NS);  // a namespace out of range affects nothing
+  const PartExchange px{};  // GIVEN_STATUS: the pre-records carry everything, no sums are read
+  const size_t rec = pre_record_bytes(R);
+  uint32_t* wrow = a.words + i * Wp;
+  uint32_t* crow = a.codes + i * 2 * Wp;
+  unsigned char ok = 1;
+#pragma unroll 1
+  for (int q = 0; q < wc.cnt; ++q) {
+    const int w = wc.at(a.tb, q);
+    const uint32_t word = eval_word<TPC, B, REG>(a.tb, rows, Lpad, ns, w);
+    if (!word) continue;
+    wrow[w] = word;
+    const uint2 c = decide_word_direct_codes(word, w, a.pre, px, rec, R, a.tb.M, pod);
+    *reinterpret_cast<uint2*>(&crow[2 * w]) = c;
+    if (c.x | c.y) ok = 0;
+  }
+  a.admit[i] = ok;
 }
 
 }  // namespace kt

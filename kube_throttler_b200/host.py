@@ -27,7 +27,7 @@ def _bind(L=None):
     L.kth_free.restype = None
     for name, args in (("kth_apply", [vp, cp]), ("kth_delete", [vp, cp, cp, cp]), ("kth_reconcile_all", [vp, cp]), ("kth_reconcile", [vp, cp, cp]),
                        ("kth_get_status", [vp, cp, cp]), ("kth_get_status_manifest", [vp, cp, cp]), ("kth_affected_pods", [vp, cp, cp]), ("kth_pre_filter", [vp, cp]), ("kth_pre_filter_batch", [vp, cp]),
-                       ("kth_admit_queue", [vp, cp]), ("kth_pre_filter_key", [vp, cp, cp]), ("kth_reserve_key", [vp, cp, cp]), ("kth_unreserve_key", [vp, cp, cp]),
+                       ("kth_admit_queue", [vp, cp]), ("kth_pre_filter_key", [vp, cp, cp]), ("kth_pre_filter_keys", [vp, cp]), ("kth_reserve_key", [vp, cp, cp]), ("kth_unreserve_key", [vp, cp, cp]),
                        ("kth_queue_stats", [vp]), ("kth_reserve", [vp, cp]), ("kth_unreserve", [vp, cp]), ("kth_reserved", [vp, C.c_int, cp]), ("kth_metrics", [vp]), ("kth_eval", [cp])):
         fn = getattr(L, name)
         fn.argtypes = args
@@ -44,7 +44,7 @@ def _bind(L=None):
 
 
 HOST_EXPORTS = ["kth_new_plugin", "kth_new_plugin_error", "kth_free", "kth_apply", "kth_delete", "kth_reconcile_all", "kth_get_status", "kth_get_status_manifest",
-                "kth_pre_filter", "kth_pre_filter_key", "kth_reserve_key", "kth_unreserve_key", "kth_pre_filter_queue", "kth_queue_row", "kth_pod_row", "kth_queue_stats", "kth_last_error", "kth_pre_filter_batch", "kth_admit_queue", "kth_reserve", "kth_unreserve", "kth_reserved", "kth_metrics", "kth_eval", "kth_affected_pods", "kth_reconcile"]
+                "kth_pre_filter", "kth_pre_filter_key", "kth_reserve_key", "kth_unreserve_key", "kth_pre_filter_queue", "kth_queue_row", "kth_pod_row", "kth_queue_stats", "kth_last_error", "kth_pre_filter_batch", "kth_admit_queue", "kth_reserve", "kth_unreserve", "kth_reserved", "kth_metrics", "kth_eval", "kth_affected_pods", "kth_reconcile", "kth_pre_filter_keys"]
 
 
 def _result(raw):
@@ -122,6 +122,11 @@ class Plugin:
     # the same for pods the informer already delivered (kth_apply), addressed by key: the resident scheduling queue
     def prefilter_key(self, namespace, name):
         return _result(self._L.kth_pre_filter_key(self._h, namespace.encode(), name.encode()))
+
+    def prefilter_keys(self, keys):
+        """PreFilter by key for the listed "namespace/name" keys, checked on the device row by row: one entry per key, in order --
+        what prefilter_key returns, or {"error": ...} for an unknown pod or a malformed key (no exception for those)."""
+        return _result(self._L.kth_pre_filter_keys(self._h, json.dumps(list(keys)).encode()))
 
     def reserve_key(self, namespace, name):
         return _result(self._L.kth_reserve_key(self._h, namespace.encode(), name.encode()))
