@@ -134,6 +134,36 @@ func (e *engine) reconcileKeys(keys []string, nowRFC3339 string) (*reconcileKeys
 	return &r, nil
 }
 
+// watchEvent is one informer event as kth_apply_events takes it: Type is "ADDED", "MODIFIED" or "DELETED".
+type watchEvent struct {
+	Type   string      `json:"type"`
+	Object interface{} `json:"object"`
+}
+
+// applyEventsEntry is what kth_apply / kth_delete report for one event, plus the keys its handlers enqueue.
+type applyEventsEntry struct {
+	OK      bool     `json:"ok"`
+	Warning string   `json:"warning"`
+	Error   string   `json:"error"`
+	Enqueue []string `json:"enqueue"`
+}
+
+type applyEventsResult struct {
+	Results []applyEventsEntry `json:"results"`
+	Enqueue []string           `json:"enqueue"` // the union of the entries' keys, first appearance first
+}
+
+// applyEvents applies a batch of informer events in order and returns, per event, the reconcile keys the reference's handlers
+// enqueue ("ns/name" for a Throttle, "/name" for a ClusterThrottle), for reconcileKeys.  The pod events between two table events
+// take one device call.
+func (e *engine) applyEvents(events []watchEvent) (*applyEventsResult, error) {
+	var r applyEventsResult
+	if err := e.call(func(p *C.char) *C.char { return C.kth_apply_events(e.h, p) }, events, &r); err != nil {
+		return nil, err
+	}
+	return &r, nil
+}
+
 // statusManifest is the `status` subresource as encoding/json would render v1alpha1.ThrottleStatus.
 func (e *engine) statusManifest(ns, name string) ([]byte, error) {
 	cn, cm := C.CString(ns), C.CString(name)

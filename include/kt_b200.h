@@ -391,6 +391,19 @@ int kt_get_check_rows(kt_ctx* ctx, int64_t k, const int64_t* rows, uint32_t* cod
  * kt_upload_status, and with a communicator (single GPU only). */
 int kt_check_pending_rows(kt_ctx* ctx, uint32_t flags, int64_t k, const int64_t* rows, uint32_t* words /*[k][words_per_row] or NULL*/,
                           uint32_t* codes /*[k][2*words_per_row] or NULL*/, uint8_t* admit /*[k] or NULL*/);
+/* affectedThrottles of k pods that live only in this call (throttle_controller.go:248-269, clusterthrottle_controller.go:272-298):
+ * the pod versions an informer event carries, matched against the throttle tables as they are now.  words[i] is bit for bit what
+ * kt_get_match_rows(KT_PODS_PENDING) would return for a pending row holding labels[.][i] and ns_id[i] after a
+ * KT_EVAL_GIVEN_STATUS | KT_EVAL_SKIP_RECONCILE pass: responsible && namespace && selector match, a KT_TERM_POD_INVALID term
+ * switching the later terms off as in the pass.  Label slots are int64 codes as in kt_upload_pods / kt_update_pod_rows; a
+ * namespace id the tables do not cover (negative, or at or above both n_ns and every Throttle's namespace id + 1) gives an
+ * all-zero row, as in the pass.  Needs kt_upload_throttles (and the namespaces) only: no pods, status
+ * or reservations.  It reads no resident pod row and writes nothing another call reads (every getter answers as before it, and
+ * the context's evaluated state is unchanged).  One copy in, one launch, one copy out, one synchronisation.  k = 0 is valid;
+ * KT_ERR_INVALID for k < 0 or a null pointer with k > 0; KT_ERR_STATE before kt_upload_throttles and with a communicator
+ * (single GPU only). */
+int kt_match_pods(kt_ctx* ctx, int64_t k, const int64_t* labels /*[L][k]*/, const int32_t* ns_id /*[k]*/,
+                  uint32_t* words /*[k][words_per_row]*/);
 
 /* Device-side status diff (replaces the apiequality.Semantic.DeepEqual(thr.Status, *newStatus) of every reconcile,
  * throttle_controller.go:157 / clusterthrottle_controller.go:160): when an observed status is uploaded (kt_upload_status) every

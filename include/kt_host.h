@@ -52,6 +52,31 @@ void kth_free(kth_plugin* p);
 const char* kth_apply(kth_plugin* p, const char* manifest_json);
 const char* kth_delete(kth_plugin* p, const char* kind, const char* ns, const char* name);
 
+/* A batch of informer watch events, applied in order, with the reconcile keys the reference's handlers enqueue for each
+ * (throttle_controller.go:401-531, clusterthrottle_controller.go:429-563).  events_json is a JSON array of
+ * {"type": "ADDED" | "MODIFIED" | "DELETED", "object": manifest}: ADDED and MODIFIED are kth_apply(object), DELETED is
+ * kth_delete(object.kind, object.metadata.namespace, object.metadata.name).  Returns
+ *   {"results": [one entry per event, in order], "enqueue": [the union of the entries' keys, first appearance first]}
+ * where an entry is what kth_apply / kth_delete return for the event plus "enqueue": [keys] on success.  Keys are spelled as
+ * kth_reconcile takes them ("namespace/name" a Throttle, "/name" a ClusterThrottle), each entry's in creation order:
+ *   Throttle / ClusterThrottle applied   its own key when the NEW object's throttlerName is this plugin's
+ *   Throttle / ClusterThrottle deleted   its own key when the plugin held it and it was this plugin's
+ *   Pod applied, not held before         if shouldCountIn(new): the throttles the new version affects
+ *   Pod applied, held before             if shouldCountIn(old) || shouldCountIn(new): those of the held copy and of the new one
+ *   Pod deleted                          if shouldCountIn(old): those of the held copy
+ *   Namespace applied / deleted          nothing
+ * per controller: a controller whose affectedThrottles fails for one of those versions (a reachable broken podSelector; for
+ * ClusterThrottles also an unknown namespace) adds no key for the event, the other one's keys stand.
+ * The pod events between two Throttle / ClusterThrottle / Namespace events form a run: the distinct (namespace, label set)
+ * versions of a run take ONE kt_match_pods call and no pass over the scheduling queue; runs of pods that are not counted take
+ * no device call at all.  Afterwards the plugin is in the state kth_apply / kth_delete event by event would leave (statuses,
+ * reservations, PreFilter verdicts, affected pods, metrics, what a following reconcile returns); kth_queue_stats' passes and
+ * hits may differ.  An event those calls refuse -- and a malformed event (not an object, unknown type, no object) -- is an
+ * {"error": ...} entry, and the batch goes on.  When a run's device call fails, its events report what the single calls
+ * report when their pass fails ({"ok":true,"warning":"pod updated; reservation move skipped: ..."}; a deleted pod leaves every
+ * reservation and is an {"error": ...}; an event that only needed its keys is {"ok":true,"warning":...}), without "enqueue". */
+const char* kth_apply_events(kth_plugin* p, const char* events_json);
+
 /* reconcile(key) for EVERY responsible Throttle and ClusterThrottle in one device pass
  * (throttle_controller.go:84-211, clusterthrottle_controller.go:87-214): status.used,
  * status.calculatedThreshold (replaced only when threshold or messages changed, Q6), status.throttled

@@ -44,7 +44,7 @@ EXPORTS = [
     "kt_create", "kt_destroy", "kt_last_error", "kt_version", "kt_set_stream", "kt_sync", "kt_enable_timing",
     "kt_enable_trace", "kt_get_trace", "kt_host_alloc", "kt_host_alloc_upload", "kt_host_free", "kt_upload_pods", "kt_upload_pods_compact", "kt_upload_pods_packed", "kt_set_async_uploads", "kt_update_pod_rows", "kt_upload_namespaces",
     "kt_upload_throttles", "kt_upload_status", "kt_set_reserved", "kt_evaluate", "kt_get_reconcile",
-    "kt_match_words", "kt_get_match_bitmap", "kt_get_match_rows", "kt_get_match_columns", "kt_reconcile_throttles", "kt_get_check", "kt_set_sparse_check", "kt_get_check_sparse", "kt_get_check_rows", "kt_check_pending_rows", "kt_get_changed", "kt_get_reconcile_rows", "kt_step_submit", "kt_step_wait", "kt_admit_queue", "kt_get_timing", "kt_comm_unique_id",
+    "kt_match_words", "kt_get_match_bitmap", "kt_get_match_rows", "kt_get_match_columns", "kt_reconcile_throttles", "kt_get_check", "kt_set_sparse_check", "kt_get_check_sparse", "kt_get_check_rows", "kt_check_pending_rows", "kt_match_pods", "kt_get_changed", "kt_get_reconcile_rows", "kt_step_submit", "kt_step_wait", "kt_admit_queue", "kt_get_timing", "kt_comm_unique_id",
     "kt_comm_init", "kt_comm_destroy", "kt_debug_compile_tables", "kt_debug_set_pass_plan", "kt_debug_get_pass_plan",
     "kt_debug_set_row_order", "kt_debug_get_row_order",
 ]
@@ -88,6 +88,7 @@ def lib():
         L.kt_get_check_rows.argtypes = [vp, C.c_int64, vp, vp, vp]
         L.kt_get_match_rows.argtypes = [vp, C.c_int, C.c_int64, vp, vp]
         L.kt_check_pending_rows.argtypes = [vp, C.c_uint32, C.c_int64, vp, vp, vp, vp]
+        L.kt_match_pods.argtypes = [vp, C.c_int64, vp, vp, vp]
         L.kt_get_changed.argtypes = [vp, vp, C.c_int64, C.POINTER(C.c_int64), vp]
         L.kt_get_reconcile_rows.argtypes = [vp, C.c_int64, vp, C.POINTER(abi.ReconcileOut)]
         L.kt_update_pod_rows.argtypes = [vp, C.c_int, C.c_int64, vp, vp, vp, vp, vp, vp]
@@ -369,6 +370,18 @@ class Engine:
         flags = abi.EVAL_ON_EQUAL if on_equal else 0
         self._ck(self._L.kt_check_pending_rows(self._h, flags, k, abi.ptr(rows), abi.ptr(words), abi.ptr(codes), abi.ptr(admit)))
         return words, codes, admit
+
+    def match_pods(self, labels, ns_id) -> np.ndarray:
+        """affectedThrottles of k pods given by value (label codes [L][k], namespace ids [k]), matched against the tables as they
+        are now: words[k][W], what match_rows(PENDING) returns for pending rows holding the same labels and namespaces."""
+        labels = np.ascontiguousarray(labels, np.int64).reshape(self.Lslots, -1)
+        ns_id = np.ascontiguousarray(ns_id, np.int32)
+        k = ns_id.shape[0]
+        if labels.shape[1] != k:
+            raise ValueError(f"labels has {labels.shape[1]} pods, ns_id {k}")
+        words = np.zeros((k, self.words_per_row), np.uint32)
+        self._ck(self._L.kt_match_pods(self._h, k, abi.ptr(labels), abi.ptr(ns_id), abi.ptr(words)))
+        return words
 
     def match_rows(self, kind: int, rows: np.ndarray) -> np.ndarray:
         """words[k][words_per_row]: the match bitmap rows of the listed rows of a kind, gathered on the device."""

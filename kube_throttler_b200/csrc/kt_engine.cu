@@ -173,6 +173,7 @@ struct kt_ctx {
   DevBuf d_adm_state, d_adm_fail, d_adm_counters;      // kt_admit_queue (kt_admit.cuh)
   DevBuf d_key_list, d_key_reach, d_key_scratch, d_key_acc, d_key_out;  // kt_reconcile_throttles (kt_keyed.cuh): scratch of one call
   DevBuf d_chk_rows, d_chk_pre, d_chk_out;  // kt_check_pending_rows (kt_keyed.cuh): scratch of one call
+  DevBuf d_mp_in, d_mp_out;                 // kt_match_pods (kt_keyed.cuh): scratch of one call
   DevBuf d_pre;    // [M] pre-records, finalize tiles -> decide tiles (kt_kernels.cuh pre_record_bytes)
   // per-throttle outputs of the reconcile half: ONE device block (and one pinned host mirror) so that kt_get_reconcile
   // is a single D2H copy; o_off[i] = byte offset of {used, used_cnt, calc_thr, calc_cnt, used_present, throttled,
@@ -726,7 +727,8 @@ void kt_destroy(kt_ctx* c) {
                    &c->d_st_used, &c->d_st_used_present, &c->d_st_used_cnt, &c->d_st_throttled, &c->d_reserved, &c->d_reserved_present,
                    &c->d_reserved_cnt, &c->d_part, &c->d_sync, &c->d_trace, &c->d_pre, &c->d_changed, &c->d_col_idx, &c->d_col_cnt, &c->d_col_off,
                    &c->d_col_rows, &c->d_adm_state, &c->d_adm_fail, &c->d_adm_counters, &c->d_out, &c->d_codes, &c->d_admit,
-                   &c->d_key_list, &c->d_key_reach, &c->d_key_scratch, &c->d_key_acc, &c->d_key_out, &c->d_chk_rows, &c->d_chk_pre, &c->d_chk_out};
+                   &c->d_key_list, &c->d_key_reach, &c->d_key_scratch, &c->d_key_acc, &c->d_key_out, &c->d_chk_rows, &c->d_chk_pre, &c->d_chk_out,
+                   &c->d_mp_in, &c->d_mp_out};
   if (c->h_out) cudaFreeHost(c->h_out);
   if (c->h_step) cudaFreeHost(c->h_step);
   if (c->ev_step) cudaEventDestroy(c->ev_step);
@@ -1632,6 +1634,40 @@ int kt_check_pending_rows(kt_ctx* c, uint32_t flags, int64_t k, const int64_t* r
   if (admit) std::memcpy(admit, hb.data(), (size_t)k);
   if (codes) std::memcpy(codes, hb.data() + adm_bytes, code_bytes);
   if (words) std::memcpy(words, hb.data() + adm_bytes + code_bytes, word_bytes);
+  return KT_OK;
+}
+
+// ---- affectedThrottles of k pods given by value (kt_keyed.cuh) ------------------------------------------------------
+int kt_match_pods(kt_ctx* c, int64_t k, const int64_t* labels, const int32_t* ns_id, uint32_t* words) {
+  if (!c || k < 0) return KT_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(c->mu);
+  const int L = c->lim.label_slots;
+  if (k > 0 && ((L > 0 && !labels) || !ns_id || !words)) return fail(c, KT_ERR_INVALID, "kt_match_pods: null pointer with k = %lld", (long long)k);
+  if (c->comm) return fail(c, KT_ERR_STATE, "kt_match_pods is single-GPU: this context has a communicator");
+  if (!c->have_throttles) return fail(c, KT_ERR_STATE, "kt_match_pods before kt_upload_throttles");
+  if (k == 0) return KT_OK;
+  int rc = set_device(c);
+  if (rc) return rc;
+  const int Wp = c->ht.Wp;
+  // the inputs in one copy: labels [L][k] | ns [k]
+  const size_t lab_bytes = (size_t)L * k * 8, in_bytes = lab_bytes + (size_t)k * 4;
+  std::vector<unsigned char> hin(in_bytes);
+  if (lab_bytes) std::memcpy(hin.data(), labels, lab_bytes);
+  std::memcpy(hin.data() + lab_bytes, ns_id, (size_t)k * 4);
+  KT_CUDA(c, c->d_mp_in.reserve(in_bytes + 16));
+  KT_CUDA(c, c->d_mp_out.reserve((size_t)k * Wp * 4 + 16));
+  KT_CUDA(c, cudaMemcpyAsync(c->d_mp_in.p, hin.data(), in_bytes, cudaMemcpyHostToDevice, c->stream));
+  MatchArgs a{};
+  a.tb = table_view(c);
+  a.L = L; a.k = k;
+  a.labels = c->d_mp_in.as<int64_t>();
+  a.ns = reinterpret_cast<const int32_t*>(c->d_mp_in.as<unsigned char>() + lab_bytes);
+  a.words = c->d_mp_out.as<uint32_t>();
+  KT_CUDA(c, with_variant(c, true, [&](auto tpc, auto b, auto, auto reg) {
+    return launch(c, k_match_pods<tpc, b, reg>, (unsigned)((k + kRowsTile - 1) / kRowsTile), kRowsTile, match_smem_bytes(L, reg), false, a);
+  }));
+  KT_CUDA(c, cudaMemcpyAsync(words, a.words, (size_t)k * Wp * 4, cudaMemcpyDeviceToHost, c->stream));
+  KT_CUDA(c, cudaStreamSynchronize(c->stream));
   return KT_OK;
 }
 

@@ -27,10 +27,11 @@
 
 // The host layer is also linked, for CPU tests, against engine test doubles (tests/host_stub) that implement only the calls
 // the rest of this file makes: weak references let such a build load, and kth_affected_pods / kth_reconcile / kth_pre_filter_keys
-// fail in it.  The product library defines these calls in kt_engine.cu, so the references are always bound there.
+// / kth_apply_events fail in it.  The product library defines these calls in kt_engine.cu, so the references are always bound there.
 #pragma weak kt_get_match_columns
 #pragma weak kt_reconcile_throttles
 #pragma weak kt_check_pending_rows
+#pragma weak kt_match_pods
 
 namespace {
 
@@ -2305,8 +2306,8 @@ struct kth_plugin {
   }
 
   // ---- informer events --------------------------------------------------------------------------------
-  void apply_pod(const Node& v) {
-    PodObj p = pod_from(v);
+  // The informer's copy of a pod is replaced (or added): returns whether the plugin held the pod before, with that copy in *old.
+  bool store_pod(PodObj p, PodObj* old) {
     auto it = pod_index.find(p.nn());
     if (it == pod_index.end()) {
       const int64_t row = alloc_row(p.ns);
@@ -2317,26 +2318,45 @@ struct kth_plugin {
       pods[(size_t)row] = std::move(p);
       dirty_rows.insert(row);
       queue_update(row);
-      return;
+      return false;
     }
-    // The informer's copy is replaced FIRST: the pass below only asks which throttles the old and the new pod match, which
-    // does not depend on the running rows, and an update that repairs a snapshot the packer refuses (column overflow) must
-    // not be refused for it.
     const int64_t row = it->second;
-    const PodObj old = pods[(size_t)row];
+    *old = pods[(size_t)row];
     p.row = row;
-    p.seq = old.seq;
-    p.pend_row = old.pend_row;
-    totals_add(old, -1);
+    p.seq = old->seq;
+    p.pend_row = old->pend_row;
+    totals_add(*old, -1);
     totals_add(p, +1);
     pods[(size_t)row] = std::move(p);
     dirty_rows.insert(row);
     queue_update(row);
-    const PodObj& cur = pods[(size_t)row];
-    // UpdateFunc (throttle_controller.go:459-507): the throttle assignment can only change with labels / namespace;
-    // then the pod's reservation moves from (old \ new) to (new \ old) throttles
-    const bool relevant = should_count_in(old) || should_count_in(cur);
-    if (relevant && !throttles.empty() && old.labels != cur.labels) {
+    return true;
+  }
+  // UpdateFunc (throttle_controller.go:459-507): the throttle assignment can only change with labels / namespace;
+  // then the pod's reservation moves from (old \ new) to (new \ old) throttles
+  bool moves_reservation(const PodObj& old, const PodObj& cur) const {
+    return (should_count_in(old) || should_count_in(cur)) && !throttles.empty() && old.labels != cur.labels;
+  }
+  void move_reservation(const PodObj& old, const PodObj& now, const RowView& ro, const RowView& rn) {
+    for (int kind = 0; kind < 2; ++kind) {
+      if (!controller_error(old, ro, kind).empty() || !controller_error(now, rn, kind).empty()) continue;  // HandleError + return
+      const std::vector<int> a = affected(ro, kind), b = affected(rn, kind);
+      for (int t : a)
+        if (std::find(b.begin(), b.end(), t) == b.end()) { cache[kind].remove(throttles[(size_t)t].nn(), now.nn()); reservation_changed((size_t)t); }
+      for (int t : b)
+        if (std::find(a.begin(), a.end(), t) == a.end()) { cache[kind].add(throttles[(size_t)t].nn(), now); reservation_changed((size_t)t); }
+    }
+  }
+  void apply_pod(const Node& v) {
+    // The informer's copy is replaced FIRST: the pass below only asks which throttles the old and the new pod match, which
+    // does not depend on the running rows, and an update that repairs a snapshot the packer refuses (column overflow) must
+    // not be refused for it.
+    PodObj old;
+    PodObj p = pod_from(v);
+    const int64_t slot = pod_index.count(p.nn()) ? pod_index.at(p.nn()) : -1;
+    if (!store_pod(std::move(p), &old)) return;
+    const PodObj& cur = pods[(size_t)slot];
+    if (moves_reservation(old, cur)) {
       const PodObj now = cur;  // check_pending may re-create the engine; keep value copies
       // From here on the update IS committed (pods[row] holds the new object, resource names it brought stay interned): the
       // reference's UpdateFunc cannot refuse an event either -- when it fails to work out the throttles it logs and returns
@@ -2350,48 +2370,284 @@ struct kth_plugin {
         apply_warning = std::string("pod updated; reservation move skipped: ") + e.what();
         return;
       }
-      for (int kind = 0; kind < 2; ++kind) {
-        if (!controller_error(old, r, 0, kind).empty() || !controller_error(now, r, 1, kind).empty()) continue;  // HandleError + return
-        const std::vector<int> a = affected(r, 0, kind), b = affected(r, 1, kind);
-        for (int t : a)
-          if (std::find(b.begin(), b.end(), t) == b.end()) { cache[kind].remove(throttles[(size_t)t].nn(), now.nn()); reservation_changed((size_t)t); }
-        for (int t : b)
-          if (std::find(a.begin(), a.end(), t) == a.end()) { cache[kind].add(throttles[(size_t)t].nn(), now); reservation_changed((size_t)t); }
-      }
+      move_reservation(old, now, r.row(0), r.row(1));
     }
   }
-  void delete_pod(const std::string& ns, const std::string& pname) {
+  // The pod leaves the informer cache: returns whether the plugin held it, with its last copy in *old.
+  bool drop_pod(const std::string& ns, const std::string& pname, PodObj* old) {
     auto it = pod_index.find(ns + "/" + pname);
-    if (it == pod_index.end()) return;
+    if (it == pod_index.end()) return false;
     const int64_t row = it->second;
-    const PodObj old = pods[(size_t)row];
+    *old = pods[(size_t)row];
     // the row goes first (see apply_pod): a delete that repairs a refused snapshot must not be refused for it
-    totals_add(old, -1);
-    if (old.pend_row >= 0) queue_release(old.pend_row);
+    totals_add(*old, -1);
+    if (old->pend_row >= 0) queue_release(old->pend_row);
     pods[(size_t)row] = PodObj();  // tombstone row: flags == 0, no labels
     pods[(size_t)row].row = row;
     pod_index.erase(it);
-    ns_free_rows[old.ns].push_back(row);  // the slot stays with its namespace's arena
+    ns_free_rows[old->ns].push_back(row);  // the slot stays with its namespace's arena
     dirty_rows.insert(row);
-    // DeleteFunc (:509-515): a scheduled pod that disappears is un-reserved from its affected throttles
-    if (should_count_in(old) && !old.node_name.empty() && !throttles.empty()) {
+    return true;
+  }
+  // DeleteFunc (:509-515): a scheduled pod that disappears is un-reserved from its affected throttles
+  bool unreserves(const PodObj& old) const { return should_count_in(old) && !old.node_name.empty() && !throttles.empty(); }
+  void unreserve_deleted(const PodObj& old, const RowView& r) {
+    for (int kind = 0; kind < 2; ++kind) {
+      if (!controller_error(old, r, kind).empty()) continue;
+      for (int t : affected(r, kind))
+        if (cache[kind].remove(throttles[(size_t)t].nn(), old.nn())) reservation_changed((size_t)t);
+    }
+  }
+  // the pod is gone whatever happens to the pass: its reservations must not outlive it (reconcile only un-reserves pods that are
+  // still in the index) -- without the device's answer it leaves every throttle's reservation, a superset
+  void unreserve_everywhere(const PodObj& old) {
+    for (int kind = 0; kind < 2; ++kind)
+      if (cache[kind].remove_everywhere(old.nn())) { reserved_dirty = true; queue_void(); }
+  }
+  void delete_pod(const std::string& ns, const std::string& pname) {
+    PodObj old;
+    if (!drop_pod(ns, pname, &old)) return;
+    if (unreserves(old)) {
       PendingResult r;
       try {
         r = check_pending({old}, 0);
       } catch (...) {
-        // the pod is gone whatever happens to the pass: its reservations must not outlive it (reconcile only un-reserves pods
-        // that are still in the index) -- without the device's answer it leaves every throttle's reservation, a superset
-        for (int kind = 0; kind < 2; ++kind)
-          if (cache[kind].remove_everywhere(old.nn())) { reserved_dirty = true; queue_void(); }
+        unreserve_everywhere(old);
         throw;
       }
-      for (int kind = 0; kind < 2; ++kind) {
-        if (!controller_error(old, r, 0, kind).empty()) continue;
-        for (int t : affected(r, 0, kind))
-          if (cache[kind].remove(throttles[(size_t)t].nn(), old.nn())) reservation_changed((size_t)t);
-      }
+      unreserve_deleted(old, r.row(0));
     }
   }
+  void delete_namespace(const std::string& nm) {
+    const int id = ns_dict.find(nm);
+    if (id >= 0) { namespaces[(size_t)id].exists = false; namespaces[(size_t)id].labels.clear(); namespaces_dirty = true; }
+  }
+
+  // ---- informer events in batches (kth_apply_events) ----------------------------------------------------------------
+  // The reference's controllers reconcile what their informer handlers enqueue (throttle_controller.go:401-531,
+  // clusterthrottle_controller.go:433-563).  A batch of watch events is applied in order; the pod events between two table
+  // events (Throttle, ClusterThrottle, Namespace) form a run whose pod versions take ONE kt_match_pods call, after the events of
+  // the run are stored.  The tables cannot change inside a run, and no affected set depends on reservations, so the run's
+  // reservation edits -- the same ones apply_pod / delete_pod make -- are applied afterwards, in event order, with the same
+  // result as event by event.
+  struct PodEvent {
+    size_t ev = 0;
+    bool keys = false;         // the handler enqueues the affected throttles (shouldCountIn of a version it looks at)
+    bool move = false;         // UpdateFunc moves the reservation (moves_reservation)
+    bool unreserve = false;    // DeleteFunc un-reserves a counted, scheduled pod (unreserves)
+    std::vector<PodObj> ver;   // the versions the handler looks at: {new} AddFunc, {old, new} UpdateFunc, {old} DeleteFunc
+    std::vector<size_t> at;    // each version's row in the run's match result
+  };
+  struct EventOut {
+    std::string error, warning;
+    bool keys = false;                 // the entry carries "enqueue"
+    std::vector<std::string> enqueue;  // reconcile keys, creation order
+  };
+  // affectedThrottles of each version (one device call for the distinct (namespace, label set) pairs), as a PendingResult
+  PendingResult match_versions(const std::vector<PodObj>& vers) {
+    const bool tables_change = throttles_dirty || namespaces_dirty;
+    sync_all();
+    sync_status();
+    sync_reserved();
+    if (tables_change) queue.valid = false;
+    const int L = lim.label_slots;
+    const size_t k = vers.size();
+    std::vector<int64_t> lab((size_t)L * k, KT_LABEL_EMPTY);
+    std::vector<int32_t> nsid(k);
+    for (size_t i = 0; i < k; ++i) {  // the label slots pack_pod gives a pending row
+      int s = 0;
+      for (auto& kv : vers[i].labels) {
+        const int64_t code = labels.encode(kv.first, kv.second);
+        if (code != KT_LABEL_EMPTY) lab[(size_t)(s++) * k + i] = code;
+      }
+      nsid[i] = ns_id(vers[i].ns);
+    }
+    if (namespaces_dirty || throttles_dirty) {  // packing introduced new namespace ids
+      sync_all();
+      sync_status();
+      sync_reserved();
+      queue.valid = false;
+    }
+    PendingResult r;
+    r.Wp = kt_match_words(ctx);
+    r.bitmap.assign(k * (size_t)r.Wp, 0);
+    r.codes.assign(k * 2 * (size_t)r.Wp, 0);
+    check(kt_match_pods(ctx, (int64_t)k, lab.data(), nsid.data(), r.bitmap.data()), "kt_match_pods");
+    return r;
+  }
+  // The keys a pod event enqueues: per controller, the affected throttles of every version the handler looks at, or none when
+  // affectedThrottles fails for one of them (HandleError + return; the other controller has its own handler).
+  std::vector<std::string> enqueued(const PodEvent& pe, const PendingResult& r) {
+    std::vector<int> cols_hit;
+    for (int kind = 0; kind < 2; ++kind) {
+      std::vector<int> mine;
+      bool failed = false;
+      for (size_t j = 0; j < pe.ver.size() && !failed; ++j) {
+        const RowView row = r.row(pe.at[j]);
+        if (!controller_error(pe.ver[j], row, kind).empty()) failed = true;
+        else for (int t : affected(row, kind)) mine.push_back(t);
+      }
+      if (!failed) cols_hit.insert(cols_hit.end(), mine.begin(), mine.end());
+    }
+    std::sort(cols_hit.begin(), cols_hit.end());
+    cols_hit.erase(std::unique(cols_hit.begin(), cols_hit.end()), cols_hit.end());
+    creation_order(cols_hit);
+    std::vector<std::string> keys;
+    for (int t : cols_hit) keys.push_back(throttles[(size_t)t].nn());
+    return keys;
+  }
+  // One device call for a run of pod events, then their reservation edits in event order and their keys.  When the call fails,
+  // each event reports what kth_apply / kth_delete report when their pass fails (the move is skipped with a warning; a deleted
+  // pod leaves every reservation and the event is an error), and none carries keys.
+  void match_run(std::vector<PodEvent>& run, std::vector<EventOut>& out) {
+    if (run.empty()) return;
+    std::vector<PodObj> uniq;
+    std::map<std::pair<std::string, std::vector<std::pair<std::string, std::string>>>, size_t> seen;
+    for (auto& pe : run) {
+      pe.at.clear();
+      for (auto& v : pe.ver) {
+        auto labs = v.labels;
+        std::sort(labs.begin(), labs.end());
+        auto ins = seen.emplace(std::make_pair(v.ns, std::move(labs)), uniq.size());
+        if (ins.second) uniq.push_back(v);
+        pe.at.push_back(ins.first->second);
+      }
+    }
+    PendingResult r;
+    std::string err;
+    try {
+      r = match_versions(uniq);
+    } catch (const std::exception& e) {
+      err = e.what();
+    }
+    for (auto& pe : run) {
+      EventOut& o = out[pe.ev];
+      if (!err.empty()) {
+        o.keys = false;
+        if (pe.move) o.warning = "pod updated; reservation move skipped: " + err;
+        else if (pe.unreserve) { unreserve_everywhere(pe.ver[0]); o.error = err; }
+        else o.warning = "affected throttles not computed: " + err;
+        continue;
+      }
+      if (pe.move) move_reservation(pe.ver[0], pe.ver[1], r.row(pe.at[0]), r.row(pe.at[1]));
+      if (pe.unreserve) unreserve_deleted(pe.ver[0], r.row(pe.at[0]));
+      if (pe.keys) o.enqueue = enqueued(pe, r);
+    }
+    run.clear();
+  }
+  // One watch event: the state change kth_apply / kth_delete makes, with the pod pass left to the run.
+  void apply_event(const std::string& type, const std::string& kind, const Node& obj, size_t i, EventOut& o, std::vector<PodEvent>& run) {
+    const bool is_thr = kind == "Throttle" || kind == "ClusterThrottle";
+    const int tkind = kind == "Throttle" ? KT_KIND_THROTTLE : KT_KIND_CLUSTERTHROTTLE;
+    if (type == "DELETED") {
+      const std::string ns = obj["metadata"]["namespace"].str(), nm = obj["metadata"]["name"].str();
+      if (kind == "Pod") {
+        PodObj old;
+        if (drop_pod(ns, nm, &old) && should_count_in(old) && !throttles.empty()) {
+          PodEvent pe;
+          pe.ev = i;
+          pe.keys = true;
+          pe.unreserve = unreserves(old);
+          pe.ver = {old};
+          run.push_back(std::move(pe));
+        }
+      } else if (is_thr) {  // DeleteFunc: isResponsibleFor the object the plugin held
+        auto it = thr_index.find(std::string(tkind == KT_KIND_THROTTLE ? "T:" + ns : "C:") + "/" + nm);
+        if (it != thr_index.end() && throttles[(size_t)it->second].throttler_name == name) o.enqueue.push_back(throttles[(size_t)it->second].nn());
+        delete_throttle(tkind, ns, nm);
+      } else if (kind == "Namespace") {
+        delete_namespace(nm);
+      } else {
+        fail("unsupported kind: " + kind);
+      }
+    } else if (kind == "Pod") {
+      PodObj p = pod_from(obj);
+      const std::string nn = p.nn();
+      PodObj old;
+      const bool held = store_pod(std::move(p), &old);
+      const PodObj& cur = pods[(size_t)pod_index.at(nn)];
+      PodEvent pe;
+      pe.ev = i;
+      if (held) {  // UpdateFunc: the plugin's own store decides, as in kth_apply
+        pe.keys = should_count_in(old) || should_count_in(cur);
+        pe.move = moves_reservation(old, cur);
+        pe.ver = {old, cur};
+      } else {     // AddFunc
+        pe.keys = should_count_in(cur);
+        pe.ver = {cur};
+      }
+      if ((pe.keys && !throttles.empty()) || pe.move) run.push_back(std::move(pe));
+    } else if (kind == "Namespace") {
+      apply_namespace(obj);
+    } else if (is_thr) {  // AddFunc / UpdateFunc: isResponsibleFor the new object
+      apply_throttle(obj, tkind);
+      const std::string ns = tkind == KT_KIND_THROTTLE ? obj["metadata"]["namespace"].str() : "";
+      const ThrottleObj& t = throttles[(size_t)thr_index.at(std::string(tkind == KT_KIND_THROTTLE ? "T:" : "C:") + ns + "/" + obj["metadata"]["name"].str())];
+      if (t.throttler_name == name) o.enqueue.push_back(t.nn());
+    } else {
+      fail("unsupported kind: " + kind);
+    }
+    o.keys = true;
+  }
+  std::string apply_events(const std::string& events_json) {
+    ktjson::NodePtr evs = ktjson::parse(events_json.c_str());
+    if (!evs->is(Node::Arr)) fail("apply_events: events must be a JSON array of watch events");
+    if (!kt_match_pods) fail("kth_apply_events: the engine this plugin is linked against has no kt_match_pods");
+    const size_t n = evs->arr.size();
+    std::vector<EventOut> out(n);
+    std::vector<PodEvent> run;
+    for (size_t i = 0; i < n; ++i) {
+      const Node& e = *evs->arr[i];
+      EventOut& o = out[i];
+      const std::string at = "event " + std::to_string(i) + ": ";
+      if (!e.is(Node::Obj)) { o.error = at + "a watch event must be an object"; continue; }
+      const std::string type = e["type"].str();
+      if (type != "ADDED" && type != "MODIFIED" && type != "DELETED") { o.error = at + "unknown type \"" + type + "\""; continue; }
+      const Node& obj = e["object"];
+      if (!obj.is(Node::Obj)) { o.error = at + "missing object"; continue; }
+      const std::string kind = obj["kind"].str();
+      if (kind == "Throttle" || kind == "ClusterThrottle" || kind == "Namespace") match_run(run, out);  // the tables change here
+      const size_t n_cols = cols.size();
+      apply_committed = false;
+      apply_warning.clear();
+      try {
+        apply_event(type, kind, obj, i, o, run);
+      } catch (const std::exception& ex) {
+        if (type != "DELETED" && !apply_committed) rollback_columns(n_cols);  // as kth_apply: the refused object's resource names go with it
+        o.error = ex.what();
+        o.keys = false;
+        o.enqueue.clear();
+      }
+    }
+    match_run(run, out);
+    Writer w;
+    std::vector<std::string> all;
+    std::unordered_set<std::string> in_all;
+    w.begin_obj().key("results").begin_arr();
+    for (auto& o : out) {
+      w.begin_obj();
+      if (!o.error.empty()) {
+        w.key("error").str(o.error).end_obj();
+        continue;
+      }
+      w.key("ok").raw("true");
+      if (!o.warning.empty()) w.key("warning").str(o.warning);
+      if (o.keys) {
+        w.key("enqueue").begin_arr();
+        for (auto& k : o.enqueue) {
+          w.str(k);
+          if (in_all.insert(k).second) all.push_back(k);
+        }
+        w.end_arr();
+      }
+      w.end_obj();
+    }
+    w.end_arr().key("enqueue").begin_arr();
+    for (auto& k : all) w.str(k);
+    w.end_arr().end_obj();
+    return w.out;
+  }
+
   void apply_namespace(const Node& v) {
     const std::string nm = v["metadata"]["name"].str();
     const Node& lab = v["metadata"]["labels"];
@@ -2760,12 +3016,13 @@ const char* kth_delete(kth_plugin* p, const char* kind, const char* ns, const ch
     if (k == "Pod") p->delete_pod(n, nm);
     else if (k == "Throttle") p->delete_throttle(KT_KIND_THROTTLE, n, nm);
     else if (k == "ClusterThrottle") p->delete_throttle(KT_KIND_CLUSTERTHROTTLE, "", nm);
-    else if (k == "Namespace") {
-      const int id = p->ns_dict.find(nm);
-      if (id >= 0) { p->namespaces[(size_t)id].exists = false; p->namespaces[(size_t)id].labels.clear(); p->namespaces_dirty = true; }
-    } else fail("unsupported kind: " + k);
+    else if (k == "Namespace") p->delete_namespace(nm);
+    else fail("unsupported kind: " + k);
     return "{\"ok\":true}";
   });
+}
+const char* kth_apply_events(kth_plugin* p, const char* events_json) {
+  return guarded(p, [&]() { return p->apply_events(events_json ? events_json : ""); });
 }
 const char* kth_reconcile_all(kth_plugin* p, const char* now_rfc3339) {
   return guarded(p, [&]() { return p->reconcile_all(now_rfc3339 ? now_rfc3339 : ""); });

@@ -1,5 +1,6 @@
-// kt_keyed.cuh -- reconcile(key) for k listed throttles on the device (kt_reconcile_throttles), and PreFilter for k listed
-// pending rows (kt_check_pending_rows, at the end of this file).
+// kt_keyed.cuh -- reconcile(key) for k listed throttles on the device (kt_reconcile_throttles), PreFilter for k listed
+// pending rows (kt_check_pending_rows) and the affected throttles of k pods given by value (kt_match_pods), the last two at the
+// end of this file.
 //
 // The reference reconciles one key at a time (throttle_controller.go:84-211, clusterthrottle_controller.go:87-214): a key costs
 // the pods of the namespaces its throttle reaches (affectedPods, :221-246), not the whole snapshot.  Here the listed throttles'
@@ -310,6 +311,74 @@ __global__ void __launch_bounds__(kRowsTile) k_check_rows(const RowsArgs a) {
     if (c.x | c.y) ok = 0;
   }
   a.admit[i] = ok;
+}
+
+// ------------------------------------------------------------------------------------------------
+// affectedThrottles of k pods that live only in this call (kt_match_pods): the selector relation of pod versions an informer
+// event carries (throttle_controller.go:248-269, clusterthrottle_controller.go:272-298), with no resident row read or written.
+// One lane per listed pod, as in k_check_rows: its label slots become table row offsets in registers (translate8, the chunk
+// k_unpack_packed translates while it is in registers), its namespace's words come from the list k_translate_rows packs
+// (winfo_pack), and each word is evaluated with the pass's eval_word.  The CTA zeroes its [kRowsTile][Wp] block of the output
+// first, so the words outside the namespace's list read 0 as in the pass's rows; the lanes then store their non-zero words.
+// ------------------------------------------------------------------------------------------------
+struct MatchArgs {
+  TableView tb;
+  int L;
+  int64_t k;
+  const int64_t* labels;  // [L][k] label codes (keyId << 32 | valId, KT_LABEL_EMPTY)
+  const int32_t* ns;      // [k]
+  uint32_t* words;        // [k][Wp]
+};
+
+__host__ __device__ inline size_t match_smem_bytes(int L, bool reg_rows) { return reg_rows ? 0 : (size_t)((L + 7) & ~7) * kRowsTile * 4; }
+
+template <int TPC, int B, bool REG>
+__global__ void __launch_bounds__(kRowsTile) k_match_pods(const MatchArgs a) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  const int tid = threadIdx.x;
+  const int Wp = a.tb.Wp, Lpad = (a.L + 7) & ~7;
+  const int64_t row0 = (int64_t)blockIdx.x * kRowsTile;
+  {  // the block's output rows, coalesced (Wp is a multiple of 4)
+    const int64_t rows_here = a.k - row0 < kRowsTile ? a.k - row0 : kRowsTile;
+    uint4* d = reinterpret_cast<uint4*>(a.words + row0 * Wp);
+    const int64_t nvec = rows_here * (Wp / 4);
+    for (int64_t v = tid; v < nvec; v += kRowsTile) d[v] = make_uint4(0, 0, 0, 0);
+  }
+  __syncthreads();
+  const int64_t i = row0 + tid;
+  if (i >= a.k) return;  // (no barrier and no warp collective below: each lane works alone)
+  const int ns = __ldg(&a.ns[i]);
+  if ((unsigned)ns >= (unsigned)a.tb.NS) return;  // a namespace out of range affects nothing
+  PodRows<REG> rows;
+  rows.init(reinterpret_cast<int32_t*>(smem_raw), tid, kRowsTile);
+#pragma unroll 1
+  for (int s0 = 0; s0 < Lpad; s0 += 8) {
+    int64_t lab[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) lab[j] = s0 + j < a.L ? __ldg(&a.labels[(int64_t)(s0 + j) * a.k + i]) : KT_LABEL_EMPTY;
+    uint4 ke[8];
+    uint32_t o[8];
+    translate8_keys(a.tb, lab, ke);
+    translate8_rows(a.tb, lab, ke, o);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      if constexpr (REG) rows.off[j] = o[j];  // (REG: L <= 8, one chunk)
+      else rows.col[(s0 + j) * rows.stride] = o[j];
+    }
+  }
+  // the words that can apply to the namespace, as k_translate_rows packs them for a resident row
+  const int lo = __ldg(&a.tb.nsw_off[ns]);
+  const int cnt = __ldg(&a.tb.nsw_off[ns + 1]) - lo;
+  const uint32_t winfo = cnt == 0 ? 0u : winfo_pack(cnt, cnt > 0 ? __ldg(&a.tb.nsw_idx[lo]) : 0, cnt > 1 ? __ldg(&a.tb.nsw_idx[lo + 1]) : 0, a.tb.W);
+  WordCursor wc;
+  wc.init(a.tb, winfo, ns, true);
+  uint32_t* wrow = a.words + i * Wp;
+#pragma unroll 1
+  for (int q = 0; q < wc.cnt; ++q) {
+    const int w = wc.at(a.tb, q);
+    const uint32_t word = eval_word<TPC, B, REG>(a.tb, rows, Lpad, ns, w);
+    if (word) wrow[w] = word;
+  }
 }
 
 }  // namespace kt

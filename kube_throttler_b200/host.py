@@ -25,7 +25,7 @@ def _bind(L=None):
     L.kth_new_plugin_error.restype = cp
     L.kth_free.argtypes = [vp]
     L.kth_free.restype = None
-    for name, args in (("kth_apply", [vp, cp]), ("kth_delete", [vp, cp, cp, cp]), ("kth_reconcile_all", [vp, cp]), ("kth_reconcile", [vp, cp, cp]),
+    for name, args in (("kth_apply", [vp, cp]), ("kth_delete", [vp, cp, cp, cp]), ("kth_apply_events", [vp, cp]), ("kth_reconcile_all", [vp, cp]), ("kth_reconcile", [vp, cp, cp]),
                        ("kth_get_status", [vp, cp, cp]), ("kth_get_status_manifest", [vp, cp, cp]), ("kth_affected_pods", [vp, cp, cp]), ("kth_pre_filter", [vp, cp]), ("kth_pre_filter_batch", [vp, cp]),
                        ("kth_admit_queue", [vp, cp]), ("kth_pre_filter_key", [vp, cp, cp]), ("kth_pre_filter_keys", [vp, cp]), ("kth_reserve_key", [vp, cp, cp]), ("kth_unreserve_key", [vp, cp, cp]),
                        ("kth_queue_stats", [vp]), ("kth_reserve", [vp, cp]), ("kth_unreserve", [vp, cp]), ("kth_reserved", [vp, C.c_int, cp]), ("kth_metrics", [vp]), ("kth_eval", [cp])):
@@ -44,7 +44,7 @@ def _bind(L=None):
 
 
 HOST_EXPORTS = ["kth_new_plugin", "kth_new_plugin_error", "kth_free", "kth_apply", "kth_delete", "kth_reconcile_all", "kth_get_status", "kth_get_status_manifest",
-                "kth_pre_filter", "kth_pre_filter_key", "kth_reserve_key", "kth_unreserve_key", "kth_pre_filter_queue", "kth_queue_row", "kth_pod_row", "kth_queue_stats", "kth_last_error", "kth_pre_filter_batch", "kth_admit_queue", "kth_reserve", "kth_unreserve", "kth_reserved", "kth_metrics", "kth_eval", "kth_affected_pods", "kth_reconcile", "kth_pre_filter_keys"]
+                "kth_pre_filter", "kth_pre_filter_key", "kth_reserve_key", "kth_unreserve_key", "kth_pre_filter_queue", "kth_queue_row", "kth_pod_row", "kth_queue_stats", "kth_last_error", "kth_pre_filter_batch", "kth_admit_queue", "kth_reserve", "kth_unreserve", "kth_reserved", "kth_metrics", "kth_eval", "kth_affected_pods", "kth_reconcile", "kth_pre_filter_keys", "kth_apply_events"]
 
 
 def _result(raw):
@@ -91,6 +91,12 @@ class Plugin:
 
     def delete(self, kind, name, namespace=""):
         _result(self._L.kth_delete(self._h, kind.encode(), namespace.encode(), name.encode()))
+
+    def apply_events(self, events):
+        """A batch of watch events ({"type": "ADDED" | "MODIFIED" | "DELETED", "object": manifest}) applied in order:
+        {"results": [per event what apply / delete return, plus "enqueue": [keys]], "enqueue": [the union of the keys]}.
+        A refused or malformed event is an {"error": ...} entry (no exception for those); the rest of the batch applies."""
+        return _result(self._L.kth_apply_events(self._h, json.dumps(list(events)).encode()))
 
     # controllers
     def reconcile_all(self, now="2026-01-01T00:00:00Z"):
