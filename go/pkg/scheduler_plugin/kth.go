@@ -210,6 +210,36 @@ func (e *engine) preFilterKeys(keys []string) ([]preFilterKeysEntry, error) {
 	return r, err
 }
 
+// queueReportThrottle is one throttle's entry of kth_queue_report.
+type queueReportThrottle struct {
+	Key                         string          `json:"key"`
+	Kind                        string          `json:"kind"`
+	Active                      int64           `json:"active"`
+	Insufficient                int64           `json:"insufficient"`
+	PodRequestsExceedsThreshold int64           `json:"podRequestsExceedsThreshold"`
+	OnlyBlocker                 int64           `json:"onlyBlocker"`
+	HeldBack                    json.RawMessage `json:"heldBack"`
+}
+
+// queueReport is kth_queue_report: the verdict counts of the scheduling queue and, for every throttle of this plugin, the queued
+// pods it holds back by status, the ones it alone blocks and their ResourceAmount sum -- one device call, not one affectedPods
+// call per throttle.
+type queueReport struct {
+	Queued        int64                 `json:"queued"`
+	Success       int64                 `json:"success"`
+	Unschedulable int64                 `json:"unschedulable"`
+	Error         int64                 `json:"error"`
+	Throttles     []queueReportThrottle `json:"throttles"`
+}
+
+func (e *engine) queueReport() (*queueReport, error) {
+	var r queueReport
+	runtime.LockOSThread()
+	raw := C.GoString(C.kth_queue_report(e.h))
+	runtime.UnlockOSThread()
+	return &r, decode(raw, &r)
+}
+
 type reserveResult struct {
 	Code    string   `json:"code"`
 	Reasons []string `json:"reasons"`

@@ -349,6 +349,25 @@ int kt_get_match_rows(kt_ctx* ctx, int kind, int64_t k, const int64_t* rows, uin
  * one read of off[], one copy of the rows).  Multi-GPU: each rank answers for its own rows. */
 int kt_get_match_columns(kt_ctx* ctx, int kind, int64_t k, const int32_t* idx, int64_t* off /*[k+1]*/, int64_t* rows /*[cap]*/,
                          uint8_t* codes /*[cap] or NULL*/, int64_t cap);
+/* The scheduling queue summarised per throttle, from what the last pass that ran the check (a kt_evaluate without
+ * KT_EVAL_SKIP_CHECK, or kt_admit_queue) wrote for the pending rows [first, first + count), in caller rows: the codes are exactly
+ * those kt_get_check delivers for these rows.  row_class[i] (NULL: every row is class 1) applies to row first + i:
+ *   0  the row is skipped;
+ *   1  the row is counted;
+ *   2  the row is counted in status_cnt and held, never in sole_cnt (a pod whose PreFilter fails has no "only blocker").
+ * Every output pointer may be NULL.  Sums are exact in int64 under kt_evaluate's value domain; requests may be negative.
+ * Only rejected rows (admit byte 0) are read beyond their admit byte.  The call writes nothing another call reads (every getter
+ * answers as before it).  count = 0 is valid and yields zeros.  KT_ERR_INVALID for a range outside [0, n_pending) or count < 0;
+ * KT_ERR_STATE before a pass has written the pending codes of the current rows and throttle columns, and with a communicator
+ * (single GPU only). */
+typedef struct kt_check_summary {
+  int64_t* status_cnt;    /* [3][m] rows whose code for t is ACTIVE, INSUFFICIENT, POD_REQUESTS_EXCEEDS_THRESHOLD (in that order) */
+  int64_t* sole_cnt;      /* [m]    rows of class 1 whose ONLY non-zero code, over all throttles of both kinds, is t's */
+  int64_t* held;          /* [R][m] sum of req[r] over the rows with a non-zero code for t */
+  uint32_t* held_present; /* [m]    bit r: some such row has resource r present; KT_COUNT_BIT: at least one such row */
+} kt_check_summary;
+int kt_get_check_summary(kt_ctx* ctx, int64_t first, int64_t count, const uint8_t* row_class /*[count] or NULL*/,
+                         const kt_check_summary* out);
 /* reconcile(key) for k listed throttles (throttle_controller.go:84-211, clusterthrottle_controller.go:87-214), evaluated at
  * `now` on the running rows as they are now -- uploaded or delta-updated, whether or not a pass has run since.  For entry j:
  *   - out: what a KT_EVAL_FRESH_STATUS pass would report for column idx[j] (used, presence, pod count, throttled with

@@ -191,6 +191,22 @@ const char* kth_reserved(kth_plugin* p, int kind, const char* throttle_nn);
  * every other call answers as it would have; a device pass runs only when the state changed since the last one this call ran. */
 const char* kth_affected_pods(kth_plugin* p, const char* ns, const char* name);
 
+/* The scheduling queue per throttle -- which throttles hold the queue back, how many pods and how much they ask for -- in one
+ * call instead of one kth_affected_pods per throttle:
+ * {"queued":n,"success":n,"unschedulable":n,"error":n,
+ *  "throttles":[{"key":"ns/name" | "/name","kind":"Throttle" | "ClusterThrottle","active":n,"insufficient":n,
+ *                "podRequestsExceedsThreshold":n,"onlyBlocker":n,"heldBack":{...}},...]}
+ *   queued, success, unschedulable, error   the counts of kth_pre_filter_queue's verdicts 1-3 (queued is their sum)
+ *   throttles       every live throttle whose throttlerName is this plugin's, in creation order, keyed as kth_reconcile takes them
+ *   active, insufficient, podRequestsExceedsThreshold   the counts of kth_affected_pods(t).queued by status
+ *   heldBack        the ResourceAmountOfPod sum of the queued pods whose status there is not "not-throttled", spelled as
+ *                   kth_get_status's "used"; {} with no such pod
+ *   onlyBlocker     the queued pods whose kth_pre_filter_key is UnschedulableAndUnresolvable with one reason naming t alone
+ * No side effects: nothing is reserved, no status written, no gauge recorded (kth_queue_stats' passes and hits may change).  At
+ * most one device pass over the pending table -- none when the cached queue verdicts are current and the device still holds
+ * the codes of a pass at this state -- then one kt_get_check_summary. */
+const char* kth_queue_report(kth_plugin* p);
+
 /* The controllers' Prometheus gauges in text exposition format (throttle_metrics.go:27-131,
  * clusterthrottle_metrics.go:27-131, metrics_recorder.go:25-67): throttle_* families labelled {name,namespace,resource,uid},
  * clusterthrottle_* families labelled {name,resource,uid}; spec threshold / status.throttled / status.used /

@@ -44,7 +44,7 @@ EXPORTS = [
     "kt_create", "kt_destroy", "kt_last_error", "kt_version", "kt_set_stream", "kt_sync", "kt_enable_timing",
     "kt_enable_trace", "kt_get_trace", "kt_host_alloc", "kt_host_alloc_upload", "kt_host_free", "kt_upload_pods", "kt_upload_pods_compact", "kt_upload_pods_packed", "kt_set_async_uploads", "kt_update_pod_rows", "kt_upload_namespaces",
     "kt_upload_throttles", "kt_upload_status", "kt_set_reserved", "kt_evaluate", "kt_get_reconcile",
-    "kt_match_words", "kt_get_match_bitmap", "kt_get_match_rows", "kt_get_match_columns", "kt_reconcile_throttles", "kt_get_check", "kt_set_sparse_check", "kt_get_check_sparse", "kt_get_check_rows", "kt_check_pending_rows", "kt_match_pods", "kt_get_changed", "kt_get_reconcile_rows", "kt_step_submit", "kt_step_wait", "kt_admit_queue", "kt_get_timing", "kt_comm_unique_id",
+    "kt_match_words", "kt_get_match_bitmap", "kt_get_match_rows", "kt_get_match_columns", "kt_get_check_summary", "kt_reconcile_throttles", "kt_get_check", "kt_set_sparse_check", "kt_get_check_sparse", "kt_get_check_rows", "kt_check_pending_rows", "kt_match_pods", "kt_get_changed", "kt_get_reconcile_rows", "kt_step_submit", "kt_step_wait", "kt_admit_queue", "kt_get_timing", "kt_comm_unique_id",
     "kt_comm_init", "kt_comm_destroy", "kt_debug_compile_tables", "kt_debug_set_pass_plan", "kt_debug_get_pass_plan",
     "kt_debug_set_row_order", "kt_debug_get_row_order",
 ]
@@ -104,6 +104,7 @@ def lib():
         L.kt_get_match_columns.argtypes = [vp, C.c_int, C.c_int64, vp, vp, vp, vp, C.c_int64]
         L.kt_reconcile_throttles.argtypes = [vp, C.c_int64, C.c_int64, vp, C.POINTER(abi.ReconcileOut), vp, vp, C.c_int64]
         L.kt_get_check.argtypes = [vp, vp, vp]
+        L.kt_get_check_summary.argtypes = [vp, C.c_int64, C.c_int64, vp, C.POINTER(abi.CheckSummary)]
         L.kt_get_timing.argtypes = [vp, C.POINTER(abi.Timing)]
         L.kt_comm_unique_id.argtypes = [vp]
         L.kt_comm_init.argtypes = [vp, vp, C.c_int, C.c_int]
@@ -311,6 +312,19 @@ class Engine:
 
     def get_check(self, codes: Optional[np.ndarray], admit: Optional[np.ndarray]):
         self._ck(self._L.kt_get_check(self._h, abi.ptr(codes), abi.ptr(admit)))
+
+    def check_summary(self, first: int, count: int, row_class: Optional[np.ndarray] = None):
+        """The pending rows [first, first + count) of the last checking pass summarised per throttle: (status_cnt[3][m] by code
+        ACTIVE / INSUFFICIENT / POD_REQUESTS_EXCEEDS_THRESHOLD, sole_cnt[m], held[R][m], held_present[m]).  row_class[count]
+        (None: all 1) is 0 skip, 1 count, 2 count but never as the only blocker (kt_get_check_summary)."""
+        m, R, z = self.m, self.R, np.zeros
+        status_cnt, sole_cnt, held, held_present = z((3, m), np.int64), z(m, np.int64), z((R, m), np.int64), z(m, np.uint32)
+        cls = None if row_class is None else np.ascontiguousarray(row_class, np.uint8)
+        if cls is not None and cls.shape[0] != count:
+            raise ValueError(f"row_class has {cls.shape[0]} entries, count is {count}")
+        out = abi.CheckSummary(abi.ptr(status_cnt), abi.ptr(sole_cnt), abi.ptr(held), abi.ptr(held_present))
+        self._ck(self._L.kt_get_check_summary(self._h, first, count, abi.ptr(cls), C.byref(out)))
+        return status_cnt, sole_cnt, held, held_present
 
     def set_sparse_check(self, cap_entries: int):
         """Later passes also append every non-zero code word to a device list (0: off)."""

@@ -67,6 +67,10 @@ class ReconcileOut(C.Structure):
                 ("calc_cnt", C.c_void_p), ("override_active", C.c_void_p)]
 
 
+class CheckSummary(C.Structure):  # kt_check_summary
+    _fields_ = [("status_cnt", C.c_void_p), ("sole_cnt", C.c_void_p), ("held", C.c_void_p), ("held_present", C.c_void_p)]
+
+
 class StepResult(C.Structure):  # kt_step_result
     _fields_ = [("n_pending", C.c_int64), ("n_sparse", C.c_int64), ("admit", C.c_void_p), ("entries", C.c_void_p), ("status", ReconcileOut)]
 

@@ -190,6 +190,8 @@ struct kt_ctx {
   int64_t step_first = 0;
   bool step_pending = false;
   DevBuf d_codes, d_admit;
+  bool have_codes = false;      // a checking pass wrote d_codes / d_admit for the current pending rows and throttle columns
+  DevBuf d_sum;                 // kt_get_check_summary (kt_keyed.cuh): {row classes | per-throttle outputs} of one call
   DevBuf d_sparse;              // kt_set_sparse_check: {count u32, pad to 16 B, entries [cap][3] u32}
   uint32_t sparse_cap = 0;      // 0: off
   uint32_t sparse_guess = 1024; // entries fetched together with the count (adapts to the last pass)
@@ -833,6 +835,7 @@ int kt_upload_pods(kt_ctx* c, int kind, int64_t n, const int64_t* labels, const 
   s.n = n;
   s.roff_valid = s.bitmap_clean = false;
   c->evaluated = false;
+  if (kind == KT_PODS_PENDING) c->have_codes = false;
   if (!c->async_uploads) KT_CUDA(c, cudaStreamSynchronize(c->stream));  // the caller may reuse its buffers as soon as we return
   return KT_OK;
 }
@@ -872,6 +875,7 @@ int kt_upload_pods_compact(kt_ctx* c, int kind, int64_t n, int32_t val_bits, con
   s.n = n;
   s.roff_valid = s.bitmap_clean = false;
   c->evaluated = false;
+  if (kind == KT_PODS_PENDING) c->have_codes = false;
   if (!c->async_uploads) KT_CUDA(c, cudaStreamSynchronize(c->stream));  // the caller may reuse its buffers as soon as we return
   return KT_OK;
 }
@@ -1000,6 +1004,7 @@ static int upload_pods_packed_locked(kt_ctx* c, int kind, int64_t n, const kt_pa
     s.roff_valid = s.bitmap_clean = false;
   }
   c->evaluated = false;
+  if (kind == KT_PODS_PENDING) c->have_codes = false;
   if (!c->async_uploads) KT_CUDA(c, cudaStreamSynchronize(c->stream));  // the caller may reuse its buffers as soon as we return
   return KT_OK;
 }
@@ -1101,6 +1106,7 @@ int kt_upload_throttles(kt_ctx* c, int32_t m, const kt_throttle_cols* cols, cons
   c->have_status = false;
   c->have_reserved = false;
   c->evaluated = false;
+  c->have_codes = false;
   return recompile_tables(c);
 }
 
@@ -1163,14 +1169,19 @@ static int evaluate_locked(kt_ctx* c, int64_t now, uint32_t flags) {
   PodStore& run = c->pods[KT_PODS_RUNNING];
   PodStore& pend = c->pods[KT_PODS_PENDING];
   {
-    const void* b0 = run.bitmap.p; const void* b1 = pend.bitmap.p; const void* b2 = c->d_codes.p;
+    // A buffer allocated here holds whatever the allocator hands back; a pass that does not write it (a check-only pass leaves
+    // the running bitmap alone, a reconcile-only pass the codes) must not let the getters deliver that: zeroed once on allocation.
+    const void* b0 = run.bitmap.p; const void* b1 = pend.bitmap.p; const void* b2 = c->d_codes.p; const void* b3 = c->d_admit.p;
     KT_CUDA(c, run.bitmap.reserve((size_t)run.n * Wp * 4 + 16));
     KT_CUDA(c, pend.bitmap.reserve((size_t)pend.n * Wp * 4 + 16));
     KT_CUDA(c, c->d_codes.reserve((size_t)pend.n * 2 * Wp * 4 + 16));
+    KT_CUDA(c, c->d_admit.reserve((size_t)pend.n + 16));
     if (run.bitmap.p != b0) run.bitmap_clean = false;
     if (pend.bitmap.p != b1 || c->d_codes.p != b2) pend.bitmap_clean = false;
+    const std::pair<DevBuf*, const void*> grown[] = {{&run.bitmap, b0}, {&pend.bitmap, b1}, {&c->d_codes, b2}, {&c->d_admit, b3}};
+    for (const auto& g : grown)
+      if (g.first->p != g.second) KT_CUDA(c, cudaMemsetAsync(g.first->p, 0, g.first->cap, c->stream));
   }
-  KT_CUDA(c, c->d_admit.reserve((size_t)pend.n + 16));
   if (do_rec && (rc = ensure_roff(c, run))) return rc;   // no-ops unless rows or tables changed since the last pass
   if (do_chk && (rc = ensure_roff(c, pend))) return rc;
   const TableView tb = table_view(c);
@@ -1264,6 +1275,7 @@ static int evaluate_locked(kt_ctx* c, int64_t now, uint32_t flags) {
     c->last = kt_timing{};
     c->last.launches = 1;
     c->evaluated = true;
+    c->have_codes = true;
     return KT_OK;
   }
 
@@ -1311,6 +1323,7 @@ static int evaluate_locked(kt_ctx* c, int64_t now, uint32_t flags) {
   c->last = kt_timing{};
   c->last.launches = launches;
   c->evaluated = true;
+  if (do_chk) c->have_codes = true;
   return KT_OK;
 }
 
@@ -1888,6 +1901,55 @@ int kt_get_check(kt_ctx* c, uint32_t* codes, uint8_t* admit) {
     KT_CUDA(c, cudaMemcpyAsync(admit, src, (size_t)P, cudaMemcpyDeviceToHost, c->stream));
   }
   KT_CUDA(c, cudaStreamSynchronize(c->stream));
+  return KT_OK;
+}
+
+// ---- the scheduling queue summarised per throttle (kt_keyed.cuh) ------------------------------------------------------
+int kt_get_check_summary(kt_ctx* c, int64_t first, int64_t count, const uint8_t* row_class, const kt_check_summary* o) {
+  if (!c || !o) return KT_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(c->mu);
+  PodStore& pend = c->pods[KT_PODS_PENDING];
+  if (first < 0 || count < 0 || first > pend.n - count)
+    return fail(c, KT_ERR_INVALID, "rows [%lld, %lld + %lld) outside the pending table (%lld rows)", (long long)first, (long long)first, (long long)count, (long long)pend.n);
+  if (c->comm) return fail(c, KT_ERR_STATE, "kt_get_check_summary is single-GPU: this context has a communicator");
+  if (!c->evaluated || !c->have_codes) return fail(c, KT_ERR_STATE, "kt_get_check_summary before a pass wrote the pending codes");
+  int rc = set_device(c);
+  if (rc) return rc;
+  if ((rc = check_pass_error(c))) return rc;
+  const int M = c->M, R = c->lim.n_resources;
+  // one block: row classes [count] (padded to 16 B) | status_cnt [3][M] | sole_cnt [M] | held [R][M] | held_present [M]
+  const size_t cls_bytes = row_class ? ((size_t)count + 15) & ~(size_t)15 : 0;
+  const size_t u64s = (size_t)(4 + R) * M, out_bytes = u64s * 8 + (size_t)M * 4;
+  std::vector<unsigned char> hb(out_bytes + 1);
+  if (count > 0 && M > 0) {
+    KT_CUDA(c, c->d_sum.reserve(cls_bytes + out_bytes + 16));
+    unsigned char* base = c->d_sum.as<unsigned char>();
+    unsigned char* ob = base + cls_bytes;
+    if (row_class) KT_CUDA(c, cudaMemcpyAsync(base, row_class, (size_t)count, cudaMemcpyHostToDevice, c->stream));
+    KT_CUDA(c, cudaMemsetAsync(ob, 0, out_bytes, c->stream));
+    SummaryArgs a{};
+    a.first = first; a.count = count; a.n = pend.n; a.Wc = 2 * c->ht.Wp; a.R = R; a.M = M;
+    a.codes = c->d_codes.as<uint32_t>(); a.admit = c->d_admit.as<unsigned char>();
+    a.req = pend.req.as<int64_t>(); a.present = pend.present.as<uint32_t>();
+    a.caller_of = pend.clustered ? pend.o_caller.as<uint32_t>() : nullptr;
+    a.row_class = row_class ? base : nullptr;
+    unsigned long long* u = reinterpret_cast<unsigned long long*>(ob);
+    a.status_cnt = o->status_cnt ? u : nullptr;
+    a.sole_cnt = o->sole_cnt ? u + (size_t)3 * M : nullptr;
+    a.held = o->held ? u + (size_t)4 * M : nullptr;
+    a.held_present = o->held_present ? reinterpret_cast<uint32_t*>(u + u64s) : nullptr;
+    const int64_t rows = pend.clustered ? pend.n : count;
+    const int64_t blocks = std::min<int64_t>((rows + kSummaryThreads - 1) / kSummaryThreads, (int64_t)c->sm_count * 8);
+    k_check_summary<<<(unsigned)std::max<int64_t>(blocks, 1), kSummaryThreads, 0, c->stream>>>(a);
+    KT_CUDA(c, cudaGetLastError());
+    KT_CUDA(c, cudaMemcpyAsync(hb.data(), ob, out_bytes, cudaMemcpyDeviceToHost, c->stream));
+    KT_CUDA(c, cudaStreamSynchronize(c->stream));
+  }
+  const unsigned char* h = hb.data();
+  if (o->status_cnt) std::memcpy(o->status_cnt, h, (size_t)3 * M * 8);
+  if (o->sole_cnt) std::memcpy(o->sole_cnt, h + (size_t)3 * M * 8, (size_t)M * 8);
+  if (o->held) std::memcpy(o->held, h + (size_t)4 * M * 8, (size_t)R * M * 8);
+  if (o->held_present) std::memcpy(o->held_present, h + u64s * 8, (size_t)M * 4);
   return KT_OK;
 }
 

@@ -27,11 +27,13 @@
 
 // The host layer is also linked, for CPU tests, against engine test doubles (tests/host_stub) that implement only the calls
 // the rest of this file makes: weak references let such a build load, and kth_affected_pods / kth_reconcile / kth_pre_filter_keys
-// / kth_apply_events fail in it.  The product library defines these calls in kt_engine.cu, so the references are always bound there.
+// / kth_apply_events / kth_queue_report fail in it.  The product library defines these calls in kt_engine.cu, so the references
+// are always bound there.
 #pragma weak kt_get_match_columns
 #pragma weak kt_reconcile_throttles
 #pragma weak kt_check_pending_rows
 #pragma weak kt_match_pods
+#pragma weak kt_get_check_summary
 
 namespace {
 
@@ -1562,7 +1564,7 @@ struct kth_plugin {
     if (found.throttler_name != name) fail(found.nn() + " belongs to throttler \"" + found.throttler_name + "\", not to \"" + name + "\"");
     if (columns_epoch != epoch) {
       run_pending_pass({}, 0, 0);
-      columns_epoch = epoch;
+      columns_epoch = codes_epoch = epoch;
     }
     const size_t t = (size_t)thr_index.at(key);  // (the pass may have laid the columns out anew)
     std::vector<int64_t> run_rows, pend_rows;
@@ -1603,6 +1605,63 @@ struct kth_plugin {
     for (const PodObj* p : finished) w.str(p->nn());
     w.end_arr().key("queued").begin_arr();
     for (auto& q : queued) w.begin_obj().key("pod").str(q.first->nn()).key("status").str(kStatus[q.second & 3u]).end_obj();
+    w.end_arr().end_obj();
+    return w.out;
+  }
+
+  // ---- the scheduling queue per throttle (kth_queue_report) ----------------------------------------------------------
+  // The verdicts are kth_pre_filter_queue's: the cached ones when they are current, else those of the one pass that refreshes
+  // them.  The per-throttle numbers come from one kt_get_check_summary over the device codes, which must be those of a pass at
+  // this state: the refresh just run, or the last pass of kth_affected_pods or of this call at the same `epoch` (the cached
+  // verdicts being current says nothing about what the device holds: other calls run passes of their own); else one runs here.
+  uint64_t codes_epoch = 0;
+  std::string queue_report() {
+    if (!kt_get_check_summary) fail("kth_queue_report: the engine this plugin is linked against has no kt_get_check_summary");
+    const int64_t n = (int64_t)pend_pod.size();
+    std::vector<uint8_t> verdicts((size_t)n);
+    const uint64_t passes = queue.passes;
+    pre_filter_queue(verdicts.data(), n);
+    if (queue.passes != passes) codes_epoch = epoch;
+    if (codes_epoch != epoch) {
+      run_pending_pass({}, 0);
+      codes_epoch = epoch;
+    }
+    int64_t count[4] = {0, 0, 0, 0};
+    for (uint8_t v : verdicts) ++count[v & 3u];
+    std::vector<size_t> ours;  // (the pass may have laid the columns out anew)
+    for (size_t t = 0; t < throttles.size(); ++t)
+      if (throttles[t].live && throttles[t].throttler_name == name) ours.push_back(t);
+    creation_order(ours);
+    const size_t m = throttles.size(), R = (size_t)lim.n_resources;
+    std::vector<int64_t> status_cnt(3 * m), sole_cnt(m), held(R * m);
+    std::vector<uint32_t> held_present(m);
+    if (!ours.empty()) {
+      // class 0: free queue rows (tombstones, which a selector without requirements still matches); 2: PreFilter is Error
+      std::vector<uint8_t> cls((size_t)pend_capacity, 0);
+      for (int64_t r = 0; r < n; ++r) cls[(size_t)r] = verdicts[(size_t)r] == 3 ? 2 : verdicts[(size_t)r] != 0 ? 1 : 0;
+      const kt_check_summary out{status_cnt.data(), sole_cnt.data(), held.data(), held_present.data()};
+      check(kt_get_check_summary(ctx, 0, pend_capacity, cls.data(), &out), "kt_get_check_summary");
+    }
+    Writer w;
+    w.begin_obj().key("queued").num((long long)(count[1] + count[2] + count[3])).key("success").num((long long)count[1]);
+    w.key("unschedulable").num((long long)count[2]).key("error").num((long long)count[3]).key("throttles").begin_arr();
+    for (size_t t : ours) {
+      const ThrottleObj& o = throttles[t];
+      w.begin_obj().key("key").str(o.nn()).key("kind").str(o.kind == KT_KIND_THROTTLE ? "Throttle" : "ClusterThrottle");
+      w.key("active").num((long long)status_cnt[t]).key("insufficient").num((long long)status_cnt[m + t]);
+      w.key("podRequestsExceedsThreshold").num((long long)status_cnt[2 * m + t]).key("onlyBlocker").num((long long)sole_cnt[t]);
+      ResAmount a;  // ResourceAmount{} .Add(ResourceAmountOfPod(p)) over the held-back pods, as reconcile sums status.used
+      if (held_present[t] & KT_COUNT_BIT) {
+        a.has_counts = true;
+        a.pod = (long long)(status_cnt[t] + status_cnt[m + t] + status_cnt[2 * m + t]);
+        a.requests_nil = false;
+        for (size_t r = 0; r < cols.size() && r < R; ++r)
+          if ((held_present[t] >> r) & 1) a.requests[(int)r] = from_scale((int)r, held[r * m + t]);
+      }
+      w.key("heldBack");
+      amount_json(w, a);
+      w.end_obj();
+    }
     w.end_arr().end_obj();
     return w.out;
   }
@@ -3152,6 +3211,9 @@ const char* kth_reserved(kth_plugin* p, int kind, const char* throttle_nn) {
 }
 const char* kth_affected_pods(kth_plugin* p, const char* ns, const char* name) {
   return guarded<true>(p, [&]() { return p->affected_pods(ns ? ns : "", name ? name : ""); });
+}
+const char* kth_queue_report(kth_plugin* p) {
+  return guarded<true>(p, [&]() { return p->queue_report(); });
 }
 const char* kth_metrics(kth_plugin* p) {
   return guarded(p, [&]() -> std::string {

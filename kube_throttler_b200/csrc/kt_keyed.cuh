@@ -1,6 +1,6 @@
 // kt_keyed.cuh -- reconcile(key) for k listed throttles on the device (kt_reconcile_throttles), PreFilter for k listed
-// pending rows (kt_check_pending_rows) and the affected throttles of k pods given by value (kt_match_pods), the last two at the
-// end of this file.
+// pending rows (kt_check_pending_rows), the affected throttles of k pods given by value (kt_match_pods) and the scheduling queue
+// summarised per throttle (kt_get_check_summary), the last three at the end of this file.
 //
 // The reference reconciles one key at a time (throttle_controller.go:84-211, clusterthrottle_controller.go:87-214): a key costs
 // the pods of the namespaces its throttle reaches (affectedPods, :221-246), not the whole snapshot.  Here the listed throttles'
@@ -378,6 +378,92 @@ __global__ void __launch_bounds__(kRowsTile) k_match_pods(const MatchArgs a) {
     const int w = wc.at(a.tb, q);
     const uint32_t word = eval_word<TPC, B, REG>(a.tb, rows, Lpad, ns, w);
     if (word) wrow[w] = word;
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
+// The scheduling queue summarised per throttle (kt_get_check_summary): what the last checking pass left in the dense codes,
+// reduced over the rejected rows for every throttle at once.
+// A warp takes 32 consecutive DEVICE rows (the per-throttle results do not depend on row order, so the rows stay where the layout
+// put them; only the caller's row classes are read through the row map).  A row that is admitted, outside the range or of class 0
+// costs its admit byte.  A rejected row reads its code words twice: once to count its non-zero codes (one alone makes its throttle
+// the only blocker), once in warp lockstep to credit them.  A code's word and position name the throttle, so the lanes holding a
+// non-zero code at the same place form the warp's group for that throttle: ballots give the counts per status, warp sums the
+// requests, and one lane adds each into HBM -- one atomic per warp and throttle however many rows the throttle rejects.
+// ------------------------------------------------------------------------------------------------
+constexpr int kSummaryThreads = 256;
+
+struct SummaryArgs {
+  int64_t first, count;            // caller rows [first, first + count)
+  int64_t n;                       // pending rows
+  int Wc, R, M;                    // code words per row (2 Wp), resources, throttles
+  const uint32_t* codes;           // [n][Wc] by device row
+  const unsigned char* admit;      // [n]
+  const int64_t* req;              // [R][n]
+  const uint32_t* present;         // [n]
+  const uint32_t* caller_of;       // device row -> caller row, or null (rows stored as given)
+  const unsigned char* row_class;  // [count] by caller row - first, or null (every row class 1)
+  unsigned long long* status_cnt;  // [3][M]
+  unsigned long long* sole_cnt;    // [M]
+  unsigned long long* held;        // [R][M]
+  uint32_t* held_present;          // [M]
+};
+
+__global__ void __launch_bounds__(kSummaryThreads) k_check_summary(const SummaryArgs a) {
+  const int lane = threadIdx.x & 31;
+  // the device rows the range occupies: itself when rows are stored as given, anywhere when they are laid out by namespace
+  const int64_t lo = a.caller_of ? 0 : a.first, rows = a.caller_of ? a.n : a.count;
+  const int64_t stride = (int64_t)gridDim.x * kSummaryThreads;
+#pragma unroll 1
+  for (int64_t base = (int64_t)blockIdx.x * kSummaryThreads + (threadIdx.x & ~31); base < rows; base += stride) {
+    const int64_t d = lo + base + lane;
+    int cls = 0;
+    if (base + lane < rows && !__ldg(&a.admit[d])) {
+      const int64_t c = a.caller_of ? (int64_t)__ldg(&a.caller_of[d]) : d;
+      if (c >= a.first && c < a.first + a.count) cls = a.row_class ? __ldg(&a.row_class[c - a.first]) : 1;
+    }
+    if (!__any_sync(kFull, cls != 0)) continue;
+    const uint32_t* crow = a.codes + (cls ? d : 0) * a.Wc;
+    int nz = 0;
+    if (cls)
+      for (int j = 0; j < a.Wc; ++j) {
+        const uint32_t w = __ldg(&crow[j]);
+        nz += __popc((w | w >> 1) & 0x55555555u);
+      }
+    const bool sole = cls == 1 && nz == 1;
+    const uint32_t present = cls ? __ldg(&a.present[d]) & ~KT_COUNT_BIT : 0u;
+#pragma unroll 1
+    for (int j = 0; j < a.Wc; ++j) {
+      const uint32_t w = cls ? __ldg(&crow[j]) : 0u;
+      uint32_t u = __reduce_or_sync(kFull, (w | w >> 1) & 0x55555555u);  // the even bit of each position some lane has non-zero
+#pragma unroll 1
+      while (u) {
+        const int q = __ffs(u) - 1;
+        u &= u - 1;
+        const int t = j * 16 + (q >> 1);
+        if (t >= a.M) break;  // (warp-uniform; no code names a column beyond the throttles)
+        const uint32_t code = (w >> q) & 3u;
+        const uint32_t b1 = __ballot_sync(kFull, code == KT_CHECK_ACTIVE), b2 = __ballot_sync(kFull, code == KT_CHECK_INSUFFICIENT);
+        const uint32_t b3 = __ballot_sync(kFull, code == KT_CHECK_POD_REQUESTS_EXCEEDS_THRESHOLD);
+        const uint32_t bs = __ballot_sync(kFull, code != 0u && sole);
+        const uint32_t pr = __reduce_or_sync(kFull, code ? present : 0u);
+        if (lane == 0) {
+          if (a.status_cnt) {
+            if (b1) atomicAdd(&a.status_cnt[t], (unsigned long long)__popc(b1));
+            if (b2) atomicAdd(&a.status_cnt[(size_t)a.M + t], (unsigned long long)__popc(b2));
+            if (b3) atomicAdd(&a.status_cnt[(size_t)2 * a.M + t], (unsigned long long)__popc(b3));
+          }
+          if (a.sole_cnt && bs) atomicAdd(&a.sole_cnt[t], (unsigned long long)__popc(bs));
+          if (a.held_present) atomicOr(&a.held_present[t], pr | KT_COUNT_BIT);
+        }
+        if (a.held)
+          for (int r = 0; r < a.R; ++r) {
+            const long long v = (code && ((present >> r) & 1u)) ? __ldg(&a.req[(int64_t)r * a.n + d]) : 0;
+            const unsigned long long s = warp_sum_u64((unsigned long long)v);  // two's complement: exact modulo 2^64
+            if (lane == (r & 31) && s) atomicAdd(&a.held[(size_t)r * a.M + t], s);
+          }
+      }
+    }
   }
 }
 
