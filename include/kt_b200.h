@@ -187,7 +187,9 @@ int kt_create(kt_ctx** out, int device, const kt_limits* limits);
 void kt_destroy(kt_ctx* ctx);
 const char* kt_last_error(const kt_ctx* ctx); /* valid until the next call on ctx */
 const char* kt_version(void);
-/* Run on a caller-owned CUDA stream (cudaStream_t as void*); NULL restores the private stream. */
+/* Run on a caller-owned CUDA stream (cudaStream_t as void*); NULL restores the private stream.  A switch keeps queued work
+ * ordered: everything queued on the old stream before the switch (async uploads, passes) runs before anything the context
+ * queues on the new one, and kt_sync, which waits on the new stream, also covers the work queued before the switch. */
 int kt_set_stream(kt_ctx* ctx, void* cuda_stream);
 int kt_sync(kt_ctx* ctx);
 /* Record CUDA events around each kernel of kt_evaluate so kt_get_timing reports device times. */
@@ -202,7 +204,8 @@ int kt_enable_timing(kt_ctx* ctx, int on);
  * Diagnostic only; off by default. */
 int kt_enable_trace(kt_ctx* ctx, int on);
 int64_t kt_get_trace(kt_ctx* ctx, uint64_t* rows /*[cap][32]*/, int64_t cap, uint32_t roles[4]);
-/* Pinned host memory for zero-staging H2D/D2H (cudaHostAlloc / cudaFreeHost). */
+/* Pinned host memory for zero-staging H2D/D2H (cudaHostAlloc / cudaFreeHost).  The columns of a packed upload carved out of
+ * ONE such block cross the host link as one transfer. */
 void* kt_host_alloc(size_t bytes);
 /* The same, write-combined (cudaHostAllocWriteCombined): for buffers the CPU only ever WRITES, front to back, and the device
  * reads (upload columns).  The device's reads need no cache snooping on the host, which some platforms reward with a faster

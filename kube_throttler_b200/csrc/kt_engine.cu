@@ -10,6 +10,7 @@
 #include <cstdint>
 #include <cstdio>
 #include <cstring>
+#include <map>
 #include <mutex>
 #include <string>
 #include <type_traits>
@@ -183,6 +184,7 @@ struct kt_ctx {
   size_t h_out_cap = 0, out_bytes = 0;
   size_t o_off[8] = {};
   bool async_uploads = false;  // kt_set_async_uploads
+  cudaEvent_t ev_switch = nullptr;  // kt_set_stream: the new stream waits for what was queued on the old one
   // kt_step_submit / kt_step_wait: one pinned result block, one event
   void* h_step = nullptr;
   size_t h_step_cap = 0, step_off[3] = {};
@@ -549,6 +551,10 @@ int ensure_window(kt_ctx* c, size_t part_bytes) {
 // Every kernel goes through cudaLaunchKernelEx so that the dependent ones can carry the programmatic
 // stream serialization attribute (PDL): the secondary grid may start while the primary still runs and
 // synchronises on it with griddepcontrol.wait where it first needs the primary's results.
+// The rule: a kernel launched with PDL either waits at its top (k_pass), or its primary -- the kernel right
+// before it in the stream -- was launched by the same call.  Its primary is otherwise whatever the caller
+// queued last (another pass of this context, another context's pass on a shared stream), and the writes it
+// makes before its wait would race with that work.
 template <class... KArgs, class... Args>
 cudaError_t launch(kt_ctx* c, void (*kern)(KArgs...), unsigned blocks, unsigned threads, size_t smem, bool pdl, Args... args) {
   cudaError_t e = cudaFuncSetAttribute((const void*)kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
@@ -682,6 +688,26 @@ cudaError_t dispatch_check(kt_ctx* c, const PodView& pv, const TableView& tb, co
   return with_variant(c, true, [&](auto tpc, auto b, auto, auto reg) { return launch_check<tpc, b, reg>(c, pv, tb, px, blocks, pdl); });
 }
 
+// The pinned blocks kt_host_alloc / kt_host_alloc_upload handed out (start -> bytes).  Separate allocations may lie side by
+// side in the address space, and the runtime refuses a copy that spans two of them: a packed upload sends its columns as one
+// transfer only when they lie inside ONE of these blocks.
+std::mutex g_host_mu;
+std::map<uintptr_t, size_t> g_host_blocks;
+void* host_alloc(size_t bytes, unsigned flags) {
+  void* p = nullptr;
+  if (cudaHostAlloc(&p, bytes ? bytes : 1, flags) != cudaSuccess) return nullptr;
+  std::lock_guard<std::mutex> lk(g_host_mu);
+  g_host_blocks[(uintptr_t)p] = bytes ? bytes : 1;
+  return p;
+}
+bool in_one_host_block(uintptr_t lo, uintptr_t hi) {
+  std::lock_guard<std::mutex> lk(g_host_mu);
+  auto it = g_host_blocks.upper_bound(lo);
+  if (it == g_host_blocks.begin()) return false;
+  --it;
+  return hi <= it->first + it->second;
+}
+
 }  // namespace
 
 extern "C" {
@@ -711,6 +737,7 @@ int kt_create(kt_ctx** out, int device, const kt_limits* lim) {
   if (cudaDeviceGetAttribute(&c->sm_count, cudaDevAttrMultiProcessorCount, device) != cudaSuccess || c->sm_count <= 0) { delete c; return KT_ERR_CUDA; }
   for (auto& e : c->ev)
     if (cudaEventCreate(&e) != cudaSuccess) { delete c; return KT_ERR_CUDA; }
+  if (cudaEventCreateWithFlags(&c->ev_switch, cudaEventDisableTiming) != cudaSuccess) { kt_destroy(c); return KT_ERR_CUDA; }
   if (c->d_sync.reserve(sizeof(PassSync)) != cudaSuccess || cudaMemset(c->d_sync.p, 0, sizeof(PassSync)) != cudaSuccess) { kt_destroy(c); return KT_ERR_CUDA; }
   *out = c;
   return KT_OK;
@@ -734,6 +761,7 @@ void kt_destroy(kt_ctx* c) {
   if (c->h_out) cudaFreeHost(c->h_out);
   if (c->h_step) cudaFreeHost(c->h_step);
   if (c->ev_step) cudaEventDestroy(c->ev_step);
+  if (c->ev_switch) cudaEventDestroy(c->ev_switch);
   if (c->h_sparse_count) cudaFreeHost(c->h_sparse_count);
   c->d_sparse.release();
   for (DevBuf* b : all) b->release();
@@ -746,7 +774,15 @@ void kt_destroy(kt_ctx* c) {
 int kt_set_stream(kt_ctx* c, void* cuda_stream) {
   if (!c) return KT_ERR_INVALID;
   std::lock_guard<std::mutex> lk(c->mu);
-  c->stream = cuda_stream ? (cudaStream_t)cuda_stream : c->own_stream;
+  const cudaStream_t next = cuda_stream ? (cudaStream_t)cuda_stream : c->own_stream;
+  if (next == c->stream) return KT_OK;
+  int rc = set_device(c);
+  if (rc) return rc;
+  // work queued on the old stream (async uploads, passes) stays ahead of everything queued on the new one, and a kt_sync on
+  // the new stream covers it
+  KT_CUDA(c, cudaEventRecord(c->ev_switch, c->stream));
+  KT_CUDA(c, cudaStreamWaitEvent(next, c->ev_switch, 0));
+  c->stream = next;
   return KT_OK;
 }
 
@@ -794,18 +830,15 @@ int kt_sync(kt_ctx* c) {
   return check_pass_error(c);
 }
 
-void* kt_host_alloc(size_t bytes) {
-  void* p = nullptr;
-  if (cudaHostAlloc(&p, bytes ? bytes : 1, cudaHostAllocDefault) != cudaSuccess) return nullptr;
-  return p;
-}
-void* kt_host_alloc_upload(size_t bytes) {
-  void* p = nullptr;
-  if (cudaHostAlloc(&p, bytes ? bytes : 1, cudaHostAllocWriteCombined) != cudaSuccess) return nullptr;
-  return p;
-}
+void* kt_host_alloc(size_t bytes) { return host_alloc(bytes, cudaHostAllocDefault); }
+void* kt_host_alloc_upload(size_t bytes) { return host_alloc(bytes, cudaHostAllocWriteCombined); }
 void kt_host_free(void* p) {
-  if (p) cudaFreeHost(p);
+  if (!p) return;
+  {
+    std::lock_guard<std::mutex> lk(g_host_mu);
+    g_host_blocks.erase((uintptr_t)p);
+  }
+  cudaFreeHost(p);
 }
 
 int kt_upload_pods(kt_ctx* c, int kind, int64_t n, const int64_t* labels, const int64_t* req, const uint32_t* present,
@@ -931,7 +964,8 @@ static int upload_pods_packed_locked(kt_ctx* c, int kind, int64_t n, const kt_pa
   KT_CUDA(c, s.ns.reserve((size_t)n * 4 + 16));
   // The columns a caller carved out of ONE pinned block (bench.py, a Go packer with one arena per snapshot) cross the link as
   // one transfer: five copies of a few hundred KB each cost more in per-copy latency than their bytes.  Detected, not declared:
-  // the device-bound arrays span little more than their own size.
+  // the device-bound arrays span little more than their own size, inside one block from kt_host_alloc / kt_host_alloc_upload
+  // (arrays in separate pinned allocations can be neighbours too, and no copy may span two allocations).
   const void* h_ptr[5] = {pk->labels16, pk->pairs, pk->meta, coded ? (const void*)pk->req_codes : (const void*)pk->req32, coded ? (const void*)pk->req_dict : nullptr};
   const size_t h_len[5] = {(size_t)L * n * 2, (size_t)pk->n_pairs * 8, (size_t)n * 4, coded ? code_bytes : (size_t)R * n * 4, coded ? dict_len * 8 : 0};
   uintptr_t lo = UINTPTR_MAX, hi = 0;
@@ -942,7 +976,7 @@ static int upload_pods_packed_locked(kt_ctx* c, int kind, int64_t n, const kt_pa
       hi = std::max(hi, (uintptr_t)h_ptr[i] + h_len[i]);
       sum += h_len[i];
     }
-  const bool one_block = n > 0 && sum > 0 && (lo & 15) == 0 && hi - lo <= sum + 2048;
+  const bool one_block = n > 0 && sum > 0 && (lo & 15) == 0 && hi - lo <= sum + 2048 && in_one_host_block(lo, hi);
   const uint16_t* d_labels16;
   const int64_t* d_pairs;
   const uint32_t* d_meta;
@@ -1288,11 +1322,13 @@ static int evaluate_locked(kt_ctx* c, int64_t now, uint32_t flags) {
     px.rank = c->rank;
   }
   if (tm) KT_CUDA(c, cudaEventRecord(c->ev[0], c->stream));
+  bool own_primary = false;  // the kernel right before k_finalize in the stream is this call's
   if (do_rec && run.n > 0 && M > 0) {
     const PodView pv = pod_view(run);
     const unsigned blocks = (unsigned)((run.n + kTileReconcile - 1) / kTileReconcile);
     KT_CUDA(c, dispatch_reconcile(c, pv, tb, px.mine, blocks));
     run.bitmap_clean = true;
+    own_primary = true;
     ++launches;
   }
   if (tm) KT_CUDA(c, cudaEventRecord(c->ev[1], c->stream));
@@ -1300,12 +1336,15 @@ static int evaluate_locked(kt_ctx* c, int64_t now, uint32_t flags) {
     // the single exchange of the pass: int64 sum of the per-throttle partials over NVLink
     int e = g_nccl.AllReduce(px.mine, px.mine, (size_t)(2 * R + 1) * M, kNcclInt64, kNcclSum, c->comm, c->stream);
     if (e != 0) return fail(c, KT_ERR_NCCL, "ncclAllReduce: %s", g_nccl.GetErrorString ? g_nccl.GetErrorString(e) : "error");
+    own_primary = true;
   }
   if (tm) KT_CUDA(c, cudaEventRecord(c->ev[2], c->stream));
   if (M > 0) {
-    // PDL: overlaps its launch + override merge with the tail of k_reconcile (or of the all-reduce kernel)
+    // PDL: overlaps its launch + override merge with the tail of k_reconcile (or of the all-reduce kernel).  k_finalize writes
+    // pre-records and zeroes the other partial-sum half BEFORE its wait, so without a primary of this call (a check-only pass:
+    // the kernel ahead is the caller's previous launch, maybe a k_pass still reading pre-records) it is a plain launch.
     const long long lanes = (long long)M * G;
-    KT_CUDA(c, launch(c, k_finalize, (unsigned)((lanes + 127) / 128), 128, 0, /*pdl=*/!tm, tv, M, R, G, (long long)now, flags, px, ov,
+    KT_CUDA(c, launch(c, k_finalize, (unsigned)((lanes + 127) / 128), 128, 0, /*pdl=*/!tm && own_primary, tv, M, R, G, (long long)now, flags, px, ov,
                       c->d_pre.as<unsigned char>()));
     ++launches;
   }
@@ -1314,7 +1353,7 @@ static int evaluate_locked(kt_ctx* c, int64_t now, uint32_t flags) {
     const PodView pv = pod_view(pend);
     const unsigned blocks = (unsigned)((pend.n + kTileCheck - 1) / kTileCheck);
     if (c->sparse_cap) KT_CUDA(c, cudaMemsetAsync(c->d_sparse.p, 0, 4, c->stream));  // k_check appends; nobody in it can clear first
-    KT_CUDA(c, dispatch_check(c, pv, tb, px, blocks, /*pdl=*/!tm && M > 0));
+    KT_CUDA(c, dispatch_check(c, pv, tb, px, blocks, /*pdl=*/!tm && M > 0));  // its primary: this call's k_finalize
     pend.bitmap_clean = true;
     ++launches;
   }

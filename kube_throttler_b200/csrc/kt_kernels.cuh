@@ -1824,9 +1824,9 @@ __global__ void __launch_bounds__(TILE, THREADS / TILE) k_pass(const __grid_cons
   __shared__ unsigned s_done[2];              // first-phase tiles this CTA has finished and not yet published: match, reconcile
   __shared__ unsigned long long s_t_start;    // trace: when the current tile began
   __shared__ __align__(8) unsigned long long s_mbar[kMaxWarps];  // transaction barriers: one per warp (bulk copies of the shared decide tiles)
-  // Launched with programmatic stream serialization: the NEXT launch in the stream (normally the next pass) may have its CTAs
-  // placed while this one still runs -- they sit in the wait below until this grid has completed and flushed, so nothing of
-  // theirs (tickets, counters, sums) can mix with ours; what overlaps is their launch latency.
+  // Launched with programmatic stream serialization, and we trigger at once: the NEXT launch in the stream may have its CTAs
+  // placed while this grid still runs.  A next k_pass sits in the wait below; any other kernel that follows with PDL must wait
+  // before its first access to shared state, which is why a pass that does not start with k_pass launches k_finalize plainly.
   pdl_launch_dependents();
   if (threadIdx.x == 0) {
 #pragma unroll
