@@ -27,27 +27,30 @@ namespace {
 
 using namespace kt;
 
-// ---- grow-only device buffer ---------------------------------------------------------------------
-struct DevBuf {
+// ---- grow-only buffers: device memory (DevBuf) and pinned host memory (PinnedBuf) -------------------------
+template <cudaError_t (*Alloc)(void**, size_t), cudaError_t (*Free)(void*)>
+struct GrowBuf {
   void* p = nullptr;
   size_t cap = 0;
   cudaError_t reserve(size_t bytes) {
     if (bytes <= cap) return cudaSuccess;
-    if (p) cudaFree(p);
+    if (p) Free(p);
     p = nullptr;
     cap = 0;
     size_t want = bytes + bytes / 8 + 256;  // slack so row appends do not reallocate every time
-    cudaError_t e = cudaMalloc(&p, want);
+    cudaError_t e = Alloc(&p, want);
     if (e == cudaSuccess) cap = want;
     return e;
   }
   void release() {
-    if (p) cudaFree(p);
+    if (p) Free(p);
     p = nullptr;
     cap = 0;
   }
   template <class T> T* as() const { return reinterpret_cast<T*>(p); }
 };
+using DevBuf = GrowBuf<cudaMalloc, cudaFree>;
+using PinnedBuf = GrowBuf<cudaMallocHost, cudaFreeHost>;
 
 struct PodStore {
   int64_t n = 0;
@@ -58,7 +61,8 @@ struct PodStore {
   DevBuf c_labels, c_req, c_meta;  // staging of the compact transfer format (kt_upload_pods_compact)
   DevBuf c_pairs;                  // label-pair dictionary of the packed transfer format (kt_upload_pods_packed)
   DevBuf c_dict;                   // request-value dictionaries of the same format
-  DevBuf t_rows, t_labels, t_req, t_present, t_flags, t_ns, t_words;  // grow-only staging of row deltas / row gathers
+  DevBuf t_rows, t_labels, t_req, t_present, t_flags, t_ns;  // grow-only staging of row deltas
+  DevBuf t_words;                                            // per-row results gathered into caller order (to_caller_order)
   DevBuf bitmap;  // [n][Wp]
   // The passes MAINTAIN the bitmap (and, for pending rows, the check codes): they store the words of each row's namespace list
   // and nothing else.  Whatever can leave a stale non-zero word outside those lists -- new rows, a row delta, new tables, a
@@ -172,28 +176,25 @@ struct kt_ctx {
   bool have_diff = false;  // the last pass produced a diff (an observed status was uploaded)
   DevBuf d_col_idx, d_col_cnt, d_col_off, d_col_rows;  // per-throttle row lists (kt_admit.cuh ColumnView): kt_admit_queue, kt_get_match_columns
   DevBuf d_adm_state, d_adm_fail, d_adm_counters;      // kt_admit_queue (kt_admit.cuh)
-  DevBuf d_key_list, d_key_reach, d_key_scratch, d_key_acc, d_key_out;  // kt_reconcile_throttles (kt_keyed.cuh): scratch of one call
-  DevBuf d_chk_rows, d_chk_pre, d_chk_out;  // kt_check_pending_rows (kt_keyed.cuh): scratch of one call
-  DevBuf d_mp_in, d_mp_out;                 // kt_match_pods (kt_keyed.cuh): scratch of one call
+  DevBuf d_key_reach, d_key_scratch, d_key_acc;  // kt_reconcile_throttles (kt_keyed.cuh): device-only scratch of one call
+  DevBuf d_chk_pre;                               // kt_check_pending_rows (kt_keyed.cuh): pre-records of one call
+  // What one call sends in (listed rows, throttles, pod values) and brings out (a block of results), and the pinned host
+  // copy a block lands in when its results are scattered into several caller arrays.  Staging of the call that uses them:
+  // no call reads what another left there.
+  DevBuf d_call_in, d_call_out;
+  PinnedBuf h_call;
   DevBuf d_pre;    // [M] pre-records, finalize tiles -> decide tiles (kt_kernels.cuh pre_record_bytes)
-  // per-throttle outputs of the reconcile half: ONE device block (and one pinned host mirror) so that kt_get_reconcile
-  // is a single D2H copy; o_off[i] = byte offset of {used, used_cnt, calc_thr, calc_cnt, used_present, throttled,
-  // calc_present, override_active}
-  DevBuf d_out;
-  void* h_out = nullptr;
-  size_t h_out_cap = 0, out_bytes = 0;
-  size_t o_off[8] = {};
+  DevBuf d_out;    // the reconcile half's per-throttle outputs: ONE status block of M columns (status_layout)
   bool async_uploads = false;  // kt_set_async_uploads
   cudaEvent_t ev_switch = nullptr;  // kt_set_stream: the new stream waits for what was queued on the old one
   // kt_step_submit / kt_step_wait: one pinned result block, one event
-  void* h_step = nullptr;
-  size_t h_step_cap = 0, step_off[3] = {};
+  PinnedBuf h_step;
+  size_t step_off[3] = {};
   cudaEvent_t ev_step = nullptr;
   int64_t step_first = 0;
   bool step_pending = false;
   DevBuf d_codes, d_admit;
   bool have_codes = false;      // a checking pass wrote d_codes / d_admit for the current pending rows and throttle columns
-  DevBuf d_sum;                 // kt_get_check_summary (kt_keyed.cuh): {row classes | per-throttle outputs} of one call
   DevBuf d_sparse;              // kt_set_sparse_check: {count u32, pad to 16 B, entries [cap][3] u32}
   uint32_t sparse_cap = 0;      // 0: off
   uint32_t sparse_guess = 1024; // entries fetched together with the count (adapts to the last pass)
@@ -277,6 +278,33 @@ int check_pass_error(kt_ctx* c) {
   c->evaluated = false;
   return fail(c, KT_ERR_STATE, "the pass timed out waiting for a peer rank (or for its own tiles): results are void");
 }
+// Before a getter reads what the last pass left: the device, then the pass's own verdict on its waits.
+int device_ready(kt_ctx* c) {
+  int rc = set_device(c);
+  return rc ? rc : check_pass_error(c);
+}
+
+// ---- argument checks: one per condition; every entry point calls the ones it needs, in its own order ----------------
+int check_kind(kt_ctx* c, const char* call, int kind) {
+  if (kind == KT_PODS_RUNNING || kind == KT_PODS_PENDING) return KT_OK;
+  return fail(c, KT_ERR_INVALID, "%s: bad pod kind %d", call, kind);
+}
+// k caller rows in [0, n)
+int check_rows(kt_ctx* c, const char* call, int64_t k, const int64_t* rows, int64_t n) {
+  for (int64_t i = 0; i < k; ++i)
+    if (rows[i] < 0 || rows[i] >= n) return fail(c, KT_ERR_INVALID, "%s: row %lld out of range [0,%lld)", call, (long long)rows[i], (long long)n);
+  return KT_OK;
+}
+// k throttle columns in [0, M)
+int check_throttles(kt_ctx* c, const char* call, int64_t k, const int32_t* idx) {
+  for (int64_t i = 0; i < k; ++i)
+    if (idx[i] < 0 || idx[i] >= c->M) return fail(c, KT_ERR_INVALID, "%s: throttle %d out of range [0,%d)", call, idx[i], c->M);
+  return KT_OK;
+}
+int check_single_gpu(kt_ctx* c, const char* call) {
+  if (!c->comm) return KT_OK;
+  return fail(c, KT_ERR_STATE, "%s is single-GPU: this context has a communicator", call);
+}
 
 TableView table_view(const kt_ctx* c) {
   TableView tb;
@@ -312,6 +340,63 @@ ThrottleView throttle_view(const kt_ctx* c) {
     tv.reserved_cnt = c->d_reserved_cnt.as<int64_t>();
   }
   return tv;
+}
+
+// ---- the status block -----------------------------------------------------------------------------------------------
+// The eight kt_reconcile_out columns of m throttles in one block, every column padded to 16 bytes:
+//   {used[R][m], used_cnt[m], calc_thr[R][m], calc_cnt[m], used_present[m], throttled[m], calc_present[m], override_active[m]}
+// The pass writes its M columns into one (d_out), so that kt_get_reconcile and a step download them in one copy; the keyed
+// calls gather or compute their k columns into one of the same shape.
+struct StatusLayout {
+  size_t used, used_cnt, calc_thr, calc_cnt, used_present, throttled, calc_present, override_active, bytes;
+};
+StatusLayout status_layout(int R, int64_t m) {
+  StatusLayout l;
+  size_t at = 0;
+  auto col = [&](size_t bytes) {
+    const size_t o = at;
+    at += (bytes + 15) & ~(size_t)15;
+    return o;
+  };
+  const size_t res = (size_t)R * m * 8;
+  l.used = col(res); l.used_cnt = col((size_t)m * 8); l.calc_thr = col(res); l.calc_cnt = col((size_t)m * 8);
+  l.used_present = col((size_t)m * 4); l.throttled = col((size_t)m * 4); l.calc_present = col((size_t)m * 4); l.override_active = col((size_t)m);
+  l.bytes = at;
+  return l;
+}
+// The columns of the block at `base`: View is ReconcileView over device memory or kt_reconcile_out over a landed host copy.
+template <class View>
+View status_at(void* base, int R, int64_t m) {
+  const StatusLayout l = status_layout(R, m);
+  unsigned char* b = static_cast<unsigned char*>(base);
+  View v{};
+  v.used = reinterpret_cast<int64_t*>(b + l.used); v.used_cnt = reinterpret_cast<int64_t*>(b + l.used_cnt);
+  v.calc_thr = reinterpret_cast<int64_t*>(b + l.calc_thr); v.calc_cnt = reinterpret_cast<int64_t*>(b + l.calc_cnt);
+  v.used_present = reinterpret_cast<uint32_t*>(b + l.used_present); v.throttled = reinterpret_cast<uint32_t*>(b + l.throttled);
+  v.calc_present = reinterpret_cast<uint32_t*>(b + l.calc_present); v.override_active = reinterpret_cast<uint8_t*>(b + l.override_active);
+  return v;
+}
+// A landed block of m columns into the caller's columns, skipping the NULL ones.
+void copy_status(const kt_reconcile_out& src, const kt_reconcile_out* dst, int R, int64_t m) {
+  auto put = [](void* d, const void* s, size_t bytes) {
+    if (d && bytes) std::memcpy(d, s, bytes);
+  };
+  const size_t res = (size_t)R * m * 8;
+  put(dst->used, src.used, res); put(dst->used_cnt, src.used_cnt, (size_t)m * 8);
+  put(dst->calc_thr, src.calc_thr, res); put(dst->calc_cnt, src.calc_cnt, (size_t)m * 8);
+  put(dst->used_present, src.used_present, (size_t)m * 4); put(dst->throttled, src.throttled, (size_t)m * 4);
+  put(dst->calc_present, src.calc_present, (size_t)m * 4); put(dst->override_active, src.override_active, (size_t)m);
+}
+
+// The partial-sum buffers of a pass that exchanges nothing with other ranks: a reconciling pass adds into the half of
+// part_parity and zeroes the other one for its successor.
+PartExchange local_exchange(const kt_ctx* c) {
+  PartExchange px{};
+  px.mine = px.total = reinterpret_cast<unsigned long long*>(c->d_part.as<unsigned char>() + (size_t)c->part_parity * c->part_stride);
+  px.zero_mine = reinterpret_cast<unsigned long long*>(c->d_part.as<unsigned char>() + (size_t)(c->part_parity ^ 1u) * c->part_stride);
+  px.sync = c->d_sync.as<PassSync>();
+  px.rank = c->rank;
+  return px;
 }
 
 PodView pod_view(const PodStore& s) {
@@ -429,6 +514,30 @@ int order_rows(kt_ctx* c, PodStore& s, int64_t n, int64_t ns_limit) {
 }
 // caller row -> device row, or nullptr when the rows are stored as given
 const uint32_t* dev_of(const PodStore& s) { return s.clustered ? s.o_dev.as<uint32_t>() : nullptr; }
+// k caller rows -> `buf` on the device, as rows of the store's layout (mapped to device rows when it is laid out by namespace)
+int stage_rows(kt_ctx* c, const PodStore& s, DevBuf& buf, int64_t k, const int64_t* rows) {
+  int rc = upload(c, buf, rows, (size_t)k);
+  if (rc) return rc;
+  if (s.clustered) k_order_map_rows<<<(unsigned)((k + 255) / 256), 256, 0, c->stream>>>(k, s.o_dev.as<uint32_t>(), buf.as<int64_t>());
+  return KT_OK;
+}
+// The end of every full upload: the n rows just landed in caller order are laid out by namespace when `cluster`, and
+// everything computed from the previous rows is void.
+int finish_upload(kt_ctx* c, int kind, int64_t n, bool cluster, int64_t ns_limit, bool roff_valid) {
+  PodStore& s = c->pods[kind];
+  s.clustered = false;
+  if (cluster) {
+    int rc = order_rows(c, s, n, ns_limit);
+    if (rc) return rc;
+  }
+  s.n = n;
+  s.roff_valid = roff_valid;
+  s.bitmap_clean = false;
+  c->evaluated = false;
+  if (kind == KT_PODS_PENDING) c->have_codes = false;
+  if (!c->async_uploads) KT_CUDA(c, cudaStreamSynchronize(c->stream));  // the caller may reuse its buffers as soon as we return
+  return KT_OK;
+}
 // n per-row results of `W` u32 words (bitmap rows, code rows; W = 0: one byte per row) gathered into caller order in the
 // store's staging buffer; returns it
 template <class T>
@@ -756,10 +865,9 @@ void kt_destroy(kt_ctx* c) {
                    &c->d_st_used, &c->d_st_used_present, &c->d_st_used_cnt, &c->d_st_throttled, &c->d_reserved, &c->d_reserved_present,
                    &c->d_reserved_cnt, &c->d_part, &c->d_sync, &c->d_trace, &c->d_pre, &c->d_changed, &c->d_col_idx, &c->d_col_cnt, &c->d_col_off,
                    &c->d_col_rows, &c->d_adm_state, &c->d_adm_fail, &c->d_adm_counters, &c->d_out, &c->d_codes, &c->d_admit,
-                   &c->d_key_list, &c->d_key_reach, &c->d_key_scratch, &c->d_key_acc, &c->d_key_out, &c->d_chk_rows, &c->d_chk_pre, &c->d_chk_out,
-                   &c->d_mp_in, &c->d_mp_out};
-  if (c->h_out) cudaFreeHost(c->h_out);
-  if (c->h_step) cudaFreeHost(c->h_step);
+                   &c->d_key_reach, &c->d_key_scratch, &c->d_key_acc, &c->d_chk_pre, &c->d_call_in, &c->d_call_out};
+  c->h_call.release();
+  c->h_step.release();
   if (c->ev_step) cudaEventDestroy(c->ev_step);
   if (c->ev_switch) cudaEventDestroy(c->ev_switch);
   if (c->h_sparse_count) cudaFreeHost(c->h_sparse_count);
@@ -845,7 +953,7 @@ int kt_upload_pods(kt_ctx* c, int kind, int64_t n, const int64_t* labels, const 
                    const uint32_t* flags, const int32_t* ns_id) {
   if (!c) return KT_ERR_INVALID;
   std::lock_guard<std::mutex> lk(c->mu);
-  if (kind != KT_PODS_RUNNING && kind != KT_PODS_PENDING) return fail(c, KT_ERR_INVALID, "bad pod kind %d", kind);
+  if (int rc = check_kind(c, __func__, kind)) return rc;
   if (n < 0 || (n > 0 && (!labels || !req || !present || !flags || !ns_id))) return fail(c, KT_ERR_INVALID, "null pod columns");
   int rc = set_device(c);
   if (rc) return rc;
@@ -863,21 +971,15 @@ int kt_upload_pods(kt_ctx* c, int kind, int64_t n, const int64_t* labels, const 
   if ((rc = upload(c, s.present, present, (size_t)n))) return rc;
   if ((rc = upload(c, s.flags, flags, (size_t)n))) return rc;
   if ((rc = upload(c, s.ns, ns_id, (size_t)n))) return rc;
-  s.clustered = false;
-  if (choose_clustered(s, n, [&](int64_t i, int32_t* ns) { *ns = ns_id[i]; return flags[i] != 0; }) && (rc = order_rows(c, s, n, (int64_t)1 << 31))) return rc;
-  s.n = n;
-  s.roff_valid = s.bitmap_clean = false;
-  c->evaluated = false;
-  if (kind == KT_PODS_PENDING) c->have_codes = false;
-  if (!c->async_uploads) KT_CUDA(c, cudaStreamSynchronize(c->stream));  // the caller may reuse its buffers as soon as we return
-  return KT_OK;
+  const bool cluster = choose_clustered(s, n, [&](int64_t i, int32_t* ns) { *ns = ns_id[i]; return flags[i] != 0; });
+  return finish_upload(c, kind, n, cluster, (int64_t)1 << 31, false);
 }
 
 int kt_upload_pods_compact(kt_ctx* c, int kind, int64_t n, int32_t val_bits, const uint32_t* labels32, const int32_t* req32, const int32_t* req_shift,
                            const uint32_t* present, const uint32_t* meta) {
   if (!c) return KT_ERR_INVALID;
   std::lock_guard<std::mutex> lk(c->mu);
-  if (kind != KT_PODS_RUNNING && kind != KT_PODS_PENDING) return fail(c, KT_ERR_INVALID, "bad pod kind %d", kind);
+  if (int rc = check_kind(c, __func__, kind)) return rc;
   if (n < 0 || !req_shift || (n > 0 && (!labels32 || !req32 || !present || !meta))) return fail(c, KT_ERR_INVALID, "null compact pod columns");
   if (val_bits < 1 || val_bits > 31) return fail(c, KT_ERR_INVALID, "val_bits %d outside 1..31", val_bits);
   const int L = c->lim.label_slots, R = c->lim.n_resources, Lpad = (L + 7) & ~7;
@@ -901,16 +1003,8 @@ int kt_upload_pods_compact(kt_ctx* c, int kind, int64_t n, int32_t val_bits, con
                                                                       s.flags.as<uint32_t>(), s.ns.as<int32_t>());
     KT_CUDA(c, cudaGetLastError());
   }
-  s.clustered = false;
-  if (choose_clustered(s, n, [&](int64_t i, int32_t* ns) { *ns = (int32_t)(meta[i] & 0x1fffffffu); return (meta[i] >> 29) != 0; }) &&
-      (rc = order_rows(c, s, n, (int64_t)1 << 29)))
-    return rc;
-  s.n = n;
-  s.roff_valid = s.bitmap_clean = false;
-  c->evaluated = false;
-  if (kind == KT_PODS_PENDING) c->have_codes = false;
-  if (!c->async_uploads) KT_CUDA(c, cudaStreamSynchronize(c->stream));  // the caller may reuse its buffers as soon as we return
-  return KT_OK;
+  const bool cluster = choose_clustered(s, n, [&](int64_t i, int32_t* ns) { *ns = (int32_t)(meta[i] & 0x1fffffffu); return (meta[i] >> 29) != 0; });
+  return finish_upload(c, kind, n, cluster, (int64_t)1 << 29, false);
 }
 
 static int upload_pods_packed_locked(kt_ctx* c, int kind, int64_t n, const kt_packed_pods* pk);
@@ -920,7 +1014,7 @@ int kt_upload_pods_packed(kt_ctx* c, int kind, int64_t n, const kt_packed_pods* 
   return upload_pods_packed_locked(c, kind, n, pk);
 }
 static int upload_pods_packed_locked(kt_ctx* c, int kind, int64_t n, const kt_packed_pods* pk) {
-  if (kind != KT_PODS_RUNNING && kind != KT_PODS_PENDING) return fail(c, KT_ERR_INVALID, "bad pod kind %d", kind);
+  if (int rc = check_kind(c, "kt_upload_pods_packed", kind)) return rc;
   if (n < 0 || !pk || (n > 0 && (!pk->labels16 || !pk->meta))) return fail(c, KT_ERR_INVALID, "null packed pod columns");
   const bool coded = pk->req_codes != nullptr;
   if (coded ? (!pk->req_dict_off || !pk->req_code_bytes) : (!pk->req_shift || (n > 0 && !pk->req32)))
@@ -957,6 +1051,9 @@ static int upload_pods_packed_locked(kt_ctx* c, int kind, int64_t n, const kt_pa
     *ns = (int32_t)(m & ns_mask);
     return ((m >> pk->ns_bits) & 7u) != 0;
   });
+  // with tables in place the rows are translated (labels -> table row offsets, namespace -> word info) in the unpacking
+  // kernel: one launch and one read of the labels less per upload (rows laid out by namespace are translated after the move)
+  const bool fuse = n > 0 && c->have_throttles && !cluster;
   KT_CUDA(c, s.labels.reserve((size_t)Lpad * n * 8 + 16));
   KT_CUDA(c, s.req.reserve((size_t)R * n * 8 + 16));
   KT_CUDA(c, s.present.reserve((size_t)n * 4 + 16));
@@ -1015,9 +1112,6 @@ static int upload_pods_packed_locked(kt_ctx* c, int kind, int64_t n, const kt_pa
     ReqShifts sh{};
     if (!coded)
       for (int r = 0; r < R; ++r) sh.s[r] = (unsigned char)pk->req_shift[r];
-    // with tables in place the rows are translated (labels -> table row offsets, namespace -> word info) in the same kernel:
-    // one launch and one read of the labels less per upload (rows laid out by namespace are translated after the move)
-    const bool fuse = c->have_throttles && !cluster;
     if (fuse) {
       KT_CUDA(c, s.roff.reserve((size_t)Lpad * n * 4 + 16));
       KT_CUDA(c, s.winfo.reserve((size_t)n * 4 + 16));
@@ -1027,40 +1121,27 @@ static int upload_pods_packed_locked(kt_ctx* c, int kind, int64_t n, const kt_pa
                                                                         s.req.as<int64_t>(), s.present.as<uint32_t>(), s.flags.as<uint32_t>(), s.ns.as<int32_t>(),
                                                                         fuse ? 1 : 0, fuse ? table_view(c) : TableView{}, s.roff.as<uint32_t>(), s.winfo.as<uint32_t>());
     KT_CUDA(c, cudaGetLastError());
-    s.clustered = false;
-    if (cluster && (err = order_rows(c, s, n, (int64_t)1 << pk->ns_bits))) return err;
-    s.n = n;
-    s.roff_valid = fuse;
-    s.bitmap_clean = false;
-  } else {
-    s.n = n;
-    s.clustered = false;
-    s.roff_valid = s.bitmap_clean = false;
   }
-  c->evaluated = false;
-  if (kind == KT_PODS_PENDING) c->have_codes = false;
-  if (!c->async_uploads) KT_CUDA(c, cudaStreamSynchronize(c->stream));  // the caller may reuse its buffers as soon as we return
-  return KT_OK;
+  return finish_upload(c, kind, n, cluster, (int64_t)1 << pk->ns_bits, fuse);
 }
 
 int kt_update_pod_rows(kt_ctx* c, int kind, int64_t k, const int64_t* rows, const int64_t* labels, const int64_t* req,
                        const uint32_t* present, const uint32_t* flags, const int32_t* ns_id) {
   if (!c) return KT_ERR_INVALID;
   std::lock_guard<std::mutex> lk(c->mu);
-  if (kind != KT_PODS_RUNNING && kind != KT_PODS_PENDING) return fail(c, KT_ERR_INVALID, "bad pod kind %d", kind);
+  if (int rc = check_kind(c, __func__, kind)) return rc;
   if (k < 0 || (k > 0 && (!rows || !labels || !req || !present || !flags || !ns_id))) return fail(c, KT_ERR_INVALID, "null delta columns");
   if (k == 0) return KT_OK;
   PodStore& s = c->pods[kind];
-  for (int64_t i = 0; i < k; ++i)
-    if (rows[i] < 0 || rows[i] >= s.n) return fail(c, KT_ERR_INVALID, "delta row %lld out of range [0,%lld)", (long long)rows[i], (long long)s.n);
+  if (int rc = check_rows(c, __func__, k, rows, s.n)) return rc;
   int rc = set_device(c);
   if (rc) return rc;
   const int L = c->lim.label_slots, R = c->lim.n_resources;
-  // grow-only staging buffers: an informer event must not cost a cudaMalloc/cudaFree pair
-  if ((rc = upload(c, s.t_rows, rows, (size_t)k)) || (rc = upload(c, s.t_labels, labels, (size_t)L * k)) || (rc = upload(c, s.t_req, req, (size_t)R * k)) ||
+  // grow-only staging buffers: an informer event must not cost a cudaMalloc/cudaFree pair.  The layout stays: the rows land
+  // where the listed caller rows live.
+  if ((rc = stage_rows(c, s, s.t_rows, k, rows)) || (rc = upload(c, s.t_labels, labels, (size_t)L * k)) || (rc = upload(c, s.t_req, req, (size_t)R * k)) ||
       (rc = upload(c, s.t_present, present, (size_t)k)) || (rc = upload(c, s.t_flags, flags, (size_t)k)) || (rc = upload(c, s.t_ns, ns_id, (size_t)k)))
     return rc;
-  if (s.clustered) k_order_map_rows<<<(unsigned)((k + 255) / 256), 256, 0, c->stream>>>(k, s.o_dev.as<uint32_t>(), s.t_rows.as<int64_t>());  // the layout stays
   k_scatter_rows<<<(unsigned)((k + 255) / 256), 256, 0, c->stream>>>(k, s.t_rows.as<int64_t>(), L, R, s.n, s.t_labels.as<int64_t>(), s.t_req.as<int64_t>(),
                                                                      s.t_present.as<uint32_t>(), s.t_flags.as<uint32_t>(), s.t_ns.as<int32_t>(),
                                                                      s.labels.as<int64_t>(), s.req.as<int64_t>(), s.present.as<uint32_t>(),
@@ -1122,20 +1203,9 @@ int kt_upload_throttles(kt_ctx* c, int32_t m, const kt_throttle_cols* cols, cons
   KT_CUDA(c, c->d_changed.reserve(16 + (size_t)m * 5 + 16));
   KT_CUDA(c, cudaMemsetAsync(c->d_changed.p, 0, 16, c->stream));
   c->have_diff = false;
-  {
-    const size_t sizes[8] = {(size_t)R * m * 8, (size_t)m * 8, (size_t)R * m * 8, (size_t)m * 8, (size_t)m * 4, (size_t)m * 4, (size_t)m * 4, (size_t)m};
-    size_t at = 0;
-    for (int i = 0; i < 8; ++i) { c->o_off[i] = at; at += (sizes[i] + 15) & ~(size_t)15; }
-    c->out_bytes = at;
-    KT_CUDA(c, c->d_out.reserve(at + 16));
-    if (c->h_out_cap < at) {
-      if (c->h_out) cudaFreeHost(c->h_out);
-      c->h_out = nullptr;
-      c->h_out_cap = 0;
-      KT_CUDA(c, cudaHostAlloc(&c->h_out, at + 16, cudaHostAllocDefault));
-      c->h_out_cap = at;
-    }
-  }
+  const size_t out_bytes = status_layout(R, m).bytes;
+  KT_CUDA(c, c->d_out.reserve(out_bytes + 16));
+  KT_CUDA(c, c->h_call.reserve(out_bytes));  // kt_get_reconcile lands the block there
   c->have_throttles = true;
   c->have_status = false;
   c->have_reserved = false;
@@ -1223,10 +1293,7 @@ static int evaluate_locked(kt_ctx* c, int64_t now, uint32_t flags) {
   const bool tm = c->timing;
 
   const ThrottleView tv = throttle_view(c);
-  unsigned char* ob = c->d_out.as<unsigned char>();
-  ReconcileView ov{reinterpret_cast<int64_t*>(ob + c->o_off[0]), reinterpret_cast<uint32_t*>(ob + c->o_off[4]), reinterpret_cast<int64_t*>(ob + c->o_off[1]),
-                   reinterpret_cast<uint32_t*>(ob + c->o_off[5]), reinterpret_cast<int64_t*>(ob + c->o_off[2]), reinterpret_cast<uint32_t*>(ob + c->o_off[6]),
-                   reinterpret_cast<int64_t*>(ob + c->o_off[3]), reinterpret_cast<uint8_t*>(ob + c->o_off[7]), nullptr, nullptr, nullptr, nullptr};
+  ReconcileView ov = status_at<ReconcileView>(c->d_out.p, R, M);
   c->have_diff = c->have_status && do_rec && M > 0;
   if (c->have_diff) {
     c->diff_parity ^= 1u;
@@ -1240,11 +1307,7 @@ static int evaluate_locked(kt_ctx* c, int64_t now, uint32_t flags) {
   while (G < R + 1) G <<= 1;  // finalize lanes per throttle: resources + the pod count, padded to a power of two
   // partial sums: a reconciling pass takes the half its predecessor left zeroed and zeroes the other one for its successor
   if (do_rec) c->part_parity ^= 1u;
-  PartExchange px{};
-  px.mine = px.total = reinterpret_cast<unsigned long long*>(c->d_part.as<unsigned char>() + (size_t)c->part_parity * c->part_stride);
-  px.zero_mine = reinterpret_cast<unsigned long long*>(c->d_part.as<unsigned char>() + (size_t)(c->part_parity ^ 1u) * c->part_stride);
-  px.sync = c->d_sync.as<PassSync>();
-  px.rank = c->rank;
+  PartExchange px = local_exchange(c);
 
   // ---- the whole pass in one launch (k_pass), both halves asked for.  With several ranks the all-reduce happens
   // inside it: finalize tiles add this rank's partial sums into every rank's totals over NVLink (exchange windows). ----
@@ -1314,13 +1377,7 @@ static int evaluate_locked(kt_ctx* c, int64_t now, uint32_t flags) {
   }
 
   // ---- separate kernels, PDL-chained: partial passes (SKIP_*), per-kernel timing, NCCL all-reduce in between ----
-  if (px.npeers > 0) {  // the window was set up but the one-launch pass is not taken after all: this rank's own buffers
-    px = PartExchange{};
-    px.mine = px.total = reinterpret_cast<unsigned long long*>(c->d_part.as<unsigned char>() + (size_t)c->part_parity * c->part_stride);
-    px.zero_mine = reinterpret_cast<unsigned long long*>(c->d_part.as<unsigned char>() + (size_t)(c->part_parity ^ 1u) * c->part_stride);
-    px.sync = c->d_sync.as<PassSync>();
-    px.rank = c->rank;
-  }
+  if (px.npeers > 0) px = local_exchange(c);  // the window was set up but the one-launch pass is not taken after all: this rank's own buffers
   if (tm) KT_CUDA(c, cudaEventRecord(c->ev[0], c->stream));
   bool own_primary = false;  // the kernel right before k_finalize in the stream is this call's
   if (do_rec && run.n > 0 && M > 0) {
@@ -1464,18 +1521,12 @@ int kt_step_submit(kt_ctx* c, int64_t n_running, const kt_packed_pods* running, 
   if (rc) return rc;
   // results -> ONE pinned block: [status block | admit | sparse count | first entries]
   const int64_t P = c->pods[KT_PODS_PENDING].n;
-  const size_t off_admit = (c->out_bytes + 63) & ~(size_t)63, off_cnt = (off_admit + (size_t)P + 63) & ~(size_t)63, off_ent = off_cnt + 16;
-  const size_t need = off_ent + (size_t)c->sparse_cap * 12 + 64;
-  if (c->h_step_cap < need) {
-    if (c->h_step) cudaFreeHost(c->h_step);
-    c->h_step = nullptr;
-    c->h_step_cap = 0;
-    KT_CUDA(c, cudaHostAlloc(&c->h_step, need, cudaHostAllocDefault));
-    c->h_step_cap = need;
-  }
+  const size_t out_bytes = status_layout(c->lim.n_resources, c->M).bytes;
+  const size_t off_admit = (out_bytes + 63) & ~(size_t)63, off_cnt = (off_admit + (size_t)P + 63) & ~(size_t)63, off_ent = off_cnt + 16;
+  KT_CUDA(c, c->h_step.reserve(off_ent + (size_t)c->sparse_cap * 12 + 64));
   if (!c->ev_step) KT_CUDA(c, cudaEventCreateWithFlags(&c->ev_step, cudaEventDisableTiming));
-  unsigned char* hb = reinterpret_cast<unsigned char*>(c->h_step);
-  if (c->out_bytes) KT_CUDA(c, cudaMemcpyAsync(hb, c->d_out.p, c->out_bytes, cudaMemcpyDeviceToHost, c->stream));
+  unsigned char* hb = c->h_step.as<unsigned char>();
+  if (out_bytes) KT_CUDA(c, cudaMemcpyAsync(hb, c->d_out.p, out_bytes, cudaMemcpyDeviceToHost, c->stream));
   if (P > 0) {
     const unsigned char* src;
     if ((rc = admit_in_caller_order(c, &src))) return rc;
@@ -1501,7 +1552,7 @@ int kt_step_wait(kt_ctx* c, kt_step_result* out) {
   KT_CUDA(c, cudaEventSynchronize(c->ev_step));
   c->step_pending = false;
   if ((rc = check_pass_error(c))) return rc;
-  unsigned char* hb = reinterpret_cast<unsigned char*>(c->h_step);
+  unsigned char* hb = c->h_step.as<unsigned char>();
   const int64_t P = c->pods[KT_PODS_PENDING].n;
   const int64_t total = P > 0 ? (int64_t)*reinterpret_cast<uint32_t*>(hb + c->step_off[1]) : 0;
   const int64_t have = total < (int64_t)c->sparse_cap ? total : (int64_t)c->sparse_cap;
@@ -1517,14 +1568,7 @@ int kt_step_wait(kt_ctx* c, kt_step_result* out) {
   out->n_sparse = total;
   out->admit = hb + c->step_off[0];
   out->entries = reinterpret_cast<const uint32_t*>(hb + c->step_off[2]);
-  out->status.used = reinterpret_cast<int64_t*>(hb + c->o_off[0]);
-  out->status.used_cnt = reinterpret_cast<int64_t*>(hb + c->o_off[1]);
-  out->status.calc_thr = reinterpret_cast<int64_t*>(hb + c->o_off[2]);
-  out->status.calc_cnt = reinterpret_cast<int64_t*>(hb + c->o_off[3]);
-  out->status.used_present = reinterpret_cast<uint32_t*>(hb + c->o_off[4]);
-  out->status.throttled = reinterpret_cast<uint32_t*>(hb + c->o_off[5]);
-  out->status.calc_present = reinterpret_cast<uint32_t*>(hb + c->o_off[6]);
-  out->status.override_active = reinterpret_cast<uint8_t*>(hb + c->o_off[7]);
+  out->status = status_at<kt_reconcile_out>(hb, c->lim.n_resources, c->M);
   return KT_OK;
 }
 
@@ -1549,25 +1593,14 @@ int kt_get_reconcile(kt_ctx* c, const kt_reconcile_out* o) {
   if (!c || !o) return KT_ERR_INVALID;
   std::lock_guard<std::mutex> lk(c->mu);
   if (!c->evaluated) return fail(c, KT_ERR_STATE, "kt_get_reconcile before kt_evaluate");
-  int rc = set_device(c);
-  if (rc) return rc;
-  if ((rc = check_pass_error(c))) return rc;
-  const size_t m = (size_t)c->M, R = (size_t)c->lim.n_resources;
+  if (int rc = device_ready(c)) return rc;
+  const int R = c->lim.n_resources, M = c->M;
   // one copy of the whole block into the pinned mirror, then plain host copies into the caller's columns
-  if (c->out_bytes) KT_CUDA(c, cudaMemcpyAsync(c->h_out, c->d_out.p, c->out_bytes, cudaMemcpyDeviceToHost, c->stream));
+  const size_t bytes = status_layout(R, M).bytes;
+  KT_CUDA(c, c->h_call.reserve(bytes));
+  if (bytes) KT_CUDA(c, cudaMemcpyAsync(c->h_call.p, c->d_out.p, bytes, cudaMemcpyDeviceToHost, c->stream));
   KT_CUDA(c, cudaStreamSynchronize(c->stream));
-  const unsigned char* hb = reinterpret_cast<const unsigned char*>(c->h_out);
-  auto put = [&](void* dst, int i, size_t bytes) {
-    if (dst && bytes) std::memcpy(dst, hb + c->o_off[i], bytes);
-  };
-  put(o->used, 0, R * m * 8);
-  put(o->used_cnt, 1, m * 8);
-  put(o->calc_thr, 2, R * m * 8);
-  put(o->calc_cnt, 3, m * 8);
-  put(o->used_present, 4, m * 4);
-  put(o->throttled, 5, m * 4);
-  put(o->calc_present, 6, m * 4);
-  put(o->override_active, 7, m);
+  copy_status(status_at<kt_reconcile_out>(c->h_call.p, R, M), o, R, M);
   return KT_OK;
 }
 
@@ -1576,9 +1609,7 @@ int kt_get_changed(kt_ctx* c, int32_t* idx, int64_t cap, int64_t* count, uint8_t
   std::lock_guard<std::mutex> lk(c->mu);
   if (!c->evaluated) return fail(c, KT_ERR_STATE, "kt_get_changed before kt_evaluate");
   if (!c->have_diff) return fail(c, KT_ERR_STATE, "kt_get_changed: the last pass had no observed status to diff against (kt_upload_status) or did not reconcile");
-  int rc = set_device(c);
-  if (rc) return rc;
-  if ((rc = check_pass_error(c))) return rc;
+  if (int rc = device_ready(c)) return rc;
   uint32_t n = 0;
   KT_CUDA(c, cudaMemcpyAsync(&n, c->d_changed.as<uint32_t>() + c->diff_parity, 4, cudaMemcpyDeviceToHost, c->stream));
   KT_CUDA(c, cudaStreamSynchronize(c->stream));
@@ -1595,41 +1626,20 @@ int kt_get_reconcile_rows(kt_ctx* c, int64_t k, const int32_t* idx, const kt_rec
   std::lock_guard<std::mutex> lk(c->mu);
   if (!c->evaluated) return fail(c, KT_ERR_STATE, "kt_get_reconcile_rows before kt_evaluate");
   if (k == 0) return KT_OK;
+  if (int rc = check_throttles(c, __func__, k, idx)) return rc;
+  if (int rc = device_ready(c)) return rc;
   const int R = c->lim.n_resources, M = c->M;
-  for (int64_t i = 0; i < k; ++i)
-    if (idx[i] < 0 || idx[i] >= M) return fail(c, KT_ERR_INVALID, "throttle %d out of range [0,%d)", idx[i], M);
-  int rc = set_device(c);
-  if (rc) return rc;
-  if ((rc = check_pass_error(c))) return rc;
-  // one packed block per call: {used[R][k], calc_thr[R][k], used_cnt[k], calc_cnt[k], used_present[k], throttled[k], calc_present[k], override_active[k]}
-  const size_t bytes = (size_t)k * ((size_t)2 * R * 8 + 16 + 12 + 1);
-  PodStore& s = c->pods[KT_PODS_RUNNING];  // its grow-only staging buffers serve small gathers
-  KT_CUDA(c, s.t_rows.reserve((size_t)k * 4 + 16));
-  KT_CUDA(c, s.t_words.reserve(bytes + 64));
-  if (c->h_out_cap < bytes + 64) {
-    if (c->h_out) cudaFreeHost(c->h_out);
-    c->h_out = nullptr;
-    c->h_out_cap = 0;
-    KT_CUDA(c, cudaHostAlloc(&c->h_out, bytes + 64, cudaHostAllocDefault));
-    c->h_out_cap = bytes + 64;
-  }
-  KT_CUDA(c, cudaMemcpyAsync(s.t_rows.p, idx, (size_t)k * 4, cudaMemcpyHostToDevice, c->stream));
-  unsigned char* ob = c->d_out.as<unsigned char>();
-  const ReconcileView ov{reinterpret_cast<int64_t*>(ob + c->o_off[0]), reinterpret_cast<uint32_t*>(ob + c->o_off[4]), reinterpret_cast<int64_t*>(ob + c->o_off[1]),
-                         reinterpret_cast<uint32_t*>(ob + c->o_off[5]), reinterpret_cast<int64_t*>(ob + c->o_off[2]), reinterpret_cast<uint32_t*>(ob + c->o_off[6]),
-                         reinterpret_cast<int64_t*>(ob + c->o_off[3]), reinterpret_cast<uint8_t*>(ob + c->o_off[7]), nullptr, nullptr, nullptr, nullptr};
-  k_gather_status<<<(unsigned)((k + 127) / 128), 128, 0, c->stream>>>(k, s.t_rows.as<int32_t>(), R, M, ov, s.t_words.as<unsigned char>());
+  // the listed columns gathered into a status block of k columns: the download is proportional to what changed, not to M
+  const size_t bytes = status_layout(R, k).bytes;
+  if (int rc = upload(c, c->d_call_in, idx, (size_t)k)) return rc;
+  KT_CUDA(c, c->d_call_out.reserve(bytes));
+  KT_CUDA(c, c->h_call.reserve(bytes));
+  k_gather_status<<<(unsigned)((k + 127) / 128), 128, 0, c->stream>>>(k, c->d_call_in.as<int32_t>(), R, M, status_at<ReconcileView>(c->d_out.p, R, M),
+                                                                      status_at<ReconcileView>(c->d_call_out.p, R, k));
   KT_CUDA(c, cudaGetLastError());
-  KT_CUDA(c, cudaMemcpyAsync(c->h_out, s.t_words.p, bytes, cudaMemcpyDeviceToHost, c->stream));
+  KT_CUDA(c, cudaMemcpyAsync(c->h_call.p, c->d_call_out.p, bytes, cudaMemcpyDeviceToHost, c->stream));
   KT_CUDA(c, cudaStreamSynchronize(c->stream));
-  const unsigned char* hb = reinterpret_cast<const unsigned char*>(c->h_out);
-  size_t at = 0;
-  auto take = [&](void* dst, size_t n) {
-    if (dst) std::memcpy(dst, hb + at, n);
-    at += n;
-  };
-  take(o->used, (size_t)R * k * 8); take(o->calc_thr, (size_t)R * k * 8); take(o->used_cnt, (size_t)k * 8); take(o->calc_cnt, (size_t)k * 8);
-  take(o->used_present, (size_t)k * 4); take(o->throttled, (size_t)k * 4); take(o->calc_present, (size_t)k * 4); take(o->override_active, (size_t)k);
+  copy_status(status_at<kt_reconcile_out>(c->h_call.p, R, k), o, R, k);
   return KT_OK;
 }
 
@@ -1638,12 +1648,11 @@ int kt_check_pending_rows(kt_ctx* c, uint32_t flags, int64_t k, const int64_t* r
   if (!c || k < 0 || (k > 0 && !rows)) return KT_ERR_INVALID;
   std::lock_guard<std::mutex> lk(c->mu);
   if (flags & ~KT_EVAL_ON_EQUAL) return fail(c, KT_ERR_INVALID, "kt_check_pending_rows: flags must be 0 or KT_EVAL_ON_EQUAL, not %u", flags);
-  if (c->comm) return fail(c, KT_ERR_STATE, "kt_check_pending_rows is single-GPU: this context has a communicator");
+  if (int rc = check_single_gpu(c, __func__)) return rc;
   if (!c->have_throttles) return fail(c, KT_ERR_STATE, "kt_check_pending_rows before kt_upload_throttles");
   if (!c->have_status) return fail(c, KT_ERR_STATE, "kt_check_pending_rows checks against the observed status: kt_upload_status first");
   PodStore& pend = c->pods[KT_PODS_PENDING];
-  for (int64_t i = 0; i < k; ++i)
-    if (rows[i] < 0 || rows[i] >= pend.n) return fail(c, KT_ERR_INVALID, "row %lld out of range [0,%lld)", (long long)rows[i], (long long)pend.n);
+  if (int rc = check_rows(c, __func__, k, rows, pend.n)) return rc;
   if (k == 0) return KT_OK;
   int rc = set_device(c);
   if (rc) return rc;
@@ -1654,10 +1663,10 @@ int kt_check_pending_rows(kt_ctx* c, uint32_t flags, int64_t k, const int64_t* r
   const size_t adm_bytes = ((size_t)k + 15) & ~(size_t)15, code_bytes = (size_t)k * 2 * Wp * 4, word_bytes = (size_t)k * Wp * 4;
   const size_t out_bytes = adm_bytes + code_bytes + word_bytes;
   const size_t fetch = words ? out_bytes : codes ? adm_bytes + code_bytes : adm_bytes;
-  KT_CUDA(c, c->d_chk_rows.reserve((size_t)k * 8 + 16));
-  KT_CUDA(c, c->d_chk_out.reserve(out_bytes + 16));
-  KT_CUDA(c, cudaMemcpyAsync(c->d_chk_rows.p, rows, (size_t)k * 8, cudaMemcpyHostToDevice, c->stream));
-  KT_CUDA(c, cudaMemsetAsync(c->d_chk_out.p, 0, adm_bytes + code_bytes + word_bytes, c->stream));
+  if ((rc = upload(c, c->d_call_in, rows, (size_t)k))) return rc;
+  KT_CUDA(c, c->d_call_out.reserve(out_bytes + 16));
+  KT_CUDA(c, c->h_call.reserve(fetch));
+  KT_CUDA(c, cudaMemsetAsync(c->d_call_out.p, 0, out_bytes, c->stream));
   if (M > 0) {  // the pre-records of every throttle (the pass's prep half, GIVEN_STATUS: no clock is read)
     KT_CUDA(c, c->d_chk_pre.reserve((size_t)M * pre_record_bytes(R) + 16));
     int G = 1;
@@ -1666,12 +1675,12 @@ int kt_check_pending_rows(kt_ctx* c, uint32_t flags, int64_t k, const int64_t* r
     k_rows_prep<<<(unsigned)((lanes + 127) / 128), 128, 0, c->stream>>>(throttle_view(c), M, R, G, eval_flags, c->d_chk_pre.as<unsigned char>());
     KT_CUDA(c, cudaGetLastError());
   }
-  unsigned char* ob = c->d_chk_out.as<unsigned char>();
+  unsigned char* ob = c->d_call_out.as<unsigned char>();
   RowsArgs a{};
   a.pods = pod_view(pend);
   a.tb = table_view(c);
   a.L = c->lim.label_slots; a.R = R; a.k = k;
-  a.rows = c->d_chk_rows.as<int64_t>();
+  a.rows = c->d_call_in.as<int64_t>();
   a.dev_of = dev_of(pend);
   a.pre = c->d_chk_pre.as<unsigned char>();
   a.admit = ob;
@@ -1680,12 +1689,12 @@ int kt_check_pending_rows(kt_ctx* c, uint32_t flags, int64_t k, const int64_t* r
   KT_CUDA(c, with_variant(c, true, [&](auto tpc, auto b, auto, auto reg) {
     return launch(c, k_check_rows<tpc, b, reg>, (unsigned)((k + kRowsTile - 1) / kRowsTile), kRowsTile, rows_smem_bytes(a.L, R, reg), false, a);
   }));
-  std::vector<unsigned char> hb(fetch);
-  KT_CUDA(c, cudaMemcpyAsync(hb.data(), ob, fetch, cudaMemcpyDeviceToHost, c->stream));
+  KT_CUDA(c, cudaMemcpyAsync(c->h_call.p, ob, fetch, cudaMemcpyDeviceToHost, c->stream));
   KT_CUDA(c, cudaStreamSynchronize(c->stream));
-  if (admit) std::memcpy(admit, hb.data(), (size_t)k);
-  if (codes) std::memcpy(codes, hb.data() + adm_bytes, code_bytes);
-  if (words) std::memcpy(words, hb.data() + adm_bytes + code_bytes, word_bytes);
+  const unsigned char* hb = c->h_call.as<unsigned char>();
+  if (admit) std::memcpy(admit, hb, (size_t)k);
+  if (codes) std::memcpy(codes, hb + adm_bytes, code_bytes);
+  if (words) std::memcpy(words, hb + adm_bytes + code_bytes, word_bytes);
   return KT_OK;
 }
 
@@ -1695,26 +1704,25 @@ int kt_match_pods(kt_ctx* c, int64_t k, const int64_t* labels, const int32_t* ns
   std::lock_guard<std::mutex> lk(c->mu);
   const int L = c->lim.label_slots;
   if (k > 0 && ((L > 0 && !labels) || !ns_id || !words)) return fail(c, KT_ERR_INVALID, "kt_match_pods: null pointer with k = %lld", (long long)k);
-  if (c->comm) return fail(c, KT_ERR_STATE, "kt_match_pods is single-GPU: this context has a communicator");
+  if (int rc = check_single_gpu(c, __func__)) return rc;
   if (!c->have_throttles) return fail(c, KT_ERR_STATE, "kt_match_pods before kt_upload_throttles");
   if (k == 0) return KT_OK;
   int rc = set_device(c);
   if (rc) return rc;
   const int Wp = c->ht.Wp;
   // the inputs in one copy: labels [L][k] | ns [k]
-  const size_t lab_bytes = (size_t)L * k * 8, in_bytes = lab_bytes + (size_t)k * 4;
-  std::vector<unsigned char> hin(in_bytes);
+  const size_t lab_bytes = (size_t)L * k * 8;
+  std::vector<unsigned char> hin(lab_bytes + (size_t)k * 4);
   if (lab_bytes) std::memcpy(hin.data(), labels, lab_bytes);
   std::memcpy(hin.data() + lab_bytes, ns_id, (size_t)k * 4);
-  KT_CUDA(c, c->d_mp_in.reserve(in_bytes + 16));
-  KT_CUDA(c, c->d_mp_out.reserve((size_t)k * Wp * 4 + 16));
-  KT_CUDA(c, cudaMemcpyAsync(c->d_mp_in.p, hin.data(), in_bytes, cudaMemcpyHostToDevice, c->stream));
+  if ((rc = upload_vec(c, c->d_call_in, hin))) return rc;
+  KT_CUDA(c, c->d_call_out.reserve((size_t)k * Wp * 4 + 16));
   MatchArgs a{};
   a.tb = table_view(c);
   a.L = L; a.k = k;
-  a.labels = c->d_mp_in.as<int64_t>();
-  a.ns = reinterpret_cast<const int32_t*>(c->d_mp_in.as<unsigned char>() + lab_bytes);
-  a.words = c->d_mp_out.as<uint32_t>();
+  a.labels = c->d_call_in.as<int64_t>();
+  a.ns = reinterpret_cast<const int32_t*>(c->d_call_in.as<unsigned char>() + lab_bytes);
+  a.words = c->d_call_out.as<uint32_t>();
   KT_CUDA(c, with_variant(c, true, [&](auto tpc, auto b, auto, auto reg) {
     return launch(c, k_match_pods<tpc, b, reg>, (unsigned)((k + kRowsTile - 1) / kRowsTile), kRowsTile, match_smem_bytes(L, reg), false, a);
   }));
@@ -1729,30 +1737,32 @@ int kt_get_check_rows(kt_ctx* c, int64_t k, const int64_t* rows, uint32_t* codes
   if (!c->evaluated) return fail(c, KT_ERR_STATE, "kt_get_check_rows before kt_evaluate");
   if (k == 0) return KT_OK;
   PodStore& s = c->pods[KT_PODS_PENDING];
-  for (int64_t i = 0; i < k; ++i)
-    if (rows[i] < 0 || rows[i] >= s.n) return fail(c, KT_ERR_INVALID, "row %lld out of range [0,%lld)", (long long)rows[i], (long long)s.n);
-  int rc = set_device(c);
-  if (rc) return rc;
-  if ((rc = check_pass_error(c))) return rc;
+  if (int rc = check_rows(c, __func__, k, rows, s.n)) return rc;
+  if (int rc = device_ready(c)) return rc;
   const int Wc = 2 * c->ht.Wp;
-  KT_CUDA(c, s.t_rows.reserve((size_t)k * 8));
-  KT_CUDA(c, s.t_words.reserve((size_t)k * Wc * 4 + (size_t)k + 64));
-  KT_CUDA(c, cudaMemcpyAsync(s.t_rows.p, rows, (size_t)k * 8, cudaMemcpyHostToDevice, c->stream));
-  if (s.clustered) k_order_map_rows<<<(unsigned)((k + 255) / 256), 256, 0, c->stream>>>(k, s.o_dev.as<uint32_t>(), s.t_rows.as<int64_t>());
-  unsigned char* adm = s.t_words.as<unsigned char>() + (size_t)k * Wc * 4;
-  k_gather_rows<<<(unsigned)((k + 7) / 8), 256, 0, c->stream>>>(k, s.t_rows.as<int64_t>(), Wc, c->d_codes.as<uint32_t>(), s.t_words.as<uint32_t>());
-  k_gather_bytes<<<(unsigned)((k + 255) / 256), 256, 0, c->stream>>>(k, s.t_rows.as<int64_t>(), c->d_admit.as<unsigned char>(), adm);
+  // the output block: admit[k] (padded to 16 B) | codes[k][Wc] -- one copy fetches the prefix the caller asked for
+  const size_t adm_bytes = ((size_t)k + 15) & ~(size_t)15, code_bytes = (size_t)k * Wc * 4;
+  const size_t fetch = codes ? adm_bytes + code_bytes : adm_bytes;
+  if (int rc = stage_rows(c, s, c->d_call_in, k, rows)) return rc;
+  KT_CUDA(c, c->d_call_out.reserve(adm_bytes + code_bytes + 16));
+  KT_CUDA(c, c->h_call.reserve(fetch));
+  const int64_t* d_rows = c->d_call_in.as<int64_t>();
+  unsigned char* ob = c->d_call_out.as<unsigned char>();
+  k_gather_bytes<<<(unsigned)((k + 255) / 256), 256, 0, c->stream>>>(k, d_rows, c->d_admit.as<unsigned char>(), ob);
+  k_gather_rows<<<(unsigned)((k + 7) / 8), 256, 0, c->stream>>>(k, d_rows, Wc, c->d_codes.as<uint32_t>(), reinterpret_cast<uint32_t*>(ob + adm_bytes));
   KT_CUDA(c, cudaGetLastError());
-  if (codes) KT_CUDA(c, cudaMemcpyAsync(codes, s.t_words.p, (size_t)k * Wc * 4, cudaMemcpyDeviceToHost, c->stream));
-  if (admit) KT_CUDA(c, cudaMemcpyAsync(admit, adm, (size_t)k, cudaMemcpyDeviceToHost, c->stream));
+  KT_CUDA(c, cudaMemcpyAsync(c->h_call.p, ob, fetch, cudaMemcpyDeviceToHost, c->stream));
   KT_CUDA(c, cudaStreamSynchronize(c->stream));
+  const unsigned char* hb = c->h_call.as<unsigned char>();
+  if (admit) std::memcpy(admit, hb, (size_t)k);
+  if (codes) std::memcpy(codes, hb + adm_bytes, code_bytes);
   return KT_OK;
 }
 
 int kt_get_match_bitmap(kt_ctx* c, int kind, uint32_t* words) {
   if (!c || !words) return KT_ERR_INVALID;
   std::lock_guard<std::mutex> lk(c->mu);
-  if (kind != KT_PODS_RUNNING && kind != KT_PODS_PENDING) return fail(c, KT_ERR_INVALID, "bad pod kind %d", kind);
+  if (int rc = check_kind(c, __func__, kind)) return rc;
   if (!c->evaluated) return fail(c, KT_ERR_STATE, "kt_get_match_bitmap before kt_evaluate");
   int rc = set_device(c);
   if (rc) return rc;
@@ -1770,22 +1780,19 @@ int kt_get_match_bitmap(kt_ctx* c, int kind, uint32_t* words) {
 int kt_get_match_rows(kt_ctx* c, int kind, int64_t k, const int64_t* rows, uint32_t* words) {
   if (!c || k < 0 || (k > 0 && (!rows || !words))) return KT_ERR_INVALID;
   std::lock_guard<std::mutex> lk(c->mu);
-  if (kind != KT_PODS_RUNNING && kind != KT_PODS_PENDING) return fail(c, KT_ERR_INVALID, "bad pod kind %d", kind);
+  if (int rc = check_kind(c, __func__, kind)) return rc;
   if (!c->evaluated) return fail(c, KT_ERR_STATE, "kt_get_match_rows before kt_evaluate");
   if (k == 0) return KT_OK;
   PodStore& s = c->pods[kind];
-  for (int64_t i = 0; i < k; ++i)
-    if (rows[i] < 0 || rows[i] >= s.n) return fail(c, KT_ERR_INVALID, "row %lld out of range [0,%lld)", (long long)rows[i], (long long)s.n);
+  if (int rc = check_rows(c, __func__, k, rows, s.n)) return rc;
   int rc = set_device(c);
   if (rc) return rc;
   const int Wp = c->ht.Wp;
-  KT_CUDA(c, s.t_rows.reserve((size_t)k * 8));
-  KT_CUDA(c, s.t_words.reserve((size_t)k * Wp * 4));
-  KT_CUDA(c, cudaMemcpyAsync(s.t_rows.p, rows, (size_t)k * 8, cudaMemcpyHostToDevice, c->stream));
-  if (s.clustered) k_order_map_rows<<<(unsigned)((k + 255) / 256), 256, 0, c->stream>>>(k, s.o_dev.as<uint32_t>(), s.t_rows.as<int64_t>());
-  k_gather_rows<<<(unsigned)((k + 7) / 8), 256, 0, c->stream>>>(k, s.t_rows.as<int64_t>(), Wp, s.bitmap.as<uint32_t>(), s.t_words.as<uint32_t>());
+  if ((rc = stage_rows(c, s, c->d_call_in, k, rows))) return rc;
+  KT_CUDA(c, c->d_call_out.reserve((size_t)k * Wp * 4 + 16));
+  k_gather_rows<<<(unsigned)((k + 7) / 8), 256, 0, c->stream>>>(k, c->d_call_in.as<int64_t>(), Wp, s.bitmap.as<uint32_t>(), c->d_call_out.as<uint32_t>());
   KT_CUDA(c, cudaGetLastError());
-  KT_CUDA(c, cudaMemcpyAsync(words, s.t_words.p, (size_t)k * Wp * 4, cudaMemcpyDeviceToHost, c->stream));
+  KT_CUDA(c, cudaMemcpyAsync(words, c->d_call_out.p, (size_t)k * Wp * 4, cudaMemcpyDeviceToHost, c->stream));
   KT_CUDA(c, cudaStreamSynchronize(c->stream));
   return KT_OK;
 }
@@ -1793,14 +1800,12 @@ int kt_get_match_rows(kt_ctx* c, int kind, int64_t k, const int64_t* rows, uint3
 int kt_get_match_columns(kt_ctx* c, int kind, int64_t k, const int32_t* idx, int64_t* off, int64_t* rows, uint8_t* codes, int64_t cap) {
   if (!c || k < 0 || cap < 0 || !off || (k > 0 && !idx) || (cap > 0 && !rows)) return KT_ERR_INVALID;
   std::lock_guard<std::mutex> lk(c->mu);
-  if (kind != KT_PODS_RUNNING && kind != KT_PODS_PENDING) return fail(c, KT_ERR_INVALID, "bad pod kind %d", kind);
+  if (int rc = check_kind(c, __func__, kind)) return rc;
   if (kind == KT_PODS_RUNNING && codes) return fail(c, KT_ERR_INVALID, "kt_get_match_columns: codes belong to the pending rows");
   if (!c->evaluated) return fail(c, KT_ERR_STATE, "kt_get_match_columns before kt_evaluate");
-  for (int64_t j = 0; j < k; ++j)
-    if (idx[j] < 0 || idx[j] >= c->M) return fail(c, KT_ERR_INVALID, "throttle %d out of range [0,%d)", idx[j], c->M);
-  int rc = set_device(c);
+  if (int rc = check_throttles(c, __func__, k, idx)) return rc;
+  int rc = device_ready(c);
   if (rc) return rc;
-  if ((rc = check_pass_error(c))) return rc;
   off[0] = 0;
   if (k == 0) return KT_OK;
   PodStore& s = c->pods[kind];
@@ -1823,11 +1828,10 @@ int kt_get_match_columns(kt_ctx* c, int kind, int64_t k, const int32_t* idx, int
 int kt_reconcile_throttles(kt_ctx* c, int64_t now, int64_t k, const int32_t* idx, const kt_reconcile_out* o, int64_t* off, int64_t* rows, int64_t cap) {
   if (!c || !o || !off || k < 0 || cap < 0 || (k > 0 && !idx) || (cap > 0 && !rows)) return KT_ERR_INVALID;
   std::lock_guard<std::mutex> lk(c->mu);
-  if (c->comm) return fail(c, KT_ERR_STATE, "kt_reconcile_throttles is single-GPU: this context has a communicator");
+  if (int rc = check_single_gpu(c, __func__)) return rc;
   if (!c->have_throttles) return fail(c, KT_ERR_STATE, "kt_reconcile_throttles before kt_upload_throttles");
+  if (int rc = check_throttles(c, __func__, k, idx)) return rc;
   const int M = c->M, R = c->lim.n_resources;
-  for (int64_t e = 0; e < k; ++e)
-    if (idx[e] < 0 || idx[e] >= M) return fail(c, KT_ERR_INVALID, "throttle %d out of range [0,%d)", idx[e], M);
   off[0] = 0;
   if (k == 0) return KT_OK;
   int rc = set_device(c);
@@ -1853,10 +1857,9 @@ int kt_reconcile_throttles(kt_ctx* c, int64_t now, int64_t k, const int32_t* idx
   for (uint32_t m : masks) list.push_back((int32_t)m);
   list.insert(list.end(), idx, idx + k);
   list.insert(list.end(), cidx.begin(), cidx.end());
-  KT_CUDA(c, c->d_key_list.reserve(list.size() * 4 + 16));
-  KT_CUDA(c, cudaMemcpyAsync(c->d_key_list.p, list.data(), list.size() * 4, cudaMemcpyHostToDevice, c->stream));
-  const int32_t* d_words = c->d_key_list.as<int32_t>();
-  const uint32_t* d_masks = c->d_key_list.as<uint32_t>() + nw;
+  if ((rc = upload_vec(c, c->d_call_in, list))) return rc;
+  const int32_t* d_words = c->d_call_in.as<int32_t>();
+  const uint32_t* d_masks = c->d_call_in.as<uint32_t>() + nw;
   const int32_t* d_idx = d_words + 2 * nw;
   const int32_t* d_cidx = d_idx + k;
   KT_CUDA(c, c->d_key_reach.reserve((size_t)NS * NC * 4 + 16));
@@ -1885,33 +1888,21 @@ int kt_reconcile_throttles(kt_ctx* c, int64_t now, int64_t k, const int32_t* idx
       return launch(c, k_keyed_rows<tpc, b, rt, reg>, grid, kKeyedTile, smem, false, a);
     }));
   }
-  // the status of the k columns, shaped as kt_get_reconcile_rows delivers it
-  ThrottleView tv{};
-  tv.flags = c->d_tflags.as<uint8_t>();
-  tv.thr = c->d_thr.as<int64_t>(); tv.thr_present = c->d_thr_present.as<uint32_t>(); tv.thr_cnt = c->d_thr_cnt.as<int64_t>();
-  tv.ovr_off = c->d_ovr_off.as<int32_t>(); tv.ovr_begin = c->d_ovr_begin.as<int64_t>(); tv.ovr_end = c->d_ovr_end.as<int64_t>();
-  tv.ovr_flags = c->d_ovr_flags.as<uint8_t>(); tv.ovr_thr = c->d_ovr_thr.as<int64_t>(); tv.ovr_present = c->d_ovr_present.as<uint32_t>();
-  tv.ovr_cnt = c->d_ovr_cnt.as<int64_t>(); tv.n_ovr = c->n_ovr;
-  const size_t bytes = (size_t)k * ((size_t)2 * R * 8 + 16 + 12 + 1);
-  KT_CUDA(c, c->d_key_out.reserve(bytes + 16));
-  k_keyed_status<<<(unsigned)((k + 127) / 128), 128, 0, c->stream>>>(k, d_idx, d_cidx, R, M, NJ, tv, (long long)now, a.used, a.cnt, a.pres,
-                                                                   c->d_key_out.as<unsigned char>());
+  // the status of the k columns: a status block of k columns, as kt_get_reconcile_rows gathers it
+  const size_t bytes = status_layout(R, k).bytes;
+  KT_CUDA(c, c->d_call_out.reserve(bytes));
+  KT_CUDA(c, c->h_call.reserve(bytes));
+  k_keyed_status<<<(unsigned)((k + 127) / 128), 128, 0, c->stream>>>(k, d_idx, d_cidx, R, M, NJ, throttle_view(c), (long long)now, a.used, a.cnt, a.pres,
+                                                                   status_at<ReconcileView>(c->d_call_out.p, R, k));
   KT_CUDA(c, cudaGetLastError());
-  std::vector<unsigned char> hb(bytes);
-  KT_CUDA(c, cudaMemcpyAsync(hb.data(), c->d_key_out.p, bytes, cudaMemcpyDeviceToHost, c->stream));
+  KT_CUDA(c, cudaMemcpyAsync(c->h_call.p, c->d_call_out.p, bytes, cudaMemcpyDeviceToHost, c->stream));
   // the matched rows: the scratch transposed (ColumnView over the compact words)
   ColumnView v{};
   v.bitmap = a.scratch; v.Wp = nw; v.first = 0; v.count = (int64_t)n; v.idx = d_cidx; v.k = k;
   v.rowmap = dev_of(run);  // the scratch is indexed by device row; the lists come out in caller rows
   int64_t total = 0;
-  if ((rc = build_columns(c, v, &total, off, cap))) return rc;  // (synchronises the stream: hb has landed)
-  size_t at = 0;
-  auto take = [&](void* dst, size_t sz) {
-    if (dst) std::memcpy(dst, hb.data() + at, sz);
-    at += sz;
-  };
-  take(o->used, (size_t)R * k * 8); take(o->calc_thr, (size_t)R * k * 8); take(o->used_cnt, (size_t)k * 8); take(o->calc_cnt, (size_t)k * 8);
-  take(o->used_present, (size_t)k * 4); take(o->throttled, (size_t)k * 4); take(o->calc_present, (size_t)k * 4); take(o->override_active, (size_t)k);
+  if ((rc = build_columns(c, v, &total, off, cap))) return rc;  // (synchronises the stream: the status block has landed)
+  copy_status(status_at<kt_reconcile_out>(c->h_call.p, R, k), o, R, k);
   if (total > cap || total == 0) return KT_OK;  // off[] says how much room the rows need
   KT_CUDA(c, cudaMemcpyAsync(rows, v.rows, (size_t)total * 8, cudaMemcpyDeviceToHost, c->stream));
   KT_CUDA(c, cudaStreamSynchronize(c->stream));
@@ -1922,9 +1913,8 @@ int kt_get_check(kt_ctx* c, uint32_t* codes, uint8_t* admit) {
   if (!c) return KT_ERR_INVALID;
   std::lock_guard<std::mutex> lk(c->mu);
   if (!c->evaluated) return fail(c, KT_ERR_STATE, "kt_get_check before kt_evaluate");
-  int rc = set_device(c);
+  int rc = device_ready(c);
   if (rc) return rc;
-  if ((rc = check_pass_error(c))) return rc;
   PodStore& pend = c->pods[KT_PODS_PENDING];
   const int64_t P = pend.n;
   const size_t code_bytes = (size_t)P * 2 * c->ht.Wp * 4;
@@ -1950,28 +1940,26 @@ int kt_get_check_summary(kt_ctx* c, int64_t first, int64_t count, const uint8_t*
   PodStore& pend = c->pods[KT_PODS_PENDING];
   if (first < 0 || count < 0 || first > pend.n - count)
     return fail(c, KT_ERR_INVALID, "rows [%lld, %lld + %lld) outside the pending table (%lld rows)", (long long)first, (long long)first, (long long)count, (long long)pend.n);
-  if (c->comm) return fail(c, KT_ERR_STATE, "kt_get_check_summary is single-GPU: this context has a communicator");
+  if (int rc = check_single_gpu(c, __func__)) return rc;
   if (!c->evaluated || !c->have_codes) return fail(c, KT_ERR_STATE, "kt_get_check_summary before a pass wrote the pending codes");
-  int rc = set_device(c);
+  int rc = device_ready(c);
   if (rc) return rc;
-  if ((rc = check_pass_error(c))) return rc;
   const int M = c->M, R = c->lim.n_resources;
-  // one block: row classes [count] (padded to 16 B) | status_cnt [3][M] | sole_cnt [M] | held [R][M] | held_present [M]
-  const size_t cls_bytes = row_class ? ((size_t)count + 15) & ~(size_t)15 : 0;
+  // one output block: status_cnt [3][M] | sole_cnt [M] | held [R][M] | held_present [M]; all zero when there is nothing to summarise
   const size_t u64s = (size_t)(4 + R) * M, out_bytes = u64s * 8 + (size_t)M * 4;
-  std::vector<unsigned char> hb(out_bytes + 1);
+  KT_CUDA(c, c->h_call.reserve(out_bytes + 16));
+  unsigned char* h = c->h_call.as<unsigned char>();
   if (count > 0 && M > 0) {
-    KT_CUDA(c, c->d_sum.reserve(cls_bytes + out_bytes + 16));
-    unsigned char* base = c->d_sum.as<unsigned char>();
-    unsigned char* ob = base + cls_bytes;
-    if (row_class) KT_CUDA(c, cudaMemcpyAsync(base, row_class, (size_t)count, cudaMemcpyHostToDevice, c->stream));
+    if (row_class && (rc = upload(c, c->d_call_in, row_class, (size_t)count))) return rc;
+    KT_CUDA(c, c->d_call_out.reserve(out_bytes + 16));
+    unsigned char* ob = c->d_call_out.as<unsigned char>();
     KT_CUDA(c, cudaMemsetAsync(ob, 0, out_bytes, c->stream));
     SummaryArgs a{};
     a.first = first; a.count = count; a.n = pend.n; a.Wc = 2 * c->ht.Wp; a.R = R; a.M = M;
     a.codes = c->d_codes.as<uint32_t>(); a.admit = c->d_admit.as<unsigned char>();
     a.req = pend.req.as<int64_t>(); a.present = pend.present.as<uint32_t>();
     a.caller_of = pend.clustered ? pend.o_caller.as<uint32_t>() : nullptr;
-    a.row_class = row_class ? base : nullptr;
+    a.row_class = row_class ? c->d_call_in.as<unsigned char>() : nullptr;
     unsigned long long* u = reinterpret_cast<unsigned long long*>(ob);
     a.status_cnt = o->status_cnt ? u : nullptr;
     a.sole_cnt = o->sole_cnt ? u + (size_t)3 * M : nullptr;
@@ -1981,10 +1969,11 @@ int kt_get_check_summary(kt_ctx* c, int64_t first, int64_t count, const uint8_t*
     const int64_t blocks = std::min<int64_t>((rows + kSummaryThreads - 1) / kSummaryThreads, (int64_t)c->sm_count * 8);
     k_check_summary<<<(unsigned)std::max<int64_t>(blocks, 1), kSummaryThreads, 0, c->stream>>>(a);
     KT_CUDA(c, cudaGetLastError());
-    KT_CUDA(c, cudaMemcpyAsync(hb.data(), ob, out_bytes, cudaMemcpyDeviceToHost, c->stream));
+    KT_CUDA(c, cudaMemcpyAsync(h, ob, out_bytes, cudaMemcpyDeviceToHost, c->stream));
     KT_CUDA(c, cudaStreamSynchronize(c->stream));
+  } else {
+    std::memset(h, 0, out_bytes);
   }
-  const unsigned char* h = hb.data();
   if (o->status_cnt) std::memcpy(o->status_cnt, h, (size_t)3 * M * 8);
   if (o->sole_cnt) std::memcpy(o->sole_cnt, h + (size_t)3 * M * 8, (size_t)M * 8);
   if (o->held) std::memcpy(o->held, h + (size_t)4 * M * 8, (size_t)R * M * 8);
@@ -2013,9 +2002,8 @@ int kt_get_check_sparse(kt_ctx* c, uint8_t* admit, uint32_t* entries, int64_t ca
   std::lock_guard<std::mutex> lk(c->mu);
   if (!c->evaluated) return fail(c, KT_ERR_STATE, "kt_get_check_sparse before kt_evaluate");
   if (!c->sparse_cap) return fail(c, KT_ERR_STATE, "kt_get_check_sparse without kt_set_sparse_check");
-  int rc = set_device(c);
+  int rc = device_ready(c);
   if (rc) return rc;
-  if ((rc = check_pass_error(c))) return rc;
   const int64_t P = c->pods[KT_PODS_PENDING].n;
   const int64_t room = cap < (int64_t)c->sparse_cap ? cap : (int64_t)c->sparse_cap;
   // one round trip in the common case: the count and as many entries as the last pass produced (plus slack) together
@@ -2089,7 +2077,7 @@ int kt_debug_get_pass_plan(kt_ctx* c, kt_pass_plan* last) {
 int kt_debug_set_row_order(kt_ctx* c, int kind, int mode) {
   if (!c) return KT_ERR_INVALID;
   std::lock_guard<std::mutex> lk(c->mu);
-  if (kind != KT_PODS_RUNNING && kind != KT_PODS_PENDING) return fail(c, KT_ERR_INVALID, "bad pod kind %d", kind);
+  if (int rc = check_kind(c, __func__, kind)) return rc;
   if (mode < KT_ROW_ORDER_AUTO || mode > KT_ROW_ORDER_BY_NAMESPACE) return fail(c, KT_ERR_INVALID, "row order %d: expected 0, 1 or 2", mode);
   c->pods[kind].order_mode = mode;
   return KT_OK;
@@ -2098,7 +2086,7 @@ int kt_debug_set_row_order(kt_ctx* c, int kind, int mode) {
 int kt_debug_get_row_order(kt_ctx* c, int kind, int64_t* dev_row, int32_t* clustered) {
   if (!c) return KT_ERR_INVALID;
   std::lock_guard<std::mutex> lk(c->mu);
-  if (kind != KT_PODS_RUNNING && kind != KT_PODS_PENDING) return fail(c, KT_ERR_INVALID, "bad pod kind %d", kind);
+  if (int rc = check_kind(c, __func__, kind)) return rc;
   const PodStore& s = c->pods[kind];
   if (clustered) *clustered = s.clustered ? 1 : 0;
   if (!dev_row || s.n == 0) return KT_OK;

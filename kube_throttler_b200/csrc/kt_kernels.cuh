@@ -2068,32 +2068,23 @@ __global__ void __launch_bounds__(256) k_unpack_rows(int64_t n, int L, int Lpad,
   flags[p] = m >> 29;
 }
 
-// Status columns of k listed throttles -> one packed block {used[R][k], calc_thr[R][k], used_cnt[k], calc_cnt[k],
-// used_present[k], throttled[k], calc_present[k], override_active[k]} (kt_get_reconcile_rows: the download is proportional
-// to what changed, not to M).
+// Status columns of k listed throttles: column idx[i] of the pass's M columns (src) -> column i of k (dst), so that
+// kt_get_reconcile_rows downloads in proportion to what changed, not to M.
 __global__ void __launch_bounds__(128) k_gather_status(int64_t k, const int32_t* __restrict__ idx, int R, int M, const ReconcileView src,
-                                                       unsigned char* __restrict__ out) {
+                                                       const ReconcileView dst) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= k) return;
   const int t = idx[i];
-  long long* used = reinterpret_cast<long long*>(out);
-  long long* calc = used + (size_t)R * k;
-  long long* used_cnt = calc + (size_t)R * k;
-  long long* calc_cnt = used_cnt + k;
-  uint32_t* used_present = reinterpret_cast<uint32_t*>(calc_cnt + k);
-  uint32_t* throttled = used_present + k;
-  uint32_t* calc_present = throttled + k;
-  unsigned char* ovr = reinterpret_cast<unsigned char*>(calc_present + k);
   for (int r = 0; r < R; ++r) {
-    used[(size_t)r * k + i] = src.used[(size_t)r * M + t];
-    calc[(size_t)r * k + i] = src.calc_thr[(size_t)r * M + t];
+    dst.used[(size_t)r * k + i] = src.used[(size_t)r * M + t];
+    dst.calc_thr[(size_t)r * k + i] = src.calc_thr[(size_t)r * M + t];
   }
-  used_cnt[i] = src.used_cnt[t];
-  calc_cnt[i] = src.calc_cnt[t];
-  used_present[i] = src.used_present[t];
-  throttled[i] = src.throttled[t];
-  calc_present[i] = src.calc_present[t];
-  ovr[i] = src.override_active[t];
+  dst.used_cnt[i] = src.used_cnt[t];
+  dst.calc_cnt[i] = src.calc_cnt[t];
+  dst.used_present[i] = src.used_present[t];
+  dst.throttled[i] = src.throttled[t];
+  dst.calc_present[i] = src.calc_present[t];
+  dst.override_active[i] = src.override_active[t];
 }
 __global__ void __launch_bounds__(256) k_gather_bytes(int64_t k, const int64_t* __restrict__ rows, const unsigned char* __restrict__ src, unsigned char* __restrict__ out) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;

@@ -172,22 +172,13 @@ __global__ void __launch_bounds__(kKeyedTile) k_keyed_rows(const KeyedArgs a) {
 }
 
 // Status of listed entry e (throttle idx[e], compact accumulator cidx[e]): what a FRESH_STATUS pass reports for that column,
-// written into one packed block shaped as kt_get_reconcile_rows delivers it:
-//   {used[R][k], calc_thr[R][k], used_cnt[k], calc_cnt[k], used_present[k], throttled[k], calc_present[k], override_active[k]}
+// written into column e of the k columns of `out`, as kt_get_reconcile_rows gathers them from the pass's.
 __global__ void __launch_bounds__(128) k_keyed_status(int64_t k, const int32_t* __restrict__ idx, const int32_t* __restrict__ cidx, int R, int M, int NJ,
                                                       const ThrottleView tv, long long now, const unsigned long long* __restrict__ used,
-                                                      const unsigned long long* __restrict__ cnt, const uint32_t* __restrict__ pres, unsigned char* __restrict__ out) {
+                                                      const unsigned long long* __restrict__ cnt, const uint32_t* __restrict__ pres, const ReconcileView out) {
   const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= k) return;
   const int t = idx[e], cj = cidx[e];
-  int64_t* o_used = reinterpret_cast<int64_t*>(out);
-  int64_t* o_calc = o_used + (size_t)R * k;
-  int64_t* o_used_cnt = o_calc + (size_t)R * k;
-  int64_t* o_calc_cnt = o_used_cnt + k;
-  uint32_t* o_used_present = reinterpret_cast<uint32_t*>(o_calc_cnt + k);
-  uint32_t* o_throttled = o_used_present + k;
-  uint32_t* o_calc_present = o_throttled + k;
-  uint8_t* o_active = reinterpret_cast<uint8_t*>(o_calc_present + k);
   const uint32_t tflags = tv.flags[t];
   const bool live = (tflags & KT_THR_RESPONSIBLE) && !(tflags & KT_THR_SELECTOR_ERROR);
   const uint32_t p = pres[cj];
@@ -206,17 +197,17 @@ __global__ void __launch_bounds__(128) k_keyed_status(int64_t k, const int32_t* 
     if (ct.calc_has) m_calc |= mybit;
     active = ct.active;
     if (is_res) {
-      o_used[(size_t)r * k + e] = used_val;
-      o_calc[(size_t)r * k + e] = ct.calc_val;
+      out.used[(size_t)r * k + e] = used_val;
+      out.calc_thr[(size_t)r * k + e] = ct.calc_val;
     } else {
-      o_used_cnt[e] = used_val;
-      o_calc_cnt[e] = ct.calc_val;
+      out.used_cnt[e] = used_val;
+      out.calc_cnt[e] = ct.calc_val;
     }
   }
-  o_used_present[e] = m_used;
-  o_throttled[e] = m_thr;
-  o_calc_present[e] = m_calc;
-  o_active[e] = active;
+  out.used_present[e] = m_used;
+  out.throttled[e] = m_thr;
+  out.calc_present[e] = m_calc;
+  out.override_active[e] = active;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -230,7 +221,7 @@ __global__ void __launch_bounds__(128) k_keyed_status(int64_t k, const int32_t* 
 //   2. k_check_rows  one lane per listed row (listed rows share no namespace locality): its row offsets, the words of its
 //                    namespace's list with the pass's eval_word, and each non-zero word decided pair by pair from the
 //                    pre-records (decide_word_direct_codes; in GIVEN_STATUS mode it reads no sums).
-// Outputs go to the call's own block [k][Wp] words | [k][2 Wp] codes | [k] admit, zeroed before the launch, so that every word
+// Outputs go to the call's own block [k] admit | [k][2 Wp] codes | [k][Wp] words, zeroed before the launch, so that every word
 // outside the row's namespace list reads 0 as in the pass's maintained rows.
 // ------------------------------------------------------------------------------------------------
 struct NoSync {  // finalize_tile's prep half signals nobody: the rows kernel is the next launch in the stream
