@@ -189,7 +189,13 @@ const char* kt_last_error(const kt_ctx* ctx); /* valid until the next call on ct
 const char* kt_version(void);
 /* Run on a caller-owned CUDA stream (cudaStream_t as void*); NULL restores the private stream.  A switch keeps queued work
  * ordered: everything queued on the old stream before the switch (async uploads, passes) runs before anything the context
- * queues on the new one, and kt_sync, which waits on the new stream, also covers the work queued before the switch. */
+ * queues on the new one, and kt_sync, which waits on the new stream, also covers the work queued before the switch.
+ * A whole pass queued right behind another whole pass of this library on the same stream (of any context; of the same one
+ * unless either pass zero-fills after new rows or tables) starts its match and reconcile tiles while the pass ahead still
+ * decides.  Copies, plain kernels and uploads queued between two passes are waited for in full as before.  A caller's own
+ * kernel launched with programmatic stream serialization right behind a pass may start before that pass has finished (as
+ * before: the pass lets its successor start early); it must wait for it (cudaGridDependencySynchronize) before reading or
+ * writing anything the pass touches. */
 int kt_set_stream(kt_ctx* ctx, void* cuda_stream);
 int kt_sync(kt_ctx* ctx);
 /* Record CUDA events around each kernel of kt_evaluate so kt_get_timing reports device times. */

@@ -162,7 +162,8 @@ struct kt_ctx {
   DevBuf d_part;   // 2 x [2R+1][M] u64 by pass parity: a reconciling pass adds into one half and leaves the other zeroed for its successor
   size_t part_stride = 0;  // bytes between the two halves
   unsigned part_parity = 0;  // half that holds the sums of the last reconcile
-  DevBuf d_sync;   // PassSync counters of the fused pass (zero between launches)
+  DevBuf d_sync;   // 2 x PassSync counters of the fused pass by pass_parity (zero between launches)
+  unsigned pass_parity = 0;  // set of counters and half of d_pre the last fused pass used; the next one takes the other
   DevBuf d_trace;  // optional trace rows of the fused pass, one per match / reconcile / status tile
   bool trace = false;
   uint32_t trace_roles[4] = {0, 0, 0, 0};  // match tiles, reconcile tiles, status tiles, CTAs launched
@@ -183,7 +184,8 @@ struct kt_ctx {
   // no call reads what another left there.
   DevBuf d_call_in, d_call_out;
   PinnedBuf h_call;
-  DevBuf d_pre;    // [M] pre-records, finalize tiles -> decide tiles (kt_kernels.cuh pre_record_bytes)
+  DevBuf d_pre;    // 2 x [M] pre-records by pass_parity, finalize tiles -> decide tiles (kt_kernels.cuh pre_record_bytes)
+  size_t pre_stride = 0;  // bytes between the two halves
   DevBuf d_out;    // the reconcile half's per-throttle outputs: ONE status block of M columns (status_layout)
   bool async_uploads = false;  // kt_set_async_uploads
   cudaEvent_t ev_switch = nullptr;  // kt_set_stream: the new stream waits for what was queued on the old one
@@ -243,7 +245,32 @@ int upload(kt_ctx* c, DevBuf& b, const T* src, size_t count) {
 template <class T>
 int upload_vec(kt_ctx* c, DevBuf& b, const std::vector<T>& v) { return upload(c, b, v.data(), v.size()); }
 
+// The library's last launch on each stream, while that launch is a fused k_pass: evaluate_locked lets the next fused pass start
+// its first phase early only behind one (k_pass).  Every other library call that queues work on a stream forgets the stream's
+// entry -- set_device at the top of the entry points, launch(), kt_set_stream, kt_destroy -- so the record never names a pass
+// that something of the library's was queued behind.
+struct LastPass {
+  const kt_ctx* ctx = nullptr;  // nullptr: the last launch was not a fused pass
+  bool zero_fill = false;       // that pass zero-filled bitmap or code rows
+};
+std::mutex g_last_pass_mu;
+std::map<cudaStream_t, LastPass> g_last_pass;
+LastPass last_pass_on(cudaStream_t s) {
+  std::lock_guard<std::mutex> lk(g_last_pass_mu);
+  auto it = g_last_pass.find(s);
+  return it == g_last_pass.end() ? LastPass{} : it->second;
+}
+void note_pass(cudaStream_t s, const kt_ctx* c, bool zero_fill) {
+  std::lock_guard<std::mutex> lk(g_last_pass_mu);
+  g_last_pass[s] = LastPass{c, zero_fill};
+}
+void forget_pass(cudaStream_t s) {
+  std::lock_guard<std::mutex> lk(g_last_pass_mu);
+  g_last_pass.erase(s);
+}
+
 int set_device(kt_ctx* c) {
+  forget_pass(c->stream);
   KT_CUDA(c, cudaSetDevice(c->device));
   return KT_OK;
 }
@@ -394,10 +421,12 @@ PartExchange local_exchange(const kt_ctx* c) {
   PartExchange px{};
   px.mine = px.total = reinterpret_cast<unsigned long long*>(c->d_part.as<unsigned char>() + (size_t)c->part_parity * c->part_stride);
   px.zero_mine = reinterpret_cast<unsigned long long*>(c->d_part.as<unsigned char>() + (size_t)(c->part_parity ^ 1u) * c->part_stride);
-  px.sync = c->d_sync.as<PassSync>();
+  px.sync = c->d_sync.as<PassSync>() + c->pass_parity;
   px.rank = c->rank;
   return px;
 }
+// The pre-records of the last pass (a fused pass switches halves first: see pass_parity)
+unsigned char* pre_records(const kt_ctx* c) { return c->d_pre.as<unsigned char>() + (size_t)c->pass_parity * c->pre_stride; }
 
 PodView pod_view(const PodStore& s) {
   PodView v;
@@ -561,6 +590,7 @@ int admit_in_caller_order(kt_ctx* c, const unsigned char** out, size_t at = 0) {
 int sparse_to_caller(kt_ctx* c) {
   const PodStore& pend = c->pods[KT_PODS_PENDING];
   if (!c->sparse_cap || !pend.clustered || pend.n == 0) return KT_OK;
+  forget_pass(c->stream);
   k_order_sparse_rows<<<(unsigned)c->sm_count * 2, 256, 0, c->stream>>>(c->d_sparse.as<uint32_t>(), c->sparse_cap, c->d_sparse.as<uint32_t>() + 4,
                                                                        pend.o_caller.as<uint32_t>());
   KT_CUDA(c, cudaGetLastError());
@@ -661,11 +691,12 @@ int ensure_window(kt_ctx* c, size_t part_bytes) {
 // stream serialization attribute (PDL): the secondary grid may start while the primary still runs and
 // synchronises on it with griddepcontrol.wait where it first needs the primary's results.
 // The rule: a kernel launched with PDL either waits at its top (k_pass), or its primary -- the kernel right
-// before it in the stream -- was launched by the same call.  Its primary is otherwise whatever the caller
-// queued last (another pass of this context, another context's pass on a shared stream), and the writes it
-// makes before its wait would race with that work.
+// before it in the stream -- was launched by the same call, or it is an early k_pass whose primary is a k_pass
+// (evaluate_locked: g_last_pass).  Its primary is otherwise whatever the caller queued last (another pass of this
+// context, another context's pass on a shared stream), and the writes it makes before its wait would race with that work.
 template <class... KArgs, class... Args>
 cudaError_t launch(kt_ctx* c, void (*kern)(KArgs...), unsigned blocks, unsigned threads, size_t smem, bool pdl, Args... args) {
+  forget_pass(c->stream);
   cudaError_t e = cudaFuncSetAttribute((const void*)kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
   cudaLaunchConfig_t cfg{};
@@ -706,7 +737,7 @@ template <int TPC, int B, bool REG>
 cudaError_t launch_check(kt_ctx* c, const PodView& pv, const TableView& tb, const PartExchange& px, unsigned blocks, bool pdl) {
   const int L = c->lim.label_slots, R = c->lim.n_resources;
   return launch(c, k_check<TPC, B, REG>, blocks, kTileCheck, check_smem_bytes(L, R, REG, kTileCheck), pdl, pv, tb, L, R,
-                (const unsigned char*)c->d_pre.as<unsigned char>(), px, c->pods[KT_PODS_PENDING].bitmap.as<uint32_t>(),
+                (const unsigned char*)pre_records(c), px, c->pods[KT_PODS_PENDING].bitmap.as<uint32_t>(),
                 c->d_codes.as<uint32_t>(), c->d_admit.as<unsigned char>(), sparse_view(c));
 }
 // Occupancy of k_pass compiled for THREADS resident threads per SM: CTAs the device holds at once.
@@ -847,7 +878,7 @@ int kt_create(kt_ctx** out, int device, const kt_limits* lim) {
   for (auto& e : c->ev)
     if (cudaEventCreate(&e) != cudaSuccess) { delete c; return KT_ERR_CUDA; }
   if (cudaEventCreateWithFlags(&c->ev_switch, cudaEventDisableTiming) != cudaSuccess) { kt_destroy(c); return KT_ERR_CUDA; }
-  if (c->d_sync.reserve(sizeof(PassSync)) != cudaSuccess || cudaMemset(c->d_sync.p, 0, sizeof(PassSync)) != cudaSuccess) { kt_destroy(c); return KT_ERR_CUDA; }
+  if (c->d_sync.reserve(2 * sizeof(PassSync)) != cudaSuccess || cudaMemset(c->d_sync.p, 0, 2 * sizeof(PassSync)) != cudaSuccess) { kt_destroy(c); return KT_ERR_CUDA; }
   *out = c;
   return KT_OK;
 }
@@ -856,6 +887,7 @@ void kt_destroy(kt_ctx* c) {
   if (!c) return;
   cudaSetDevice(c->device);
   cudaStreamSynchronize(c->stream);
+  forget_pass(c->stream);
   release_window(c);
   if (c->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(c->comm);
   for (auto& s : c->pods) s.release();
@@ -890,6 +922,7 @@ int kt_set_stream(kt_ctx* c, void* cuda_stream) {
   // the new stream covers it
   KT_CUDA(c, cudaEventRecord(c->ev_switch, c->stream));
   KT_CUDA(c, cudaStreamWaitEvent(next, c->ev_switch, 0));
+  forget_pass(next);
   c->stream = next;
   return KT_OK;
 }
@@ -1199,7 +1232,8 @@ int kt_upload_throttles(kt_ctx* c, int32_t m, const kt_throttle_cols* cols, cons
   KT_CUDA(c, cudaMemsetAsync(c->d_part.p, 0, c->d_part.cap, c->stream));
   c->part_parity = 0;
   c->win_stale = c->win != nullptr;  // laid out for the previous M
-  KT_CUDA(c, c->d_pre.reserve((size_t)((m + 31) & ~31) * pre_record_bytes(R) + 16));  // whole 32-throttle words: a decide slot is staged as one block
+  c->pre_stride = (size_t)((m + 31) & ~31) * pre_record_bytes(R);  // whole 32-throttle words: a decide slot is staged as one block
+  KT_CUDA(c, c->d_pre.reserve(2 * c->pre_stride + 16));
   KT_CUDA(c, c->d_changed.reserve(16 + (size_t)m * 5 + 16));
   KT_CUDA(c, cudaMemsetAsync(c->d_changed.p, 0, 16, c->stream));
   c->have_diff = false;
@@ -1267,6 +1301,7 @@ static int evaluate_locked(kt_ctx* c, int64_t now, uint32_t flags) {
   const bool do_rec = !(flags & KT_EVAL_SKIP_RECONCILE), do_chk = !(flags & KT_EVAL_SKIP_CHECK);
   if (given && !c->have_status) return fail(c, KT_ERR_STATE, "KT_EVAL_GIVEN_STATUS without kt_upload_status");
   if (!do_rec && !given && do_chk) return fail(c, KT_ERR_INVALID, "KT_EVAL_SKIP_RECONCILE needs KT_EVAL_GIVEN_STATUS");
+  const LastPass prev = last_pass_on(c->stream);  // (set_device forgets it)
   int rc = set_device(c);
   if (rc) return rc;
   const int R = c->lim.n_resources, M = c->M, Wp = c->ht.Wp;
@@ -1347,10 +1382,19 @@ static int evaluate_locked(kt_ctx* c, int64_t now, uint32_t flags) {
         if (b->p) KT_CUDA(c, cudaMemsetAsync(b->p, 0xA5, b->cap, c->stream));
       run.bitmap_clean = pend.bitmap_clean = false;
     }
+    // counters and pre-records of the other parity: an early successor uses them while this pass may still read its own
+    c->pass_parity ^= 1u;
+    if (px.npeers == 0) px.sync = c->d_sync.as<PassSync>() + c->pass_parity;
     PassArgs a{};
     a.run = pod_view(run); a.pend = pod_view(pend); a.tb = tb; a.tv = tv; a.out = ov; a.px = px;
     a.run_bitmap = run.bitmap.as<uint32_t>(); a.pend_bitmap = pend.bitmap.as<uint32_t>(); a.codes = c->d_codes.as<uint32_t>();
-    a.admit = c->d_admit.as<unsigned char>(); a.pre = c->d_pre.as<unsigned char>(); a.sync = px.sync;
+    a.admit = c->d_admit.as<unsigned char>(); a.pre = pre_records(c); a.sync = px.sync;
+    // Early: the first phase runs before the wait for the previous grid (k_pass has the argument).  Only behind a fused pass of
+    // this library -- of another context, or of this one when neither pass zero-fills (a zero-fill clears words the other pass
+    // writes or reads) -- and not across GPUs.  Anything queued between the two (copies, plain kernels, a stream switch) is
+    // waited for in full before this pass starts, whatever the flag says.
+    const bool zero_fill = a.run.zero_fill || a.pend.zero_fill;
+    a.early = px.npeers == 0 && prev.ctx && (prev.ctx != c || (!prev.zero_fill && !zero_fill));
     a.sparse = sparse_view(c);
     a.now = (long long)now; a.eval_flags = flags; a.L = c->lim.label_slots; a.R = R; a.S = reconcile_slots(c); a.G = G;
     a.n_rec = (unsigned)((run.n + kTileReconcile - 1) / kTileReconcile);
@@ -1358,11 +1402,11 @@ static int evaluate_locked(kt_ctx* c, int64_t now, uint32_t flags) {
     a.n_chk = (unsigned)((pend.n + kTileReconcile - 1) / kTileReconcile);
     if (c->trace) {
       const size_t rows = (size_t)a.n_chk + a.n_rec + a.n_fin;  // one per match, reconcile and status tile (at 128-row tiles: an upper bound for 256-row ones)
-      KT_CUDA(c, c->d_trace.reserve(rows * kTraceRow * 8));
-      KT_CUDA(c, cudaMemsetAsync(c->d_trace.p, 0, rows * kTraceRow * 8, c->stream));
+      KT_CUDA(c, c->d_trace.reserve(rows * kTraceRow * 8));  // (k_pass clears each row it writes: no memset between queued passes)
       a.trace = c->d_trace.as<unsigned long long>();
     }
     KT_CUDA(c, dispatch_pass(c, a));
+    note_pass(c->stream, c, zero_fill);
     if ((rc = sparse_to_caller(c))) return rc;
     c->have_ran = true;
     run.bitmap_clean = pend.bitmap_clean = true;  // zero-filled (if need be) and written by this pass: maintained from here on
@@ -1402,7 +1446,7 @@ static int evaluate_locked(kt_ctx* c, int64_t now, uint32_t flags) {
     // the kernel ahead is the caller's previous launch, maybe a k_pass still reading pre-records) it is a plain launch.
     const long long lanes = (long long)M * G;
     KT_CUDA(c, launch(c, k_finalize, (unsigned)((lanes + 127) / 128), 128, 0, /*pdl=*/!tm && own_primary, tv, M, R, G, (long long)now, flags, px, ov,
-                      c->d_pre.as<unsigned char>()));
+                      pre_records(c)));
     ++launches;
   }
   if (tm) KT_CUDA(c, cudaEventRecord(c->ev[3], c->stream));
@@ -1469,7 +1513,7 @@ int kt_admit_queue(kt_ctx* c, int64_t first, int64_t count, uint32_t flags, int3
   const int R = c->lim.n_resources, M = c->M;
   AdmitView a{};
   a.first = first; a.count = count; a.req = pend.req.as<int64_t>(); a.present = pend.present.as<uint32_t>(); a.bitmap = pend.bitmap.as<uint32_t>();
-  a.n = pend.n; a.Wp = c->ht.Wp; a.W = c->ht.W; a.M = M; a.R = R; a.pre = c->d_pre.as<unsigned char>();
+  a.n = pend.n; a.Wp = c->ht.Wp; a.W = c->ht.W; a.M = M; a.R = R; a.pre = pre_records(c);
   KT_CUDA(c, c->d_adm_state.reserve((size_t)count + 16));
   KT_CUDA(c, c->d_adm_fail.reserve((size_t)count * 4 + 16));
   KT_CUDA(c, c->d_adm_counters.reserve(16));
@@ -1519,6 +1563,7 @@ int kt_step_submit(kt_ctx* c, int64_t n_running, const kt_packed_pods* running, 
   if (!rc) rc = evaluate_locked(c, now, flags);
   c->async_uploads = saved;
   if (rc) return rc;
+  forget_pass(c->stream);  // the result copies follow the pass
   // results -> ONE pinned block: [status block | admit | sparse count | first entries]
   const int64_t P = c->pods[KT_PODS_PENDING].n;
   const size_t out_bytes = status_layout(c->lim.n_resources, c->M).bytes;

@@ -178,7 +178,8 @@ __device__ __forceinline__ void pdl_wait_primary() { asm volatile("griddepcontro
 // wait for it, and before its CTA starts a piece that can wait.  prep_done and tot_done are signalled piece by piece.  Signals are
 // fence + relaxed add (release pattern) by thread 0 after a CTA barrier; waits are relaxed polls + one acquire by thread 0 + a CTA barrier.
 struct PassSync {
-  // counters of ONE pass, re-armed by its last CTA (everything before `error`)
+  // counters of ONE pass, re-armed by its last CTA (everything before `error`).  A context keeps one set per pass parity: an
+  // early k_pass draws tickets while its predecessor still runs on the other set.
   unsigned ticket;      // next piece of work
   unsigned rec_done;    // reconcile tiles finished and published (their REDs are performed at L2)
   unsigned prep_done;   // finalize tiles that have written their throttles' pre-records (nothing to wait for: early)
@@ -862,6 +863,7 @@ __host__ __device__ inline size_t pre_record_bytes(int R) { return 16 + 16 * (si
 
 constexpr int kFinPrep = 1, kFinStatus = 2;  // the halves of a finalize tile: the fused pass runs them as separate tiles (prep first, so
                                              // that nobody ever waits for pre-records), the chained k_finalize runs both
+constexpr int kFinZero = 4;  // with kFinStatus: also zero the other parity's partial sums (k_finalize; k_pass zeroes them after its wait)
 
 // CalculateThreshold(now) of throttle t for resource r (is_res) or the pod count: merged active overrides REPLACE
 // spec.threshold; per resource name the first active override wins (throttle_types.go:65-106).  mybit is r's presence bit
@@ -895,7 +897,7 @@ __device__ __forceinline__ CalcThreshold calculate_threshold(const ThrottleView&
 template <class Sync>
 __device__ __forceinline__ void finalize_tile(const ThrottleView& tv, int M, int R, int G, long long now, uint32_t eval_flags, const PartExchange& px,
                                               const ReconcileView& out, unsigned char* __restrict__ pre /* [M][pre_record_bytes(R)] */, int tile_index,
-                                              const Sync& sync, unsigned long long* trace_row = nullptr, int halves = kFinPrep | kFinStatus) {
+                                              const Sync& sync, unsigned long long* trace_row = nullptr, int halves = kFinPrep | kFinStatus | kFinZero) {
   // optional stage stamps (kt_enable_trace): [4] pre-records written; [5] this rank's reconcile tiles done; [6] sums of every
   // rank read; [7] status columns written
   auto stamp = [&](int k) {
@@ -919,7 +921,7 @@ __device__ __forceinline__ void finalize_tile(const ThrottleView& tv, int M, int
   const size_t i_has = (size_t)(R + r) * M + t;               // resource lanes: its presence flag
 
   // the other parity's buffers are left zeroed for the next pass
-  if (halves & kFinStatus) {
+  if (halves & kFinZero) {
     if (is_res) {
       px.zero_mine[col] = 0ull;
       px.zero_mine[i_has] = 0ull;
@@ -1799,6 +1801,7 @@ struct PassArgs {
   int L, R, S, G;
   unsigned quad;                 // 1: decide sub-tiles of TILE/4 pending pods, four lanes per pod (check_decide_quad); 0: decide tiles of
                                  // TILE pods, one lane per pod (check_decide_tile) -- the host picks (launch_pass)
+  unsigned early;                // 1: run the first phase before waiting for the previous grid (the host decides: evaluate_locked)
   unsigned n_chk, n_rec, n_fin;  // tiles per role; tickets: [match (+ prep) n_chk][reconcile n_rec][second phase: n_fin status tiles and n_sub
   unsigned n_sub;                // decide (sub-)tiles -- status first with peers (they carry the exchange the decide
                                  // sub-tiles wait for), last alone (nobody waits for them)]; a piece only ever waits for SMALLER tickets
@@ -1822,20 +1825,35 @@ __global__ void __launch_bounds__(TILE, THREADS / TILE) k_pass(const __grid_cons
   __shared__ unsigned s_ticket;
   __shared__ unsigned s_last;                 // trace: this CTA's last first-phase ticket (~0u: none yet)
   __shared__ unsigned s_done[2];              // first-phase tiles this CTA has finished and not yet published: match, reconcile
+  __shared__ unsigned s_tail;                 // 1: this CTA ran the last first-phase ticket
   __shared__ unsigned long long s_t_start;    // trace: when the current tile began
   __shared__ __align__(8) unsigned long long s_mbar[kMaxWarps];  // transaction barriers: one per warp (bulk copies of the shared decide tiles)
-  // Launched with programmatic stream serialization, and we trigger at once: the NEXT launch in the stream may have its CTAs
-  // placed while this grid still runs.  A next k_pass sits in the wait below; any other kernel that follows with PDL must wait
-  // before its first access to shared state, which is why a pass that does not start with k_pass launches k_finalize plainly.
-  pdl_launch_dependents();
+  // Launched with programmatic stream serialization.  The previous grid in the stream is waited for at the top, or -- an EARLY
+  // pass -- only once this CTA leaves the first phase.  An early pass is one the host has proven safe (evaluate_locked): its
+  // primary is a k_pass of another context, or of this one when neither zero-fills.  Its first phase then writes only what is
+  // its own or what the primary's second phase does not read differently:
+  //   - PassSync counters and pre-records: one set per pass parity (the host alternates them), re-armed / rewritten only by
+  //     the pass two back, which had completed before the primary's CTAs got past their wait and triggered us;
+  //   - partial sums: the half of this parity, zeroed by the primary after its wait and before its trigger (below);
+  //   - match rows (pending and running bitmaps): rows and tables are unchanged since the primary, so every word is rewritten
+  //     with the value the primary stored and reads;
+  //   - code words: a match tile writes them only when it zero-fills (never in an early pass); decide rewrites every word
+  //     whose match bits are set, and codes are zero elsewhere;
+  //   - the sparse list's counter is reset after the wait (s_tail), before anything this pass decides can append.
+  // The trigger follows the wait, so at most two passes run at once.  No wait can deadlock: first-phase tiles never wait; a
+  // second-phase piece waits for smaller tickets of its own pass, or for the previous grid, all of whose CTAs were placed
+  // before it triggered and none of which waits for this one; a CTA of this grid that cannot be placed yet only starts later.
+  // Any other kernel that follows with PDL must wait before its first access to shared state, which is why a pass that does
+  // not start with k_pass launches k_finalize plainly.
   if (threadIdx.x == 0) {
 #pragma unroll
     for (int i = 0; i < kMaxWarps; ++i) mbar_init(&s_mbar[i], 1u);
     mbar_init_fence();
     s_last = ~0u;
     s_done[0] = s_done[1] = 0u;
+    s_tail = 0u;
   }
-  pdl_wait_primary();
+  if (!a.early) pdl_wait_primary();
   const unsigned n_tiles = a.n_chk + a.n_rec;
   auto draw = [&]() -> unsigned {
     __syncthreads();  // everybody has read the previous ticket, and the CTA's shared memory is free again
@@ -1845,6 +1863,10 @@ __global__ void __launch_bounds__(TILE, THREADS / TILE) k_pass(const __grid_cons
   };
   // (the trace bookkeeping lives in shared memory: nothing of it stays in registers across a tile, which runs at the register cap)
   auto trace_row = [&](unsigned t) -> unsigned long long* { return a.trace && t != ~0u ? a.trace + (size_t)t * kTraceRow : nullptr; };
+  auto open_row = [&](unsigned long long* row) {  // thread 0, before a traced tile stamps anything: the rows are not cleared
+    for (int k = 0; k < kTraceRow; ++k) row[k] = 0ull;  // between passes (no memset may come between two queued passes)
+    s_t_start = globaltimer_ns();
+  };
   auto close_row = [&](unsigned long long* row) {  // thread 0, at the end of a traced tile
     unsigned smid;
     asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
@@ -1862,33 +1884,51 @@ __global__ void __launch_bounds__(TILE, THREADS / TILE) k_pass(const __grid_cons
       atomicAdd(&a.sync->match_done, s_done[0]);
       s_done[0] = 0u;
     }
-    if (a.trace && threadIdx.x == 0) s_t_start = globaltimer_ns();
+    if (a.trace && threadIdx.x == 0) open_row(trace_row(ticket));
     if (ticket < a.n_chk) {
       const FlagSync sync{a.sync, a.n_rec, a.n_fin, a.n_chk};
       // The match tiles also write the pre-records (the prep half of the finalize tiles, spread over them): they hold the first
       // tickets, so every pre-record exists a few microseconds into the pass and no decide sub-tile ever waits for one.
       for (unsigned ft = ticket; ft < a.n_fin; ft += a.n_chk)
         finalize_tile(a.tv, a.tb.M, a.R, a.G, a.now, a.eval_flags, a.px, a.out, a.pre, (int)ft, sync, nullptr, kFinPrep);
-      // the first match tile also clears the sparse list's counter: every decide sub-tile waits for ALL match tiles before it appends
-      if (ticket == 0 && threadIdx.x == 0 && a.sparse.count) *a.sparse.count = 0u;
       check_match_tile<TPC, B, REG, TILE>(a.pend, a.tb, a.L, a.pend_bitmap, a.codes, smem_raw, ticket);
     } else {
       reconcile_tile<TPC, B, RT, REG, TILE>(a.run, a.tb, a.L, a.R, a.S, a.run_bitmap, a.px.mine, smem_raw, ticket - a.n_chk, trace_row(ticket));
     }
     if (threadIdx.x == 0) {  // (s_ticket is still this tile's: the next draw begins with a CTA barrier)
       ++s_done[ticket < a.n_chk ? 0 : 1];
+      if (ticket == n_tiles - 1) s_tail = 1u;
       if (a.trace) {
         close_row(trace_row(s_ticket));
         s_last = s_ticket;
       }
     }
   }
-  // the rest, before this CTA starts anything that can wait (release pattern, as cta_signal)
-  if (threadIdx.x == 0 && (s_done[0] | s_done[1])) {
-    __threadfence();
-    if (s_done[0]) atomicAdd(&a.sync->match_done, s_done[0]);
-    if (s_done[1]) atomicAdd(&a.sync->rec_done, s_done[1]);
+  if (a.early) pdl_wait_primary();
+  // The previous grid has completed.  The CTA that ran the last first-phase ticket clears the sparse list's counter before it
+  // publishes that tile: every decide piece waits for it (match_done or rec_done) before it appends.  Then the rest of this
+  // CTA's tiles, before it starts anything that can wait (release pattern, as cta_signal).
+  if (threadIdx.x == 0) {
+    if (s_tail && a.sparse.count) *a.sparse.count = 0u;
+    if (s_done[0] | s_done[1]) {
+      __threadfence();
+      if (s_done[0]) atomicAdd(&a.sync->match_done, s_done[0]);
+      if (s_done[1]) atomicAdd(&a.sync->rec_done, s_done[1]);
+    }
   }
+  // The other parity's partial sums -- the previous pass's, read by nobody now -- are zeroed for the next pass before this CTA
+  // lets it start: the next pass adds into them from its first phase on.
+  {
+    const size_t len = (size_t)(2 * a.R + 1) * a.tb.M, stride = (size_t)gridDim.x * TILE;
+    bool wrote = false;
+    for (size_t i = (size_t)blockIdx.x * TILE + threadIdx.x; i < len; i += stride) {
+      a.px.zero_mine[i] = 0ull;
+      wrote = true;
+    }
+    if (wrote) __threadfence();
+  }
+  __syncthreads();
+  pdl_launch_dependents();
   // ---- second phase: status tiles and decide sub-tiles, until the counter runs past them ----
   unsigned mbar_phase = 0;
   bool first = true;
@@ -1900,7 +1940,7 @@ __global__ void __launch_bounds__(TILE, THREADS / TILE) k_pass(const __grid_cons
     const FlagSync sync{a.sync, a.n_rec, a.n_fin, a.n_chk};
     if (is_status) {  // traced as row n_tiles + index (after the first-phase tickets' rows)
       unsigned long long* trow = trace_row(n_tiles + index);
-      if (trow && threadIdx.x == 0) s_t_start = globaltimer_ns();
+      if (trow && threadIdx.x == 0) open_row(trow);
       finalize_tile(a.tv, a.tb.M, a.R, a.G, a.now, a.eval_flags, a.px, a.out, a.pre, (int)index, sync, trow, kFinStatus);
       if (trow && threadIdx.x == 0) close_row(trow);
     } else if (a.quad) {
@@ -1912,7 +1952,7 @@ __global__ void __launch_bounds__(TILE, THREADS / TILE) k_pass(const __grid_cons
                                   a.sparse);
     }
   }
-  // the last CTA out re-arms the counters for the next launch (stream-ordered after this one)
+  // the last CTA out re-arms the counters for the next pass of this parity (it starts after this grid has completed)
   __syncthreads();
   if (threadIdx.x == 0) {
     if (unsigned long long* row = trace_row(s_last)) row[29] = globaltimer_ns();
