@@ -416,6 +416,10 @@ struct ThrottleObj {
     return "";
   }
 };
+// The key of a throttle in kth_plugin::thr_index: "T:namespace/name" for a Throttle, "C:/name" for a ClusterThrottle.
+std::string thr_key(int kind, const std::string& ns, const std::string& name) {
+  return (kind == KT_KIND_THROTTLE ? "T:" + ns : std::string("C:")) + "/" + name;
+}
 
 // label key of the internal "this namespace exists" marker: not a legal label key, so it cannot collide with a real one
 const char* const kNsExistsKey = "\x01kt/exists";
@@ -511,7 +515,12 @@ struct kth_plugin {
   bool pods_full_upload = true;
 
   std::vector<ThrottleObj> throttles;  // column order == device order (both kinds interleaved, insertion order)
-  std::unordered_map<std::string, int> thr_index;  // "T:ns/name" | "C:/name"
+  std::unordered_map<std::string, int> thr_index;  // thr_key -> column, live throttles only
+  // the column of the throttle a (namespace, name) argument names -- a ClusterThrottle when the namespace is empty --, -1 if none
+  int find_throttle(const std::string& ns, const std::string& tname) const {
+    auto it = thr_index.find(thr_key(ns.empty() ? KT_KIND_CLUSTERTHROTTLE : KT_KIND_THROTTLE, ns, tname));
+    return it == thr_index.end() ? -1 : it->second;
+  }
   // Device columns of deleted throttles are handed out again (a scheduler that lives for months sees throttles come and go: M,
   // the table compile and every pass would only ever grow otherwise).  Whatever lists throttles for the caller -- affected
   // throttles of a pod (the order of the names inside a PreFilter reason), the broken-selector walk (WHICH error a pod gets),
@@ -527,6 +536,16 @@ struct kth_plugin {
   bool throttles_dirty = true, namespaces_dirty = true, status_dirty = true, reserved_dirty = true;
   std::vector<size_t> broken;  // columns of the throttles with a podSelector that does not convert (controller_error)
   bool broken_valid = false;
+  const std::vector<size_t>& broken_throttles() {  // usually none, so not a walk over all throttles per pod: built on first need
+    if (!broken_valid) {
+      broken.clear();
+      for (size_t t = 0; t < throttles.size(); ++t)
+        if (throttles[t].live && !throttles[t].selector_error().empty()) broken.push_back(t);
+      creation_order(broken);
+      broken_valid = true;
+    }
+    return broken;
+  }
 
   ReservationCache cache[2];  // one per controller (controller.go:34-50)
 
@@ -932,7 +951,7 @@ struct kth_plugin {
     free_thr.clear();
     thr_reused = false;
     for (size_t t = 0; t < throttles.size(); ++t) {
-      thr_index[std::string(throttles[t].kind == KT_KIND_THROTTLE ? "T:" : "C:") + throttles[t].nn()] = (int)t;
+      thr_index[thr_key(throttles[t].kind, throttles[t].ns, throttles[t].name)] = (int)t;
       if (t && throttles[t].seq < throttles[t - 1].seq) thr_reused = true;  // column order is not creation order
     }
     broken_valid = false;
@@ -1150,6 +1169,13 @@ struct kth_plugin {
     sync_namespaces();
     sync_throttles();
   }
+  // Everything a PreFilter view reads: the tables, the informer copy of the statuses and the reservations.  A table change voids
+  // the cached queue verdicts on the way (sync_namespaces / sync_throttles); afterwards no dirty flag is set.
+  void sync_state() {
+    sync_all();
+    sync_status();
+    sync_reserved();
+  }
 
   // ---- results -> objects ------------------------------------------------------------------------------
   Quantity from_scale(int c, int64_t v) const {
@@ -1328,9 +1354,25 @@ struct kth_plugin {
     return out;
   }
 
-  // What reconcile writes for throttle t from its device status (entry q of columns shaped for k throttles): status.used,
-  // calculatedThreshold (Q6), throttled, compared under Semantic.DeepEqual; records the gauges.  Returns whether the status changed.
-  bool update_status(size_t t, const kt_reconcile_out& ro, size_t k, size_t q, const GoTime& now) {
+  // The kt_reconcile_out columns of k throttles, as kt_get_reconcile_rows and kt_reconcile_throttles fill them.
+  struct ReconcileCols {
+    size_t k;
+    std::vector<int64_t> used, used_cnt, calc_thr, calc_cnt;
+    std::vector<uint32_t> used_present, throttled, calc_present;
+    std::vector<uint8_t> ovr_active;
+    kt_reconcile_out out;
+    ReconcileCols(size_t k, int R)
+        : k(k), used((size_t)R * std::max<size_t>(k, 1)), used_cnt(k), calc_thr((size_t)R * std::max<size_t>(k, 1)), calc_cnt(k),
+          used_present(k), throttled(k), calc_present(k), ovr_active(k),
+          out{used.data(), used_present.data(), used_cnt.data(), throttled.data(), calc_thr.data(), calc_present.data(), calc_cnt.data(), ovr_active.data()} {}
+    ReconcileCols(const ReconcileCols&) = delete;  // `out` points into this object's columns
+    ReconcileCols& operator=(const ReconcileCols&) = delete;
+  };
+  // What reconcile writes for throttle t from its device status (entry q of st): status.used, calculatedThreshold (Q6),
+  // throttled, compared under Semantic.DeepEqual; records the gauges.  Returns whether the status changed.
+  bool update_status(size_t t, const ReconcileCols& st, size_t q, const GoTime& now) {
+    const kt_reconcile_out& ro = st.out;
+    const size_t k = st.k;
     ThrottleObj& o = throttles[t];
     o.host_dirty = false;
     ResAmount nu;  // used := ResourceAmount{}; used = used.Add(ResourceAmountOfPod(p)) ...
@@ -1381,22 +1423,98 @@ struct kth_plugin {
     return status_changed;
   }
 
+  // What a reconcile of several throttles returns: kth_reconcile_all's object; kth_reconcile's adds errors and notFound.
+  struct ReconcileReport {
+    int reconciled = 0;
+    std::vector<std::string> changed;
+    std::vector<std::pair<std::string, long long>> requeue;  // enqueueAfter(thr, *nextOverrideHappensIn)
+    std::vector<std::pair<std::string, std::string>> errors;
+    std::vector<std::string> not_found;
+    std::string json(bool keyed) const {
+      Writer w;
+      w.begin_obj().key("reconciled").num(reconciled).key("changed").begin_arr();
+      for (auto& c : changed) w.str(c);
+      w.end_arr().key("requeueAfterNanos").begin_obj();
+      for (auto& r : requeue) w.key(r.first).num(r.second);
+      w.end_obj();
+      if (keyed) {
+        w.key("errors").begin_obj();
+        for (auto& er : errors) w.key(er.first).str(er.second);
+        w.end_obj().key("notFound").begin_arr();
+        for (auto& nf : not_found) w.str(nf);
+        w.end_arr();
+      }
+      w.end_obj();
+      return w.out;
+    }
+  };
+
+  // reconcile(key) of the responsible throttle t once the device has answered for it.  Both callers give the answer in one form:
+  // matched(row) says whether t matches running row `row` -- the RUNNING relation, affectedPods: counted pods, finished ones
+  // included --, and [fin0, fin1) holds every finished row t matches (rows t does not match may be among them).  err_rows are
+  // selector_error_rows(t); q is t's entry in st, < 0 when the device says its status does not change.  Returns the error that
+  // fails the reconcile, "" when it ran.
+  template <class Matched>
+  std::string reconcile_throttle(size_t t, const Matched& matched, const std::vector<int64_t>& err_rows, const int64_t* fin0, const int64_t* fin1,
+                                 const ReconcileCols& st, int64_t q, const GoTime& now, ReconcileReport& rep) {
+    ThrottleObj& o = throttles[t];
+    // A Throttle with a podSelector term that does not convert: affectedPods (throttle_controller.go:221-246) only fails -- and
+    // the reconcile with it: status untouched, nothing un-reserved (:233-236) -- when some counted pod of the namespace actually
+    // REACHES that term, i.e. matches none of the valid terms before it (those are what the device column holds,
+    // sync_throttles).  The first such pod in informer order names the error.  ClusterThrottles: see DESIGN.md "Known
+    // deviations" (their terms carry their own namespace scope).
+    const PodObj* first = nullptr;
+    for (int64_t r : err_rows)
+      if (!matched(r) && (!first || pods[(size_t)r].seq < first->seq)) first = &pods[(size_t)r];
+    if (first) return reachable_selector_error(o, first->ns);
+    ++rep.reconciled;
+    if (q >= 0 && update_status(t, st, (size_t)q, now)) rep.changed.push_back(o.nn());
+    __int128 after = 0;
+    if (next_override_happens_in(o, now, &after)) rep.requeue.emplace_back(o.nn(), (long long)(after > INT64_MAX ? INT64_MAX : after));
+    // unreserveAffectedPods: every affected pod the informer has observed leaves the reservation cache -- except, for a
+    // Throttle, the finished ones the reference's list loses.  Q8 (throttle_controller.go:241, `terminatedPods =
+    // append(nonterminatedPods, pod)`): the THROTTLE controller's list of terminated affected pods ends up holding only the
+    // LAST terminated match of the namespace (a Throttle matches the pods of its own namespace only), so of the finished pods
+    // that still hold a reservation only that one is un-reserved; the others keep it until the pod is deleted.  (Which pod is
+    // "last" is the informer's map order in the reference; the oracle and this code take the order of first appearance.)
+    auto it = cache[o.kind].by_thr.find(o.nn());
+    if (it == cache[o.kind].by_thr.end()) return "";
+    int64_t last_fin = -2;  // computed on first need
+    std::vector<std::string> gone;
+    for (auto& pod : it->second) {
+      auto pi = pod_index.find(pod.first);
+      if (pi == pod_index.end() || !matched(pi->second)) continue;
+      if (o.kind == KT_KIND_THROTTLE && !(pod_flags(pods[(size_t)pi->second]) & KT_POD_NOT_FINISHED)) {
+        if (last_fin == -2) {
+          last_fin = -1;
+          for (const int64_t* r = fin0; r < fin1; ++r) {
+            const PodObj& p = pods[(size_t)*r];
+            if (matched(*r) && !(pod_flags(p) & KT_POD_NOT_FINISHED) && (last_fin < 0 || p.seq > pods[(size_t)last_fin].seq)) last_fin = *r;
+          }
+        }
+        if (pi->second != last_fin) continue;
+      }
+      gone.push_back(pod.first);
+    }
+    for (auto& g : gone)
+      if (it->second.erase(g)) reservation_changed(t);
+    return "";
+  }
+
   std::string reconcile_all(const std::string& now_s) {
     GoTime now;
     std::string e = parse_rfc3339(now_s, &now);
     if (!e.empty()) fail(e);
     sync_all();
     const size_t m = throttles.size();
-    Writer w;
-    w.begin_obj();
-    if (m == 0) { w.key("reconciled").num(0).key("changed").begin_arr().end_arr().key("requeueAfterNanos").begin_obj().end_obj().end_obj(); return w.out; }
+    ReconcileReport rep;
+    if (m == 0) return rep.json(false);
     // The informer copy of every status is on the device (sync_status: a no-op unless some status changed since the last
     // upload), so the pass itself diffs what it computes against it (throttle_controller.go:157 DeepEqual): only the throttles it
     // lists -- plus those applied since their last reconcile, whose host-only status parts may differ -- are looked at and
     // downloaded below (SURVEY 8f.3: the download and the host's work are proportional to what changed, not to M).
     sync_status();
     check(kt_evaluate(ctx, clamp_ns(now.ns()), KT_EVAL_FRESH_STATUS | KT_EVAL_SKIP_CHECK), "kt_evaluate");
-    const int R = lim.n_resources;
     std::vector<int32_t> todo_idx(m);
     std::vector<int32_t> pos(m, -1);  // throttle column -> its row in the gathered status columns
     size_t k = 0;
@@ -1410,110 +1528,59 @@ struct kth_plugin {
       for (size_t t = 0; t < m; ++t)
         if (mark[t]) { pos[t] = (int32_t)k; todo_idx[k++] = (int32_t)t; }
     }
-    std::vector<int64_t> used((size_t)R * std::max<size_t>(k, 1)), used_cnt(k), calc_thr((size_t)R * std::max<size_t>(k, 1)), calc_cnt(k);
-    std::vector<uint32_t> used_present(k), throttled(k), calc_present(k);
-    std::vector<uint8_t> ovr_active(k);
-    kt_reconcile_out ro{used.data(), used_present.data(), used_cnt.data(), throttled.data(), calc_thr.data(), calc_present.data(), calc_cnt.data(), ovr_active.data()};
-    if (k) check(kt_get_reconcile_rows(ctx, (int64_t)k, todo_idx.data(), &ro), "kt_get_reconcile_rows");
-    // pods that are reserved somewhere: their match rows decide what reconcile un-reserves (:135-155)
+    ReconcileCols st(k, lim.n_resources);
+    if (k) check(kt_get_reconcile_rows(ctx, (int64_t)k, todo_idx.data(), &st.out), "kt_get_reconcile_rows");
+    // The match words of the running rows the throttles' steps ask about (a row's words hold every throttle's bit).  First the
+    // pods that are reserved somewhere: their match rows decide what reconcile un-reserves (:135-155).
     std::vector<int64_t> rows;
-    std::vector<std::string> row_pod;
     {
       std::set<std::string> seen;
       for (int k = 0; k < 2; ++k)
         for (auto& thr : cache[k].by_thr)
           for (auto& pod : thr.second) {
             auto it = pod_index.find(pod.first);
-            if (it != pod_index.end() && seen.insert(pod.first).second) { rows.push_back(it->second); row_pod.push_back(pod.first); }
+            if (it != pod_index.end() && seen.insert(pod.first).second) rows.push_back(it->second);
           }
     }
     const int Wp = kt_match_words(ctx);
-    std::vector<uint32_t> words(rows.size() * (size_t)Wp);
-    if (!rows.empty()) check(kt_get_match_rows(ctx, KT_PODS_RUNNING, (int64_t)rows.size(), rows.data(), words.data()), "kt_get_match_rows");
-    // Q8 (throttle_controller.go:241, `terminatedPods = append(nonterminatedPods, pod)`): the THROTTLE controller's list of
-    // terminated affected pods ends up holding only the LAST terminated match of the namespace, so of the finished pods that
-    // still hold a reservation only that one is un-reserved; the others keep it until the pod is deleted.  (Which pod is "last"
-    // is the informer's map order in the reference; the oracle and this code take the order of first appearance.)  Needed only
-    // when a finished pod holds a reservation: then the match rows of the finished counted pods say who is last per throttle.
-    std::vector<char> row_finished(rows.size(), 0);
+    std::vector<std::vector<uint32_t>> words;
+    std::unordered_map<int64_t, const uint32_t*> words_of;
+    auto fetch = [&](const std::vector<int64_t>& rs) {
+      if (rs.empty()) return;
+      words.emplace_back(rs.size() * (size_t)Wp);
+      check(kt_get_match_rows(ctx, KT_PODS_RUNNING, (int64_t)rs.size(), rs.data(), words.back().data()), "kt_get_match_rows");
+      for (size_t i = 0; i < rs.size(); ++i) words_of[rs[i]] = words.back().data() + i * (size_t)Wp;
+    };
+    fetch(rows);
+    // Q8 asks which finished pod is the last match of a Throttle only when a finished pod holds a reservation: then the rows of
+    // the finished counted pods
     bool any_finished_reserved = false;
-    for (size_t i = 0; i < rows.size(); ++i) {
-      const PodObj& p = pods[(size_t)rows[i]];
-      row_finished[i] = p.live && !(pod_flags(p) & KT_POD_NOT_FINISHED);
-      any_finished_reserved |= row_finished[i] != 0;
-    }
+    for (int64_t r : rows) any_finished_reserved |= !(pod_flags(pods[(size_t)r]) & KT_POD_NOT_FINISHED);
     std::vector<int64_t> fin_rows;
-    std::vector<uint32_t> fin_words;
     if (any_finished_reserved) {
       for (auto& p : pods)
         if (p.live && should_count_in(p) && !(pod_flags(p) & KT_POD_NOT_FINISHED)) fin_rows.push_back(p.row);
-      fin_words.resize(fin_rows.size() * (size_t)Wp);
-      if (!fin_rows.empty()) check(kt_get_match_rows(ctx, KT_PODS_RUNNING, (int64_t)fin_rows.size(), fin_rows.data(), fin_words.data()), "kt_get_match_rows");
+      fetch(fin_rows);
     }
-    auto last_finished_match = [&](size_t t, const std::string& ns) -> int64_t {  // row of the last finished pod of ns that matches t
-      int64_t best = -1;
-      uint64_t best_seq = 0;
-      for (size_t i = 0; i < fin_rows.size(); ++i) {
-        const PodObj& p = pods[(size_t)fin_rows[i]];
-        if (p.ns != ns || !((fin_words[i * (size_t)Wp + (t >> 5)] >> (t & 31)) & 1)) continue;
-        if (best < 0 || p.seq > best_seq) { best = p.row; best_seq = p.seq; }
+    // the counted pods a broken podSelector term may be in the way of
+    std::vector<std::vector<int64_t>> err_rows(m);
+    for (size_t t = 0; t < m; ++t)
+      if (throttles[t].live && throttles[t].throttler_name == name) {
+        err_rows[t] = selector_error_rows(throttles[t]);
+        fetch(err_rows[t]);
       }
-      return best;
-    };
 
-    // A Throttle with a podSelector term that does not convert: affectedPods (throttle_controller.go:221-246) only fails -- and
-    // the reconcile with it -- when some counted pod of the namespace actually REACHES that term, i.e. matches none of the
-    // valid terms before it (those are what the device column holds, sync_throttles).  The rows of the namespace's counted
-    // pods tell.  ClusterThrottles: see DESIGN.md "Known deviations" (their terms carry their own namespace scope).
-    std::vector<char> selector_fails(m, 0);
-    for (size_t t = 0; t < m; ++t) {
-      const ThrottleObj& o = throttles[t];
-      if (!o.live || o.throttler_name != name) continue;
-      const std::vector<int64_t> ns_rows = selector_error_rows(o);
-      if (ns_rows.empty()) continue;  // nobody to ask the selector about: no error
-      std::vector<uint32_t> w((size_t)ns_rows.size() * (size_t)Wp);
-      check(kt_get_match_rows(ctx, KT_PODS_RUNNING, (int64_t)ns_rows.size(), ns_rows.data(), w.data()), "kt_get_match_rows");
-      for (size_t i = 0; i < ns_rows.size() && !selector_fails[t]; ++i)
-        if (!((w[i * (size_t)Wp + (t >> 5)] >> (t & 31)) & 1)) selector_fails[t] = 1;
-    }
-
-    int reconciled = 0;
-    std::vector<std::string> changed;
-    std::vector<std::pair<std::string, long long>> requeue;
     std::vector<size_t> thr_order(m);
     for (size_t t = 0; t < m; ++t) thr_order[t] = t;
     creation_order(thr_order);
     for (size_t t : thr_order) {
-      ThrottleObj& o = throttles[t];
-      if (!o.live || o.throttler_name != name) continue;   // only responsible throttles are ever enqueued (:403-425)
-      if (selector_fails[t]) continue;                      // affectedPods fails -> reconcile returns the error, status untouched
-      ++reconciled;
-      const int32_t q = pos[t];  // >= 0: the device says its status changes (or the object was applied since its last reconcile)
-      if (q >= 0 && update_status(t, ro, k, (size_t)q, now)) changed.push_back(o.nn());
-      __int128 after = 0;
-      if (next_override_happens_in(o, now, &after)) requeue.emplace_back(o.nn(), (long long)(after > INT64_MAX ? INT64_MAX : after));
-      // unreserveAffectedPods: every affected pod the informer has observed leaves the reservation cache -- except, for a
-      // Throttle, the finished ones the reference's list loses (Q8)
-      auto it = cache[o.kind].by_thr.find(o.nn());
-      if (it != cache[o.kind].by_thr.end()) {
-        int64_t last_fin = -2;  // computed on first need
-        for (size_t i = 0; i < rows.size(); ++i) {
-          if (!((words[i * (size_t)Wp + (t >> 5)] >> (t & 31)) & 1)) continue;
-          if (o.kind == KT_KIND_THROTTLE && row_finished[i]) {
-            if (last_fin == -2) last_fin = last_finished_match(t, o.ns);
-            if (rows[i] != last_fin) continue;
-          }
-          if (it->second.erase(row_pod[i])) reservation_changed(t);
-        }
-      }
+      const ThrottleObj& o = throttles[t];
+      if (!o.live || o.throttler_name != name) continue;  // only responsible throttles are ever enqueued (:403-425)
+      auto matched = [&](int64_t r) { return ((words_of.at(r)[t >> 5] >> (t & 31)) & 1) != 0; };
+      // (a selector error leaves t as it is: kth_reconcile_all does not report it)
+      reconcile_throttle(t, matched, err_rows[t], fin_rows.data(), fin_rows.data() + fin_rows.size(), st, pos[t], now, rep);
     }
-    w.key("reconciled").num(reconciled).key("changed").begin_arr();
-    for (auto& c : changed) w.str(c);
-    w.end_arr();
-    w.key("requeueAfterNanos").begin_obj();  // enqueueAfter(thr, *nextOverrideHappensIn)
-    for (auto& r : requeue) w.key(r.first).num(r.second);
-    w.end_obj().end_obj();
-    return w.out;
+    return rep.json(false);
   }
 
   // The counted pods a broken podSelector term of o is in the way of: the Throttle's namespace, or -- per term -- the
@@ -1557,16 +1624,15 @@ struct kth_plugin {
     if (codes) codes->resize((size_t)off[1]);
   }
   std::string affected_pods(const std::string& ns, const std::string& tname) {
-    const std::string key = ns.empty() ? "C:/" + tname : "T:" + ns + "/" + tname;
-    auto it = thr_index.find(key);
-    if (it == thr_index.end()) fail((ns.empty() ? "clusterthrottle " : "throttle ") + ns + "/" + tname + " not found");
-    const ThrottleObj& found = throttles[(size_t)it->second];
+    const int found_at = find_throttle(ns, tname);
+    if (found_at < 0) fail((ns.empty() ? "clusterthrottle " : "throttle ") + ns + "/" + tname + " not found");
+    const ThrottleObj& found = throttles[(size_t)found_at];
     if (found.throttler_name != name) fail(found.nn() + " belongs to throttler \"" + found.throttler_name + "\", not to \"" + name + "\"");
     if (columns_epoch != epoch) {
       run_pending_pass({}, 0, 0);
       columns_epoch = codes_epoch = epoch;
     }
-    const size_t t = (size_t)thr_index.at(key);  // (the pass may have laid the columns out anew)
+    const size_t t = (size_t)find_throttle(ns, tname);  // (the pass may have laid the columns out anew)
     std::vector<int64_t> run_rows, pend_rows;
     std::vector<uint8_t> codes;
     column_of(KT_PODS_RUNNING, (int32_t)t, run_rows, nullptr);
@@ -1667,9 +1733,8 @@ struct kth_plugin {
   }
 
   // ---- reconcile(key) for listed throttles (kth_reconcile) -----------------------------------------------------------
-  // Each distinct key gets what reconcile_all does for its throttle -- status (Q6, Semantic.DeepEqual), cached verdicts, gauges,
-  // NextOverrideHappensIn, unreserveAffectedPods (Q8) or the reachable broken-podSelector error -- from one kt_reconcile_throttles
-  // call over the listed columns only.  Throttles that are not listed are not touched.
+  // Each distinct key gets what reconcile_all does for its throttle (reconcile_throttle) from one kt_reconcile_throttles call
+  // over the listed columns only.  Throttles that are not listed are not touched.
   std::string reconcile_keys(const std::string& keys_json, const std::string& now_s) {
     GoTime now;
     std::string e = parse_rfc3339(now_s, &now);
@@ -1678,8 +1743,7 @@ struct kth_plugin {
     if (!keys->is(Node::Arr)) fail("reconcile: keys must be a JSON array of \"namespace/name\" (Throttle) or \"/name\" (ClusterThrottle)");
     if (!kt_reconcile_throttles) fail("kth_reconcile: the engine this plugin is linked against has no kt_reconcile_throttles");
     sync_all();  // (may lay the throttle columns out anew: keys are resolved after it)
-    std::vector<std::pair<std::string, std::string>> errors;
-    std::vector<std::string> not_found;
+    ReconcileReport rep;
     std::vector<std::pair<std::string, int32_t>> todo;  // key, throttle column
     std::set<std::string> seen;
     for (auto& kp : keys->arr) {
@@ -1690,81 +1754,35 @@ struct kth_plugin {
       const size_t slash = key.find('/');
       const std::string ns = slash == std::string::npos ? "" : key.substr(0, slash), tname = slash == std::string::npos ? "" : key.substr(slash + 1);
       if (slash == std::string::npos || tname.empty() || tname.find('/') != std::string::npos) {
-        errors.emplace_back(key, "unexpected key format: \"" + key + "\"");
+        rep.errors.emplace_back(key, "unexpected key format: \"" + key + "\"");
         continue;
       }
-      auto it = thr_index.find(ns.empty() ? "C:/" + tname : "T:" + ns + "/" + tname);
-      if (it == thr_index.end() || !throttles[(size_t)it->second].live) { not_found.push_back(key); continue; }  // the lister's NotFound: nil
-      if (throttles[(size_t)it->second].throttler_name != name) continue;  // only responsible throttles are ever enqueued (:403-425)
-      todo.emplace_back(key, (int32_t)it->second);
+      const int t = find_throttle(ns, tname);
+      if (t < 0 || !throttles[(size_t)t].live) { rep.not_found.push_back(key); continue; }  // the lister's NotFound: nil
+      if (throttles[(size_t)t].throttler_name != name) continue;  // only responsible throttles are ever enqueued (:403-425)
+      todo.emplace_back(key, (int32_t)t);
     }
     const size_t k = todo.size();
-    const int R = lim.n_resources;
     std::vector<int32_t> idx(k);
     for (size_t q = 0; q < k; ++q) idx[q] = todo[q].second;
-    std::vector<int64_t> used((size_t)R * std::max<size_t>(k, 1)), used_cnt(k), calc_thr((size_t)R * std::max<size_t>(k, 1)), calc_cnt(k);
-    std::vector<uint32_t> used_present(k), throttled(k), calc_present(k);
-    std::vector<uint8_t> ovr_active(k);
-    kt_reconcile_out ro{used.data(), used_present.data(), used_cnt.data(), throttled.data(), calc_thr.data(), calc_present.data(), calc_cnt.data(), ovr_active.data()};
+    ReconcileCols st(k, lim.n_resources);
     std::vector<int64_t> off(k + 1, 0), rows;
     int64_t cap = 1024;
     while (k) {  // the matched rows of every listed throttle, ascending
       rows.resize((size_t)cap);
-      check(kt_reconcile_throttles(ctx, clamp_ns(now.ns()), (int64_t)k, idx.data(), &ro, off.data(), rows.data(), cap), "kt_reconcile_throttles");
+      check(kt_reconcile_throttles(ctx, clamp_ns(now.ns()), (int64_t)k, idx.data(), &st.out, off.data(), rows.data(), cap), "kt_reconcile_throttles");
       if (off[k] <= cap) break;
       cap = off[k];
     }
-    int reconciled = 0;
-    std::vector<std::string> changed;
-    std::vector<std::pair<std::string, long long>> requeue;
     for (size_t q = 0; q < k; ++q) {
       const size_t t = (size_t)idx[q];
-      ThrottleObj& o = throttles[t];
       const int64_t* r0 = rows.data() + off[q];
       const int64_t* r1 = rows.data() + off[q + 1];
-      // a counted pod that reaches a broken term: affectedPods fails, and reconcile with it -- status untouched, nothing
-      // un-reserved (throttle_controller.go:233-236); the first such pod in informer order names the error
-      const std::vector<int64_t> err_rows = selector_error_rows(o);
-      const PodObj* first = nullptr;
-      for (int64_t r : err_rows)
-        if (!std::binary_search(r0, r1, r) && (!first || pods[(size_t)r].seq < first->seq)) first = &pods[(size_t)r];
-      if (first) { errors.emplace_back(todo[q].first, reachable_selector_error(o, first->ns)); continue; }
-      ++reconciled;
-      if (update_status(t, ro, k, q, now)) changed.push_back(o.nn());
-      __int128 after = 0;
-      if (next_override_happens_in(o, now, &after)) requeue.emplace_back(o.nn(), (long long)(after > INT64_MAX ? INT64_MAX : after));
-      // unreserveAffectedPods: every affected pod the informer has observed leaves the reservation cache -- except, for a
-      // Throttle, the finished ones but the last (Q8; "last" is the order of first appearance, as in reconcile_all)
-      auto it = cache[o.kind].by_thr.find(o.nn());
-      if (it == cache[o.kind].by_thr.end()) continue;
-      int64_t last_fin = -1;
-      if (o.kind == KT_KIND_THROTTLE)
-        for (const int64_t* r = r0; r < r1; ++r) {
-          const PodObj& p = pods[(size_t)*r];
-          if (!(pod_flags(p) & KT_POD_NOT_FINISHED) && (last_fin < 0 || p.seq > pods[(size_t)last_fin].seq)) last_fin = *r;
-        }
-      std::vector<std::string> gone;
-      for (auto& pod : it->second) {
-        auto pi = pod_index.find(pod.first);
-        if (pi == pod_index.end() || !std::binary_search(r0, r1, pi->second)) continue;
-        const PodObj& p = pods[(size_t)pi->second];
-        if (o.kind == KT_KIND_THROTTLE && !(pod_flags(p) & KT_POD_NOT_FINISHED) && pi->second != last_fin) continue;
-        gone.push_back(pod.first);
-      }
-      for (auto& g : gone)
-        if (it->second.erase(g)) reservation_changed(t);
+      auto matched = [&](int64_t r) { return std::binary_search(r0, r1, r); };
+      const std::string err = reconcile_throttle(t, matched, selector_error_rows(throttles[t]), r0, r1, st, (int64_t)q, now, rep);
+      if (!err.empty()) rep.errors.emplace_back(todo[q].first, err);
     }
-    Writer w;
-    w.begin_obj().key("reconciled").num(reconciled).key("changed").begin_arr();
-    for (auto& c : changed) w.str(c);
-    w.end_arr().key("requeueAfterNanos").begin_obj();
-    for (auto& r : requeue) w.key(r.first).num(r.second);
-    w.end_obj().key("errors").begin_obj();
-    for (auto& er : errors) w.key(er.first).str(er.second);
-    w.end_obj().key("notFound").begin_arr();
-    for (auto& nf : not_found) w.str(nf);
-    w.end_arr().end_obj();
-    return w.out;
+    return rep.json(true);
   }
 
   // ---- pending pods: one device pass for a batch ----------------------------------------------------------
@@ -1774,73 +1792,78 @@ struct kth_plugin {
     uint8_t admit;
     int Wp;
   };
-  struct PendingResult {
+  struct PendingResult {  // k pending rows: Wp match words, 2 * Wp check-code words and the admit byte each
     std::vector<uint32_t> bitmap, codes;
     std::vector<uint8_t> admit;
     int Wp = 0;
-    RowView row(size_t i) const { return RowView{bitmap.data() + i * (size_t)Wp, codes.data() + i * 2 * (size_t)Wp, admit.empty() ? (uint8_t)1 : admit[i], Wp}; }
+    PendingResult() = default;
+    PendingResult(size_t k, int Wp) : bitmap(k * (size_t)Wp, 0), codes(k * 2 * (size_t)Wp, 0), admit(k, 1), Wp(Wp) {}
+    RowView row(size_t i) const { return RowView{bitmap.data() + i * (size_t)Wp, codes.data() + i * 2 * (size_t)Wp, admit[i], Wp}; }
   };
   // The device's PENDING table = the resident queue rows + `k` scratch rows holding `batch` (pods that are not in the informer
-  // cache).  Brings it up to date with row deltas; a full upload only when a capacity grows or the packing changed.
+  // cache), brought up to date together with the state a PreFilter view reads (sync_state).  Row deltas; a full upload only
+  // when a capacity grows or the packing changed.
   void sync_pending(const std::vector<PodObj>& batch) {
+    sync_state();
     const int L = lim.label_slots, R = lim.n_resources;
     const int64_t k = (int64_t)batch.size();
     int64_t want_q = std::max<int64_t>(64, pend_capacity), want_s = std::max<int64_t>(16, scratch_capacity);
     while (want_q < (int64_t)pend_pod.size()) want_q *= 2;
     while (want_s < k) want_s *= 2;
     if (want_q != pend_capacity || want_s != scratch_capacity) pend_full_upload = true;
-    PodObj tomb;
-    auto queue_pod = [&](int64_t row) -> const PodObj& {
-      const int64_t slot = row < (int64_t)pend_pod.size() ? pend_pod[(size_t)row] : -1;
-      return slot >= 0 ? pods[(size_t)slot] : tomb;
-    };
-    if (pend_full_upload) {
-      const size_t n = (size_t)(want_q + want_s);
+    const bool full = pend_full_upload;
+    const int64_t first_scratch = full ? want_q : pend_capacity;
+    std::vector<int64_t> rows;  // the rows a delta packs (a full upload packs every row)
+    if (!full) {
+      rows.assign(pend_dirty.begin(), pend_dirty.end());
+      const int64_t n_scratch = std::max(k, scratch_used);  // this batch, and what the last one left behind
+      for (int64_t i = 0; i < n_scratch; ++i) rows.push_back(pend_capacity + i);
+    }
+    const size_t n = full ? (size_t)(want_q + want_s) : rows.size();
+    if (n) {
+      PodObj tomb;
+      auto pod_at = [&](int64_t row) -> const PodObj& {
+        if (row >= first_scratch) return row - first_scratch < k ? batch[(size_t)(row - first_scratch)] : tomb;
+        const int64_t slot = row < (int64_t)pend_pod.size() ? pend_pod[(size_t)row] : -1;
+        return slot >= 0 ? pods[(size_t)slot] : tomb;
+      };
       std::vector<int64_t> lab((size_t)L * n), req((size_t)R * n);
       std::vector<uint32_t> present(n), flags(n);
       std::vector<int32_t> nsid(n);
-      for (int64_t i = 0; i < want_q; ++i) pack_pod(queue_pod(i), lab, req, present, flags, nsid, n, (size_t)i);
-      for (int64_t i = 0; i < want_s; ++i) pack_pod(i < k ? batch[(size_t)i] : tomb, lab, req, present, flags, nsid, n, (size_t)(want_q + i));
-      if (namespaces_dirty || throttles_dirty) { sync_all(); sync_status(); sync_reserved(); }  // packing introduced new namespace ids
-      check(kt_upload_pods(ctx, KT_PODS_PENDING, (int64_t)n, lab.data(), req.data(), present.data(), flags.data(), nsid.data()), "kt_upload_pods(pending)");
+      for (size_t i = 0; i < n; ++i) pack_pod(pod_at(full ? (int64_t)i : rows[i]), lab, req, present, flags, nsid, n, i);
+      if (namespaces_dirty || throttles_dirty) sync_state();  // packing introduced new namespace ids
+      if (full)
+        check(kt_upload_pods(ctx, KT_PODS_PENDING, (int64_t)n, lab.data(), req.data(), present.data(), flags.data(), nsid.data()), "kt_upload_pods(pending)");
+      else
+        check(kt_update_pod_rows(ctx, KT_PODS_PENDING, (int64_t)n, rows.data(), lab.data(), req.data(), present.data(), flags.data(), nsid.data()),
+              "kt_update_pod_rows(pending)");
+    }
+    if (full) {
       pend_capacity = want_q;
       scratch_capacity = want_s;
       pend_full_upload = false;
-      pend_dirty.clear();
       queue.valid = false;
-    } else {
-      std::vector<int64_t> rows(pend_dirty.begin(), pend_dirty.end());
-      const int64_t n_scratch = std::max(k, scratch_used);  // this batch, and what the last one left behind
-      for (int64_t i = 0; i < n_scratch; ++i) rows.push_back(pend_capacity + i);
-      const size_t n = rows.size();
-      if (n) {
-        std::vector<int64_t> lab((size_t)L * n), req((size_t)R * n);
-        std::vector<uint32_t> present(n), flags(n);
-        std::vector<int32_t> nsid(n);
-        for (size_t i = 0; i < n; ++i) {
-          const int64_t row = rows[i];
-          pack_pod(row < pend_capacity ? queue_pod(row) : (row - pend_capacity < k ? batch[(size_t)(row - pend_capacity)] : tomb), lab, req, present, flags, nsid, n, i);
-        }
-        if (namespaces_dirty || throttles_dirty) { sync_all(); sync_status(); sync_reserved(); }
-        check(kt_update_pod_rows(ctx, KT_PODS_PENDING, (int64_t)n, rows.data(), lab.data(), req.data(), present.data(), flags.data(), nsid.data()),
-              "kt_update_pod_rows(pending)");
-      }
-      pend_dirty.clear();
     }
+    pend_dirty.clear();
     scratch_used = k;
   }
   // One pass over the PENDING table (queue + scratch rows): PreFilter reads the informer copy of .status; reconcile is a
   // separate event (KT_EVAL_GIVEN_STATUS).  Afterwards the device holds the verdicts of every queue row at this state.
   // (kth_affected_pods asks for skip = 0: the running relation of the same state as well)
   void run_pending_pass(const std::vector<PodObj>& batch, uint32_t extra_flags, uint32_t skip = KT_EVAL_SKIP_RECONCILE) {
-    const bool tables_change = throttles_dirty || namespaces_dirty;
-    sync_all();
-    sync_status();
-    sync_reserved();
-    if (tables_change) queue.valid = false;
     sync_pending(batch);
     if (throttles.empty()) return;
     check(kt_evaluate(ctx, 0, KT_EVAL_GIVEN_STATUS | skip | extra_flags), "kt_evaluate");
+  }
+  // The first k scratch rows as the pass (or kt_admit_queue) that just ran left them.
+  PendingResult scratch_rows(size_t k) {
+    PendingResult out(k, kt_match_words(ctx));
+    if (throttles.empty() || k == 0) return out;
+    std::vector<int64_t> rows(k);
+    for (size_t i = 0; i < k; ++i) rows[i] = pend_capacity + (int64_t)i;
+    check(kt_get_check_rows(ctx, (int64_t)k, rows.data(), out.codes.data(), out.admit.data()), "kt_get_check_rows");
+    check(kt_get_match_rows(ctx, KT_PODS_PENDING, (int64_t)k, rows.data(), out.bitmap.data()), "kt_get_match_rows");
+    return out;
   }
   // Bring the host copy of the queue's verdicts up to date (admit bits, affectedThrottles rows, non-zero check codes).
   void fetch_queue_results() {
@@ -1902,36 +1925,22 @@ struct kth_plugin {
   }
 
   PendingResult check_pending(const std::vector<PodObj>& batch, uint32_t extra_flags) {
-    const size_t k = batch.size();
     run_pending_pass(batch, extra_flags);
-    PendingResult out;
-    out.Wp = kt_match_words(ctx);
-    out.bitmap.assign(k * (size_t)out.Wp, 0);
-    out.codes.assign(k * 2 * (size_t)out.Wp, 0);
-    out.admit.assign(k, 1);
-    if (throttles.empty() || k == 0) return out;
-    std::vector<int64_t> rows(k);
-    for (size_t i = 0; i < k; ++i) rows[i] = pend_capacity + (int64_t)i;
-    check(kt_get_check_rows(ctx, (int64_t)k, rows.data(), out.codes.data(), out.admit.data()), "kt_get_check_rows");
-    check(kt_get_match_rows(ctx, KT_PODS_PENDING, (int64_t)k, rows.data(), out.bitmap.data()), "kt_get_match_rows");
-    return out;
+    return scratch_rows(batch.size());
   }
   // PreFilter of a pod of the resident queue: from the cached verdicts when they are current, else after ONE pass that
   // refreshes the whole queue's.
   PendingResult queue_result(int64_t row) {
     if (!queue_row_current(row)) refresh_queue();
     else ++queue.hits;
-    PendingResult out;
-    out.Wp = queue.Wp;
-    out.bitmap.assign(&queue.bitmap[(size_t)row * (size_t)queue.Wp], &queue.bitmap[(size_t)row * (size_t)queue.Wp] + queue.Wp);
-    out.codes.assign(2 * (size_t)queue.Wp, 0);
-    out.admit.assign(1, queue.admit[(size_t)row]);
+    PendingResult out(1, queue.Wp);
+    std::copy_n(&queue.bitmap[(size_t)row * (size_t)queue.Wp], queue.Wp, out.bitmap.begin());
+    out.admit[0] = queue.admit[(size_t)row];
     auto it = queue.codes.find(row);
     if (it != queue.codes.end())
       for (auto& e : it->second) out.codes[e.first] = e.second;
     return out;
   }
-  std::vector<int> affected(const PendingResult& r, size_t i, int kind) const { return affected(r.row(i), kind); }
   std::vector<int> affected(const RowView& r, int kind) const {  // the set bits of the pod's match row, in column order
     std::vector<int> out;
     const uint32_t* row = r.bitmap;
@@ -1945,20 +1954,12 @@ struct kth_plugin {
   }
   // affectedThrottles / affectedClusterThrottles error paths that never reach the device:
   // an invalid podSelector (MatchesToPod returns the error) and a namespace the informer does not know.
-  std::string controller_error(const PodObj& pod, const PendingResult& r, size_t i, int kind) { return controller_error(pod, r.row(i), kind); }
   std::string controller_error(const PodObj& pod, const RowView& r, int kind) {
     if (kind == KT_KIND_CLUSTERTHROTTLE) {
       const int id = ns_dict.find(pod.ns);
       if (id < 0 || !namespaces[(size_t)id].exists) return "namespace \"" + pod.ns + "\" not found";  // namespaceInformer.Lister().Get (clusterthrottle_controller.go:273-276)
     }
-    if (!broken_valid) {  // the throttles whose podSelector does not convert: usually none, so not a walk over all of them per pod
-      broken.clear();
-      for (size_t t = 0; t < throttles.size(); ++t)
-        if (throttles[t].live && !throttles[t].selector_error().empty()) broken.push_back(t);
-      creation_order(broken);
-      broken_valid = true;
-    }
-    for (size_t t : broken) {
+    for (size_t t : broken_throttles()) {
       const ThrottleObj& o = throttles[t];
       if (!o.live || o.kind != kind || o.throttler_name != name) continue;
       if (kind == KT_KIND_THROTTLE && o.ns != pod.ns) continue;
@@ -2019,7 +2020,6 @@ struct kth_plugin {
     return s;
   }
   // plugin.go:148-215
-  void prefilter_json(Writer& w, const PodObj& pod, const PendingResult& r, size_t i) { prefilter_json(w, pod, r.row(i)); }
   void prefilter_json(Writer& w, const PodObj& pod, const RowView& r) {
     std::vector<int> bucket[2][4], aff[2];
     std::string err;
@@ -2157,11 +2157,6 @@ struct kth_plugin {
       if (pod.pend_row < 0) { scratch_of[i] = (int64_t)batch.size(); batch.push_back(pod); }  // (value copy: the sync may re-pack)
     }
     // the state sync every entry point does (it may void cached verdicts, as anywhere else), then the rows as they are now
-    const bool tables_change = throttles_dirty || namespaces_dirty;
-    sync_all();
-    sync_status();
-    sync_reserved();
-    if (tables_change) queue.valid = false;
     sync_pending(batch);
     std::vector<int64_t> rows, at(n, -1);
     std::vector<PodObj> who;
@@ -2178,18 +2173,14 @@ struct kth_plugin {
       }
     }
     const size_t k = rows.size();
-    PendingResult r;
-    r.Wp = kt_match_words(ctx);
-    r.bitmap.assign(k * (size_t)r.Wp, 0);
-    r.codes.assign(k * 2 * (size_t)r.Wp, 0);
-    r.admit.assign(k, 1);
+    PendingResult r(k, kt_match_words(ctx));
     if (!throttles.empty() && k)  // PreFilter passes isThrottledOnEqual = false
       check(kt_check_pending_rows(ctx, 0, (int64_t)k, rows.data(), r.bitmap.data(), r.codes.data(), r.admit.data()), "kt_check_pending_rows");
     Writer w;
     w.begin_arr();
     for (size_t i = 0; i < n; ++i) {
       if (at[i] < 0) w.begin_obj().key("error").str(err[i]).end_obj();
-      else prefilter_json(w, who[(size_t)at[i]], r, (size_t)at[i]);
+      else prefilter_json(w, who[(size_t)at[i]], r.row((size_t)at[i]));
     }
     w.end_arr();
     return w.out;
@@ -2210,7 +2201,7 @@ struct kth_plugin {
       if (pend_pod[(size_t)row] >= 0 && !queue_row_current(row)) current = false;
     if (!current) refresh_queue();
     else ++queue.hits;
-    if (!broken_valid) { PendingResult none; none.Wp = queue.Wp; none.bitmap.assign((size_t)queue.Wp, 0); none.codes.assign(2 * (size_t)queue.Wp, 0); controller_error(PodObj(), none.row(0), KT_KIND_THROTTLE); }
+    const bool any_broken = !broken_throttles().empty();
     const std::vector<uint32_t> no_codes(2 * (size_t)queue.Wp, 0);
     for (int64_t row = 0; row < n && row < cap; ++row) {
       const int64_t slot = pend_pod[(size_t)row];
@@ -2218,7 +2209,7 @@ struct kth_plugin {
       uint8_t v = queue.admit[(size_t)row] ? 1 : 2;
       const PodObj& pod = pods[(size_t)slot];
       const int nsid = ns_dict.find(pod.ns);
-      if (!broken.empty() || nsid < 0 || !namespaces[(size_t)nsid].exists) {  // the error paths that never reach the device
+      if (any_broken || nsid < 0 || !namespaces[(size_t)nsid].exists) {  // the error paths that never reach the device
         const RowView rv{&queue.bitmap[(size_t)row * (size_t)queue.Wp], no_codes.data(), queue.admit[(size_t)row], queue.Wp};
         if (!controller_error(pod, rv, KT_KIND_THROTTLE).empty() || !controller_error(pod, rv, KT_KIND_CLUSTERTHROTTLE).empty()) v = 3;
       }
@@ -2230,14 +2221,7 @@ struct kth_plugin {
   // ---- queue-ordered admission on the device (kt_admit_queue, csrc/kt_admit.cuh) ------------------------------
   bool admit_queue_on_device_possible(const std::vector<PodObj>& queue) {
     if (throttles.empty() || queue.empty()) return false;
-    if (!broken_valid) {
-      broken.clear();
-      for (size_t t = 0; t < throttles.size(); ++t)
-        if (throttles[t].live && !throttles[t].selector_error().empty()) broken.push_back(t);
-      creation_order(broken);
-      broken_valid = true;
-    }
-    if (!broken.empty()) return false;  // some pod may run into a conversion error: framework.Error, no Reserve
+    if (!broken_throttles().empty()) return false;  // some pod may run into a conversion error: framework.Error, no Reserve
     // Reserve is idempotent per pod (podResourceAmountMap.add overwrites, reserved_resource_amounts.go:131-136): a queue pod that
     // already holds a reservation -- reserved in an earlier cycle and neither bound-and-observed nor unreserved since -- or that
     // stands in the queue twice adds NOTHING when it is admitted again, whereas the device's prefix sums would count its requests
@@ -2259,23 +2243,11 @@ struct kth_plugin {
   }
   std::string admit_queue_on_device(const std::vector<PodObj>& queue) {
     const size_t n = queue.size();
-    sync_all();
-    sync_status();
-    sync_reserved();
     sync_pending(queue);
-    if (namespaces_dirty || throttles_dirty || status_dirty || reserved_dirty) { sync_all(); sync_status(); sync_reserved(); }
     int32_t rounds = 0;
     int64_t admitted_dev = 0;
     check(kt_admit_queue(ctx, pend_capacity, (int64_t)n, 0, &rounds, &admitted_dev), "kt_admit_queue");
-    PendingResult r;
-    r.Wp = kt_match_words(ctx);
-    r.bitmap.assign(n * (size_t)r.Wp, 0);
-    r.codes.assign(n * 2 * (size_t)r.Wp, 0);
-    r.admit.assign(n, 1);
-    std::vector<int64_t> rows(n);
-    for (size_t i = 0; i < n; ++i) rows[i] = pend_capacity + (int64_t)i;
-    check(kt_get_check_rows(ctx, (int64_t)n, rows.data(), r.codes.data(), r.admit.data()), "kt_get_check_rows");
-    check(kt_get_match_rows(ctx, KT_PODS_PENDING, (int64_t)n, rows.data(), r.bitmap.data()), "kt_get_match_rows");
+    const PendingResult r = scratch_rows(n);
     Writer out;
     int admitted = 0;
     std::vector<std::string> results(n);
@@ -2339,18 +2311,18 @@ struct kth_plugin {
           continue;
         }
         Writer w;
-        prefilter_json(w, batch[k], r, k);
+        prefilter_json(w, batch[k], r.row(k));
         results[i] = w.out;
         round_of[i] = rounds;
         bool success = w.out.compare(0, 17, "{\"code\":\"Success\"") == 0;
         if (!success) continue;
         // Reserve (throttle_controller.go:271-292): ResourceAmountOfPod joins the reservation of every affected throttle
         bool reserve_error = false;
-        for (int kind = 0; kind < 2; ++kind) reserve_error = reserve_error || !controller_error(batch[k], r, k, kind).empty();
+        for (int kind = 0; kind < 2; ++kind) reserve_error = reserve_error || !controller_error(batch[k], r.row(k), kind).empty();
         if (reserve_error) continue;
         ++admitted;
         for (int kind = 0; kind < 2; ++kind)
-          for (int t : affected(r, k, kind)) { cache[kind].add(throttles[(size_t)t].nn(), batch[k]); reservation_changed((size_t)t); }
+          for (int t : affected(r.row(k), kind)) { cache[kind].add(throttles[(size_t)t].nn(), batch[k]); reservation_changed((size_t)t); }
         for (size_t w2 = 0; w2 < W; ++w2) dirty[w2] |= row[w2];
       }
       undecided.swap(next);
@@ -2504,11 +2476,7 @@ struct kth_plugin {
   };
   // affectedThrottles of each version (one device call for the distinct (namespace, label set) pairs), as a PendingResult
   PendingResult match_versions(const std::vector<PodObj>& vers) {
-    const bool tables_change = throttles_dirty || namespaces_dirty;
-    sync_all();
-    sync_status();
-    sync_reserved();
-    if (tables_change) queue.valid = false;
+    sync_state();
     const int L = lim.label_slots;
     const size_t k = vers.size();
     std::vector<int64_t> lab((size_t)L * k, KT_LABEL_EMPTY);
@@ -2521,16 +2489,8 @@ struct kth_plugin {
       }
       nsid[i] = ns_id(vers[i].ns);
     }
-    if (namespaces_dirty || throttles_dirty) {  // packing introduced new namespace ids
-      sync_all();
-      sync_status();
-      sync_reserved();
-      queue.valid = false;
-    }
-    PendingResult r;
-    r.Wp = kt_match_words(ctx);
-    r.bitmap.assign(k * (size_t)r.Wp, 0);
-    r.codes.assign(k * 2 * (size_t)r.Wp, 0);
+    if (namespaces_dirty || throttles_dirty) sync_state();  // packing introduced new namespace ids
+    PendingResult r(k, kt_match_words(ctx));
     check(kt_match_pods(ctx, (int64_t)k, lab.data(), nsid.data(), r.bitmap.data()), "kt_match_pods");
     return r;
   }
@@ -2611,7 +2571,7 @@ struct kth_plugin {
           run.push_back(std::move(pe));
         }
       } else if (is_thr) {  // DeleteFunc: isResponsibleFor the object the plugin held
-        auto it = thr_index.find(std::string(tkind == KT_KIND_THROTTLE ? "T:" + ns : "C:") + "/" + nm);
+        auto it = thr_index.find(thr_key(tkind, ns, nm));
         if (it != thr_index.end() && throttles[(size_t)it->second].throttler_name == name) o.enqueue.push_back(throttles[(size_t)it->second].nn());
         delete_throttle(tkind, ns, nm);
       } else if (kind == "Namespace") {
@@ -2640,8 +2600,7 @@ struct kth_plugin {
       apply_namespace(obj);
     } else if (is_thr) {  // AddFunc / UpdateFunc: isResponsibleFor the new object
       apply_throttle(obj, tkind);
-      const std::string ns = tkind == KT_KIND_THROTTLE ? obj["metadata"]["namespace"].str() : "";
-      const ThrottleObj& t = throttles[(size_t)thr_index.at(std::string(tkind == KT_KIND_THROTTLE ? "T:" : "C:") + ns + "/" + obj["metadata"]["name"].str())];
+      const ThrottleObj& t = throttles[(size_t)thr_index.at(thr_key(tkind, obj["metadata"]["namespace"].str(), obj["metadata"]["name"].str()))];
       if (t.throttler_name == name) o.enqueue.push_back(t.nn());
     } else {
       fail("unsupported kind: " + kind);
@@ -2770,7 +2729,7 @@ struct kth_plugin {
       for (auto& kv : st["throttled"]["resourceRequests"].obj) o.st_thr_req[column(kv.first)] = kv.second->boolean(false);
       o.st_used = res_amount(st["used"]);
     }
-    const std::string key = std::string(kind == KT_KIND_THROTTLE ? "T:" : "C:") + o.nn();
+    const std::string key = thr_key(kind, o.ns, o.name);
     auto it = thr_index.find(key);
     if (it == thr_index.end()) {
       o.seq = ++thr_seq;
@@ -2798,8 +2757,7 @@ struct kth_plugin {
     broken_valid = false;
   }
   void delete_throttle(int kind, const std::string& ns, const std::string& tname) {
-    const std::string nn = (kind == KT_KIND_THROTTLE ? ns : std::string()) + "/" + tname;
-    auto it = thr_index.find(std::string(kind == KT_KIND_THROTTLE ? "T:" : "C:") + nn);
+    auto it = thr_index.find(thr_key(kind, ns, tname));
     if (it == thr_index.end()) return;
     // the column can never match or be reconciled again; the next new throttle takes it over
     ThrottleObj& o = throttles[(size_t)it->second];
@@ -2815,9 +2773,9 @@ struct kth_plugin {
   }
 
   std::string status_json(const std::string& ns, const std::string& tname) {
-    auto it = thr_index.find(ns.empty() ? "C:/" + tname : "T:" + ns + "/" + tname);
-    if (it == thr_index.end()) fail("throttle " + ns + "/" + tname + " not found");
-    const ThrottleObj& o = throttles[(size_t)it->second];
+    const int t = find_throttle(ns, tname);
+    if (t < 0) fail("throttle " + ns + "/" + tname + " not found");
+    const ThrottleObj& o = throttles[(size_t)t];
     Writer w;
     w.begin_obj().key("calculatedThreshold").begin_obj().key("threshold");
     amount_json(w, o.st_calc);
@@ -2861,9 +2819,9 @@ struct kth_plugin {
     w.end_obj();
   }
   std::string status_manifest_json(const std::string& ns, const std::string& tname) {
-    auto it = thr_index.find(ns.empty() ? "C:/" + tname : "T:" + ns + "/" + tname);
-    if (it == thr_index.end()) fail("throttle " + ns + "/" + tname + " not found");
-    const ThrottleObj& o = throttles[(size_t)it->second];
+    const int t = find_throttle(ns, tname);
+    if (t < 0) fail("throttle " + ns + "/" + tname + " not found");
+    const ThrottleObj& o = throttles[(size_t)t];
     Writer w;
     w.begin_obj().key("calculatedThreshold").begin_obj().key("threshold");
     amount_manifest(w, o.st_calc, false);
@@ -3104,7 +3062,7 @@ const char* kth_pre_filter(kth_plugin* p, const char* pod_json) {
     p->check_only_names = false;
     kth_plugin::PendingResult r = p->check_pending(batch, 0);  // PreFilter passes isThrottledOnEqual = false
     Writer w;
-    p->prefilter_json(w, batch[0], r, 0);
+    p->prefilter_json(w, batch[0], r.row(0));
     return w.out;
   });
 }
@@ -3192,7 +3150,7 @@ const char* kth_pre_filter_batch(kth_plugin* p, const char* pods_json) {
     kth_plugin::PendingResult r = p->check_pending(batch, 0);
     Writer w;
     w.begin_arr();
-    for (size_t i = 0; i < batch.size(); ++i) p->prefilter_json(w, batch[i], r, i);
+    for (size_t i = 0; i < batch.size(); ++i) p->prefilter_json(w, batch[i], r.row(i));
     w.end_arr();
     return w.out;
   });
