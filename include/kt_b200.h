@@ -290,6 +290,21 @@ int kt_upload_status(kt_ctx* ctx, const kt_status_cols* st);
  * in present[t] iff >=1 pod is reserved on t).  NULL pointers mean "nothing reserved". */
 int kt_set_reserved(kt_ctx* ctx, const int64_t* reserved /*[R][m]*/,
                     const uint32_t* present /*[m]*/, const int64_t* cnt /*[m]*/);
+/* Column deltas of the throttle-side state, for a caller that keeps the snapshot resident: a status echoed back by the informer,
+ * or one Reserve / Unreserve, changes a few columns, and the selector tables do not depend on either.
+ * kt_update_status_rows: the observed status of k listed throttle columns, shaped as kt_get_reconcile_rows fills them ([R][k] /
+ * [k]).  Afterwards every call answers exactly as after a kt_upload_status whose columns equal the previous ones with these k
+ * replaced.  KT_ERR_STATE before kt_upload_status (a partial status over no status has no meaning).
+ * kt_update_reserved_rows: reserved[R][k], present[k], cnt[k] of k listed columns; as kt_set_reserved with those k replaced.
+ * Before any kt_set_reserved (or after kt_set_reserved(NULL, ...)) the other columns are "nothing reserved".
+ * Both: idx entries distinct and in [0, M), k >= 0, no null column when k > 0 (KT_ERR_INVALID otherwise); KT_ERR_STATE before
+ * kt_upload_throttles; k = 0 is a no-op.  One staged copy of the k columns, one scatter launch, one synchronisation (the caller
+ * may reuse its buffers on return); no table compile, no re-upload of the other columns.  The state flags move as the full
+ * calls move them.  Multi-GPU: the throttle columns are replicated, so the call is local, not collective -- every rank must
+ * apply the same updates. */
+int kt_update_status_rows(kt_ctx* ctx, int64_t k, const int32_t* idx, const kt_status_cols* st);
+int kt_update_reserved_rows(kt_ctx* ctx, int64_t k, const int32_t* idx, const int64_t* reserved /*[R][k]*/,
+                            const uint32_t* present /*[k]*/, const int64_t* cnt /*[k]*/);
 
 /* ---- the pass ------------------------------------------------------------------- */
 /* One batched pass: reconcile every throttle (throttle_controller.go:84-133) and check

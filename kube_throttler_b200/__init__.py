@@ -43,7 +43,7 @@ def build(force: bool = False) -> str:
 EXPORTS = [
     "kt_create", "kt_destroy", "kt_last_error", "kt_version", "kt_set_stream", "kt_sync", "kt_enable_timing",
     "kt_enable_trace", "kt_get_trace", "kt_host_alloc", "kt_host_alloc_upload", "kt_host_free", "kt_upload_pods", "kt_upload_pods_compact", "kt_upload_pods_packed", "kt_set_async_uploads", "kt_update_pod_rows", "kt_upload_namespaces",
-    "kt_upload_throttles", "kt_upload_status", "kt_set_reserved", "kt_evaluate", "kt_get_reconcile",
+    "kt_upload_throttles", "kt_upload_status", "kt_set_reserved", "kt_update_status_rows", "kt_update_reserved_rows", "kt_evaluate", "kt_get_reconcile",
     "kt_match_words", "kt_get_match_bitmap", "kt_get_match_rows", "kt_get_match_columns", "kt_get_check_summary", "kt_reconcile_throttles", "kt_get_check", "kt_set_sparse_check", "kt_get_check_sparse", "kt_get_check_rows", "kt_check_pending_rows", "kt_match_pods", "kt_get_changed", "kt_get_reconcile_rows", "kt_step_submit", "kt_step_wait", "kt_admit_queue", "kt_get_timing", "kt_comm_unique_id",
     "kt_comm_init", "kt_comm_destroy", "kt_debug_compile_tables", "kt_debug_set_pass_plan", "kt_debug_get_pass_plan",
     "kt_debug_set_row_order", "kt_debug_get_row_order",
@@ -96,6 +96,8 @@ def lib():
         L.kt_upload_throttles.argtypes = [vp, C.c_int32, C.POINTER(abi.ThrottleCols), C.POINTER(abi.SelectorTable)]
         L.kt_upload_status.argtypes = [vp, C.POINTER(abi.StatusCols)]
         L.kt_set_reserved.argtypes = [vp, vp, vp, vp]
+        L.kt_update_status_rows.argtypes = [vp, C.c_int64, vp, C.POINTER(abi.StatusCols)]
+        L.kt_update_reserved_rows.argtypes = [vp, C.c_int64, vp, vp, vp, vp]
         L.kt_evaluate.argtypes = [vp, C.c_int64, C.c_uint32]
         L.kt_get_reconcile.argtypes = [vp, C.POINTER(abi.ReconcileOut)]
         L.kt_match_words.argtypes = [vp]
@@ -264,6 +266,27 @@ class Engine:
 
     def set_reserved(self, snap: Snapshot):
         self._ck(self._L.kt_set_reserved(self._h, abi.ptr(snap.reserved), abi.ptr(snap.reserved_present), abi.ptr(snap.reserved_cnt)))
+
+    def update_status_rows(self, idx: np.ndarray, status: dict):
+        """kt_update_status_rows: the observed status of the listed throttle columns, replaced in place.  `status` holds the k
+        listed columns, named and shaped like Snapshot.status ([R][k] / [k]); idx entries distinct and in [0, m)."""
+        idx = np.ascontiguousarray(idx, np.int32)
+        k, R = idx.shape[0], self.R
+        cols = dict(calculated=abi._arr(status["calculated"], np.uint8), calc_thr=abi._arr(status["calc_thr"], np.int64, (R, k)),
+                    calc_present=abi._arr(status["calc_present"], np.uint32), calc_cnt=abi._arr(status["calc_cnt"], np.int64),
+                    used=abi._arr(status["used"], np.int64, (R, k)), used_present=abi._arr(status["used_present"], np.uint32),
+                    used_cnt=abi._arr(status["used_cnt"], np.int64), throttled=abi._arr(status["throttled"], np.uint32))
+        st = abi.StatusCols(*(abi.ptr(cols[f]) for f in ("calculated", "calc_thr", "calc_present", "calc_cnt", "used", "used_present", "used_cnt", "throttled")))
+        self._ck(self._L.kt_update_status_rows(self._h, k, abi.ptr(idx), C.byref(st)))
+
+    def update_reserved_rows(self, idx: np.ndarray, reserved: np.ndarray, present: np.ndarray, cnt: np.ndarray):
+        """kt_update_reserved_rows: reserved[R][k], present[k], cnt[k] of the listed throttle columns, replaced in place (the
+        columns never set since the last set_reserved(None) / upload_throttles count as nothing reserved)."""
+        idx = np.ascontiguousarray(idx, np.int32)
+        k = idx.shape[0]
+        reserved = abi._arr(reserved, np.int64, (self.R, k))
+        present, cnt = abi._arr(present, np.uint32), abi._arr(cnt, np.int64)
+        self._ck(self._L.kt_update_reserved_rows(self._h, k, abi.ptr(idx), abi.ptr(reserved), abi.ptr(present), abi.ptr(cnt)))
 
     def upload_snapshot(self, snap: Snapshot):
         """Everything a pass needs, in dependency order."""

@@ -1287,6 +1287,107 @@ int kt_set_reserved(kt_ctx* c, const int64_t* reserved, const uint32_t* present,
   return KT_OK;
 }
 
+// ---- throttle-side column deltas ------------------------------------------------------------------------------------
+namespace {
+// k listed throttle columns: in [0, M) and distinct (a scatter of two values into one column has no defined winner)
+int check_distinct_throttles(kt_ctx* c, const char* call, int64_t k, const int32_t* idx) {
+  if (int rc = check_throttles(c, call, k, idx)) return rc;
+  std::vector<int32_t> s(idx, idx + k);
+  std::sort(s.begin(), s.end());
+  auto d = std::adjacent_find(s.begin(), s.end());
+  if (d != s.end()) return fail(c, KT_ERR_INVALID, "%s: throttle %d listed twice", call, *d);
+  return KT_OK;
+}
+// The listed columns in ONE host-to-device copy: the pieces packed back to back into the pinned call block (each padded to 16
+// bytes), copied into d_call_in.  at[i] is piece i's offset there.
+struct Piece {
+  const void* src;
+  size_t bytes;
+};
+int stage_pieces(kt_ctx* c, std::initializer_list<Piece> pieces, size_t* at) {
+  size_t total = 0, i = 0;
+  for (const Piece& p : pieces) {
+    at[i++] = total;
+    total += (p.bytes + 15) & ~(size_t)15;
+  }
+  KT_CUDA(c, c->h_call.reserve(total));
+  KT_CUDA(c, c->d_call_in.reserve(total + 16));
+  i = 0;
+  for (const Piece& p : pieces) std::memcpy(c->h_call.as<unsigned char>() + at[i++], p.src, p.bytes);
+  KT_CUDA(c, cudaMemcpyAsync(c->d_call_in.p, c->h_call.p, total, cudaMemcpyHostToDevice, c->stream));
+  return KT_OK;
+}
+}  // namespace
+
+int kt_update_status_rows(kt_ctx* c, int64_t k, const int32_t* idx, const kt_status_cols* st) {
+  if (!c) return KT_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(c->mu);
+  if (k < 0) return fail(c, KT_ERR_INVALID, "kt_update_status_rows: k = %lld", (long long)k);
+  if (k > 0 && (!idx || !st || !st->calculated || !st->calc_thr || !st->calc_present || !st->calc_cnt || !st->used || !st->used_present ||
+                !st->used_cnt || !st->throttled))
+    return fail(c, KT_ERR_INVALID, "kt_update_status_rows: null column with k = %lld", (long long)k);
+  if (!c->have_throttles) return fail(c, KT_ERR_STATE, "kt_update_status_rows before kt_upload_throttles");
+  if (!c->have_status) return fail(c, KT_ERR_STATE, "kt_update_status_rows replaces columns of an uploaded status: kt_upload_status first");
+  if (k == 0) return KT_OK;
+  if (int rc = check_distinct_throttles(c, __func__, k, idx)) return rc;
+  int rc = set_device(c);
+  if (rc) return rc;
+  const int R = c->lim.n_resources, M = c->M;
+  const size_t K = (size_t)k, res = (size_t)R * K * 8;
+  size_t at[9];
+  if ((rc = stage_pieces(c, {{idx, K * 4}, {st->calculated, K}, {st->calc_thr, res}, {st->calc_present, K * 4}, {st->calc_cnt, K * 8},
+                             {st->used, res}, {st->used_present, K * 4}, {st->used_cnt, K * 8}, {st->throttled, K * 4}}, at)))
+    return rc;
+  const unsigned char* in = c->d_call_in.as<unsigned char>();
+  StatusScatter src;
+  src.calculated = in + at[1]; src.calc_thr = reinterpret_cast<const int64_t*>(in + at[2]);
+  src.calc_present = reinterpret_cast<const uint32_t*>(in + at[3]); src.calc_cnt = reinterpret_cast<const int64_t*>(in + at[4]);
+  src.used = reinterpret_cast<const int64_t*>(in + at[5]); src.used_present = reinterpret_cast<const uint32_t*>(in + at[6]);
+  src.used_cnt = reinterpret_cast<const int64_t*>(in + at[7]); src.throttled = reinterpret_cast<const uint32_t*>(in + at[8]);
+  k_scatter_status<<<(unsigned)((k + 127) / 128), 128, 0, c->stream>>>(
+      k, reinterpret_cast<const int32_t*>(in + at[0]), R, M, src, c->d_st_calculated.as<uint8_t>(), c->d_st_calc_thr.as<int64_t>(),
+      c->d_st_calc_present.as<uint32_t>(), c->d_st_calc_cnt.as<int64_t>(), c->d_st_used.as<int64_t>(), c->d_st_used_present.as<uint32_t>(),
+      c->d_st_used_cnt.as<int64_t>(), c->d_st_throttled.as<uint32_t>());
+  KT_CUDA(c, cudaGetLastError());
+  KT_CUDA(c, cudaStreamSynchronize(c->stream));  // the caller may reuse its buffers as soon as we return
+  c->evaluated = false;
+  return KT_OK;
+}
+
+int kt_update_reserved_rows(kt_ctx* c, int64_t k, const int32_t* idx, const int64_t* reserved, const uint32_t* present, const int64_t* cnt) {
+  if (!c) return KT_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(c->mu);
+  if (k < 0) return fail(c, KT_ERR_INVALID, "kt_update_reserved_rows: k = %lld", (long long)k);
+  if (k > 0 && (!idx || !reserved || !present || !cnt)) return fail(c, KT_ERR_INVALID, "kt_update_reserved_rows: null column with k = %lld", (long long)k);
+  if (!c->have_throttles) return fail(c, KT_ERR_STATE, "kt_update_reserved_rows before kt_upload_throttles");
+  if (k == 0) return KT_OK;
+  if (int rc = check_distinct_throttles(c, __func__, k, idx)) return rc;
+  int rc = set_device(c);
+  if (rc) return rc;
+  const int R = c->lim.n_resources, M = c->M;
+  const size_t K = (size_t)k;
+  if (!c->have_reserved) {  // nothing reserved so far (or the columns belong to an earlier throttle set): every other column is zero
+    const size_t m = (size_t)M;
+    KT_CUDA(c, c->d_reserved.reserve((size_t)R * m * 8 + 16));
+    KT_CUDA(c, c->d_reserved_present.reserve(m * 4 + 16));
+    KT_CUDA(c, c->d_reserved_cnt.reserve(m * 8 + 16));
+    KT_CUDA(c, cudaMemsetAsync(c->d_reserved.p, 0, (size_t)R * m * 8, c->stream));
+    KT_CUDA(c, cudaMemsetAsync(c->d_reserved_present.p, 0, m * 4, c->stream));
+    KT_CUDA(c, cudaMemsetAsync(c->d_reserved_cnt.p, 0, m * 8, c->stream));
+  }
+  size_t at[4];
+  if ((rc = stage_pieces(c, {{idx, K * 4}, {reserved, (size_t)R * K * 8}, {present, K * 4}, {cnt, K * 8}}, at))) return rc;
+  const unsigned char* in = c->d_call_in.as<unsigned char>();
+  k_scatter_reserved<<<(unsigned)((k + 127) / 128), 128, 0, c->stream>>>(
+      k, reinterpret_cast<const int32_t*>(in + at[0]), R, M, reinterpret_cast<const int64_t*>(in + at[1]), reinterpret_cast<const uint32_t*>(in + at[2]),
+      reinterpret_cast<const int64_t*>(in + at[3]), c->d_reserved.as<int64_t>(), c->d_reserved_present.as<uint32_t>(), c->d_reserved_cnt.as<int64_t>());
+  KT_CUDA(c, cudaGetLastError());
+  KT_CUDA(c, cudaStreamSynchronize(c->stream));  // the caller may reuse its buffers as soon as we return
+  c->have_reserved = true;
+  c->evaluated = false;
+  return KT_OK;
+}
+
 int32_t kt_match_words(const kt_ctx* c) { return c && c->have_throttles ? c->ht.Wp : 0; }
 
 static int evaluate_locked(kt_ctx* c, int64_t now, uint32_t flags);

@@ -34,6 +34,8 @@
 #pragma weak kt_check_pending_rows
 #pragma weak kt_match_pods
 #pragma weak kt_get_check_summary
+#pragma weak kt_update_status_rows    // without them (older engine doubles) sync_status / sync_reserved upload whole tables
+#pragma weak kt_update_reserved_rows
 
 namespace {
 
@@ -533,7 +535,22 @@ struct kth_plugin {
   void creation_order(V& cols_list) const {  // sort a list of throttle columns by creation
     if (thr_reused) std::stable_sort(cols_list.begin(), cols_list.end(), [&](size_t a, size_t b) { return throttles[a].seq < throttles[b].seq; });
   }
+  // status_dirty / reserved_dirty: the next sync uploads every column (the engine holds none, or the columns' layout or scale
+  // changed).  Otherwise the columns listed in status_cols / reserved_cols go alone (kt_update_status_rows / _reserved_rows).
   bool throttles_dirty = true, namespaces_dirty = true, status_dirty = true, reserved_dirty = true;
+  struct ColumnSet {  // throttle columns, each listed once
+    std::vector<size_t> list;
+    std::vector<char> in;
+    void add(size_t t) {
+      if (in.size() <= t) in.resize(t + 1, 0);
+      if (!in[t]) { in[t] = 1; list.push_back(t); }
+    }
+    void clear() {
+      for (size_t t : list) in[t] = 0;
+      list.clear();
+    }
+  } status_cols, reserved_cols;
+  uint64_t col_epoch = 0;  // bumped whenever a resource column is added or changes its scale: every packed column may change
   std::vector<size_t> broken;  // columns of the throttles with a podSelector that does not convert (controller_error)
   bool broken_valid = false;
   const std::vector<size_t>& broken_throttles() {  // usually none, so not a walk over all throttles per pod: built on first need
@@ -578,7 +595,7 @@ struct kth_plugin {
   void throttle_state_changed(size_t t) {  // status or reservations of throttle column t
     if (queue.valid && (t >> 5) < queue.dirty.size()) queue.dirty[t >> 5] |= 1u << (t & 31);
   }
-  void reservation_changed(size_t t) { reserved_dirty = true; throttle_state_changed(t); }
+  void reservation_changed(size_t t) { reserved_cols.add(t); throttle_state_changed(t); }
   bool apply_committed = false;  // kth_apply: the object was stored; whatever fails afterwards must not roll its resource names back
   std::string apply_warning;     // kth_apply: a committed object whose follow-up pass failed
   int max_labels = 0, max_ns_labels = 0;
@@ -590,6 +607,7 @@ struct kth_plugin {
     // refuse BEFORE interning: the object that brought the name is rejected, the plugin stays usable
     if ((int)cols.size() >= KT_MAX_RESOURCES) fail("more than " + std::to_string(KT_MAX_RESOURCES) + " distinct resource names (" + rname + ")");
     c = (int)col_dict.id(rname);
+    ++col_epoch;
     ResourceColumn rc;
     rc.name = rname;
     rc.scale_exp = rname == "cpu" ? -3 : 0;  // milli-cpu, whole units / bytes elsewhere; refined on demand
@@ -611,6 +629,7 @@ struct kth_plugin {
     const int need = kt::quantity_min_exp(q);
     if (need < cols[c].scale_exp) {  // a finer value than the column holds: every row of the column is re-packed
       cols[c].scale_exp = need;
+      ++col_epoch;
       totals_valid = false;  // the running column totals were counted in the coarser unit
       pods_full_upload = pend_full_upload = throttles_dirty = status_dirty = reserved_dirty = true;
     }
@@ -1070,54 +1089,100 @@ struct kth_plugin {
     status_dirty = reserved_dirty = true;  // kt_upload_throttles forgets both
   }
 
-  void sync_status() {
-    if (!status_dirty) return;
-    const int R = lim.n_resources;
-    const size_t m = throttles.size();
-    if (m == 0) { status_dirty = false; return; }
-    std::vector<uint8_t> calculated(m, 0);
-    std::vector<int64_t> calc_thr((size_t)R * m, 0), calc_cnt(m, 0), used((size_t)R * m, 0), used_cnt(m, 0);
-    std::vector<uint32_t> calc_present(m, 0), used_present(m, 0), throttled(m, 0);
-    for (size_t t = 0; t < m; ++t) {
-      const ThrottleObj& o = throttles[t];
-      calculated[t] = o.st_calc_at_set;  // !CalculatedAt.Time.IsZero() (throttle_types.go:129-132)
-      if (o.st_calc.has_counts) { calc_present[t] |= KT_COUNT_BIT; calc_cnt[t] = o.st_calc.pod; }
-      for (auto& kv : o.st_calc.requests) { calc_thr[(size_t)kv.first * m + t] = at_scale(kv.first, kv.second); calc_present[t] |= 1u << kv.first; }
-      if (o.st_used.has_counts) { used_present[t] |= KT_COUNT_BIT; used_cnt[t] = o.st_used.pod; }
-      for (auto& kv : o.st_used.requests) { used[(size_t)kv.first * m + t] = at_scale(kv.first, kv.second); used_present[t] |= 1u << kv.first; }
-      if (o.st_thr_pod) throttled[t] |= KT_COUNT_BIT;
-      for (auto& kv : o.st_thr_req)
-        if (kv.second) throttled[t] |= 1u << kv.first;
+  // Whether the dirty columns go as a delta (the callers check first that no full upload is pending): the engine has the call and
+  // at most half the columns changed.  Past half a delta carries about as many bytes as the whole table; the half itself is a
+  // guess, not a measured break-even point.
+  bool column_delta(const ColumnSet& dirty, bool have_call) const { return have_call && 2 * dirty.list.size() <= throttles.size(); }
+  // The observed status of the listed throttle columns, shaped [R][k] / [k] (k = list.size()).
+  struct StatusColumns {
+    std::vector<uint8_t> calculated;
+    std::vector<int64_t> calc_thr, calc_cnt, used, used_cnt;
+    std::vector<uint32_t> calc_present, used_present, throttled;
+    kt_status_cols cols() const {
+      return kt_status_cols{calculated.data(), calc_thr.data(), calc_present.data(), calc_cnt.data(), used.data(), used_present.data(), used_cnt.data(), throttled.data()};
     }
-    kt_status_cols sc{calculated.data(), calc_thr.data(), calc_present.data(), calc_cnt.data(), used.data(), used_present.data(), used_cnt.data(), throttled.data()};
-    check(kt_upload_status(ctx, &sc), "kt_upload_status");
+  };
+  template <class List>
+  StatusColumns status_columns(const List& list) const {
+    const int R = lim.n_resources;
+    const size_t k = list.size();
+    StatusColumns sc;
+    sc.calculated.assign(k, 0);
+    sc.calc_thr.assign((size_t)R * k, 0); sc.calc_cnt.assign(k, 0); sc.used.assign((size_t)R * k, 0); sc.used_cnt.assign(k, 0);
+    sc.calc_present.assign(k, 0); sc.used_present.assign(k, 0); sc.throttled.assign(k, 0);
+    for (size_t i = 0; i < k; ++i) {
+      const ThrottleObj& o = throttles[list[i]];
+      sc.calculated[i] = o.st_calc_at_set;  // !CalculatedAt.Time.IsZero() (throttle_types.go:129-132)
+      if (o.st_calc.has_counts) { sc.calc_present[i] |= KT_COUNT_BIT; sc.calc_cnt[i] = o.st_calc.pod; }
+      for (auto& kv : o.st_calc.requests) { sc.calc_thr[(size_t)kv.first * k + i] = at_scale(kv.first, kv.second); sc.calc_present[i] |= 1u << kv.first; }
+      if (o.st_used.has_counts) { sc.used_present[i] |= KT_COUNT_BIT; sc.used_cnt[i] = o.st_used.pod; }
+      for (auto& kv : o.st_used.requests) { sc.used[(size_t)kv.first * k + i] = at_scale(kv.first, kv.second); sc.used_present[i] |= 1u << kv.first; }
+      if (o.st_thr_pod) sc.throttled[i] |= KT_COUNT_BIT;
+      for (auto& kv : o.st_thr_req)
+        if (kv.second) sc.throttled[i] |= 1u << kv.first;
+    }
+    return sc;
+  }
+  struct AllColumns {  // 0 .. m-1 as a list
+    size_t m;
+    size_t size() const { return m; }
+    size_t operator[](size_t i) const { return i; }
+  };
+  void sync_status() {
+    const size_t m = throttles.size();
+    if (m > 0 && (status_dirty || (!status_cols.list.empty() && !column_delta(status_cols, kt_update_status_rows != nullptr)))) {
+      const StatusColumns sc = status_columns(AllColumns{m});
+      const kt_status_cols c = sc.cols();
+      check(kt_upload_status(ctx, &c), "kt_upload_status");
+    } else if (m > 0 && !status_cols.list.empty()) {
+      const StatusColumns sc = status_columns(status_cols.list);
+      const kt_status_cols c = sc.cols();
+      const std::vector<int32_t> idx(status_cols.list.begin(), status_cols.list.end());
+      check(kt_update_status_rows(ctx, (int64_t)idx.size(), idx.data(), &c), "kt_update_status_rows");
+    }
     status_dirty = false;
+    status_cols.clear();
   }
 
-  void sync_reserved() {
-    if (!reserved_dirty) return;
+  // reservedResourceAmounts.reservedResourceAmount(nn) of the listed throttle columns, re-summed from the reservation cache,
+  // shaped [R][k] / [k]; returns whether any of them holds a reservation.
+  template <class List>
+  bool reserved_columns(const List& list, std::vector<int64_t>& reserved, std::vector<uint32_t>& present, std::vector<int64_t>& cnt) const {
     const int R = lim.n_resources;
-    const size_t m = throttles.size();
-    if (m == 0) { reserved_dirty = false; return; }
-    std::vector<int64_t> reserved((size_t)R * m, 0), cnt(m, 0);
-    std::vector<uint32_t> present(m, 0);
+    const size_t k = list.size();
+    reserved.assign((size_t)R * k, 0);
+    present.assign(k, 0);
+    cnt.assign(k, 0);
     bool any = false;
-    for (size_t t = 0; t < m; ++t) {
-      const ThrottleObj& o = throttles[t];
+    for (size_t i = 0; i < k; ++i) {
+      const ThrottleObj& o = throttles[list[i]];
       auto it = cache[o.kind].by_thr.find(o.nn());
       if (it == cache[o.kind].by_thr.end() || it->second.empty()) continue;
       any = true;
-      present[t] |= KT_COUNT_BIT;  // every reserved ResourceAmountOfPod carries Counts{Pod: 1}
-      cnt[t] = (int64_t)it->second.size();
+      present[i] |= KT_COUNT_BIT;  // every reserved ResourceAmountOfPod carries Counts{Pod: 1}
+      cnt[i] = (int64_t)it->second.size();
       for (auto& pod : it->second)
         for (auto& kv : pod.second) {
-          reserved[(size_t)kv.first * m + t] += at_scale(kv.first, kv.second);
-          present[t] |= 1u << kv.first;
+          reserved[(size_t)kv.first * k + i] += at_scale(kv.first, kv.second);
+          present[i] |= 1u << kv.first;
         }
     }
-    if (any) check(kt_set_reserved(ctx, reserved.data(), present.data(), cnt.data()), "kt_set_reserved");
-    else check(kt_set_reserved(ctx, nullptr, nullptr, nullptr), "kt_set_reserved");
+    return any;
+  }
+  void sync_reserved() {
+    const size_t m = throttles.size();
+    std::vector<int64_t> reserved, cnt;
+    std::vector<uint32_t> present;
+    if (m > 0 && (reserved_dirty || (!reserved_cols.list.empty() && !column_delta(reserved_cols, kt_update_reserved_rows != nullptr)))) {
+      if (reserved_columns(AllColumns{m}, reserved, present, cnt)) check(kt_set_reserved(ctx, reserved.data(), present.data(), cnt.data()), "kt_set_reserved");
+      else check(kt_set_reserved(ctx, nullptr, nullptr, nullptr), "kt_set_reserved");
+    } else if (m > 0 && !reserved_cols.list.empty()) {  // only the columns whose reservations changed are summed again
+      reserved_columns(reserved_cols.list, reserved, present, cnt);
+      const std::vector<int32_t> idx(reserved_cols.list.begin(), reserved_cols.list.end());
+      check(kt_update_reserved_rows(ctx, (int64_t)idx.size(), idx.data(), reserved.data(), present.data(), cnt.data()), "kt_update_reserved_rows");
+    }
     reserved_dirty = false;
+    reserved_cols.clear();
   }
   // What the selectors mention goes into the label dictionaries BEFORE any row is packed; rows that carry newly mentioned keys or
   // values (they were packed as "invisible" / "some other value") are packed again.
@@ -1418,7 +1483,7 @@ struct kth_plugin {
     o.metrics_pending = true;  // both branches of the status comparison record (throttle_controller.go:159,187); see record_metrics
     if (status_changed) {
       throttle_state_changed(t);  // PreFilter reads this status: cached verdicts of the pods it affects are void
-      status_dirty = true;
+      status_cols.add(t);
     }
     return status_changed;
   }
@@ -2683,7 +2748,30 @@ struct kth_plugin {
     }
     namespaces_dirty = true;
   }
+  // Everything of two throttles of one key that the compiled tables and the per-column spec on the device are made of.
+  static bool same_selector(const CompiledSelector& a, const CompiledSelector& b) {
+    if (a.error != b.error || a.reqs.size() != b.reqs.size()) return false;
+    for (size_t i = 0; i < a.reqs.size(); ++i)
+      if (a.reqs[i].key != b.reqs[i].key || a.reqs[i].op != b.reqs[i].op || a.reqs[i].values != b.reqs[i].values) return false;
+    return true;
+  }
+  static bool same_spec(const ThrottleObj& a, const ThrottleObj& b) {
+    if (a.kind != b.kind || a.ns != b.ns || a.throttler_name != b.throttler_name || !amount_equal(a.threshold, b.threshold)) return false;
+    if (a.overrides.size() != b.overrides.size() || a.terms.size() != b.terms.size()) return false;
+    for (size_t i = 0; i < a.overrides.size(); ++i)
+      if (a.overrides[i].begin != b.overrides[i].begin || a.overrides[i].end != b.overrides[i].end || !amount_equal(a.overrides[i].threshold, b.overrides[i].threshold))
+        return false;
+    for (size_t i = 0; i < a.terms.size(); ++i)
+      if (!same_selector(a.terms[i].pod_sel, b.terms[i].pod_sel) || !same_selector(a.terms[i].ns_sel, b.terms[i].ns_sel)) return false;
+    return true;
+  }
+  // apiequality.Semantic.DeepEqual on two ThrottleStatus values (empty maps are nil maps)
+  static bool same_status(const ThrottleObj& a, const ThrottleObj& b) {
+    return amount_equal(a.st_calc, b.st_calc) && a.st_calc_at_set == b.st_calc_at_set && a.st_calc_at == b.st_calc_at && a.st_messages == b.st_messages &&
+           a.st_thr_pod == b.st_thr_pod && a.st_thr_req == b.st_thr_req && amount_equal(a.st_used, b.st_used);
+  }
   void apply_throttle(const Node& v, int kind) {
+    const uint64_t epoch = col_epoch;  // a new resource name or a finer scale re-packs every column
     ThrottleObj o;
     o.kind = kind;
     const Node& md = v["metadata"];
@@ -2751,7 +2839,18 @@ struct kth_plugin {
         o.st_calc = old.st_calc; o.st_calc_at_set = old.st_calc_at_set; o.st_calc_at = old.st_calc_at; o.st_messages = old.st_messages;
         o.st_thr_pod = old.st_thr_pod; o.st_thr_req = old.st_thr_req; o.st_thr_req_nil = old.st_thr_req_nil; o.st_used = old.st_used;
       }
+      // The same spec (a status echoed back by the informer after reconcile's UpdateStatus, or written by another replica): the
+      // tables and the spec columns stay; only this column's status is sent again, and only the cached verdicts of the pods this
+      // throttle affects are void.
+      const bool spec_kept = epoch == col_epoch && same_spec(old, o), status_kept = same_status(old, o);
       old = std::move(o);
+      if (spec_kept) {
+        if (!status_kept) {
+          status_cols.add((size_t)it->second);
+          throttle_state_changed((size_t)it->second);
+        }
+        return;
+      }
     }
     throttles_dirty = status_dirty = reserved_dirty = true;
     broken_valid = false;

@@ -2126,6 +2126,40 @@ __global__ void __launch_bounds__(128) k_gather_status(int64_t k, const int32_t*
   dst.calc_present[i] = src.calc_present[t];
   dst.override_active[i] = src.override_active[t];
 }
+// Column deltas of the throttle-side state (kt_update_status_rows / kt_update_reserved_rows): column i of k staged columns ->
+// column idx[i] of the M resident ones.  The idx are distinct (checked on the host), so no two lanes write one column.
+struct StatusScatter {
+  const uint8_t* calculated; const int64_t* calc_thr; const uint32_t* calc_present; const int64_t* calc_cnt;
+  const int64_t* used; const uint32_t* used_present; const int64_t* used_cnt; const uint32_t* throttled;
+};
+__global__ void __launch_bounds__(128) k_scatter_status(int64_t k, const int32_t* __restrict__ idx, int R, int M, const StatusScatter src,
+                                                        uint8_t* calculated, int64_t* calc_thr, uint32_t* calc_present, int64_t* calc_cnt,
+                                                        int64_t* used, uint32_t* used_present, int64_t* used_cnt, uint32_t* throttled) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= k) return;
+  const int t = idx[i];
+  for (int r = 0; r < R; ++r) {
+    calc_thr[(size_t)r * M + t] = src.calc_thr[(size_t)r * k + i];
+    used[(size_t)r * M + t] = src.used[(size_t)r * k + i];
+  }
+  calculated[t] = src.calculated[i];
+  calc_present[t] = src.calc_present[i];
+  calc_cnt[t] = src.calc_cnt[i];
+  used_present[t] = src.used_present[i];
+  used_cnt[t] = src.used_cnt[i];
+  throttled[t] = src.throttled[i];
+}
+__global__ void __launch_bounds__(128) k_scatter_reserved(int64_t k, const int32_t* __restrict__ idx, int R, int M, const int64_t* __restrict__ src_res,
+                                                          const uint32_t* __restrict__ src_present, const int64_t* __restrict__ src_cnt,
+                                                          int64_t* reserved, uint32_t* present, int64_t* cnt) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= k) return;
+  const int t = idx[i];
+  for (int r = 0; r < R; ++r) reserved[(size_t)r * M + t] = src_res[(size_t)r * k + i];
+  present[t] = src_present[i];
+  cnt[t] = src_cnt[i];
+}
+
 __global__ void __launch_bounds__(256) k_gather_bytes(int64_t k, const int64_t* __restrict__ rows, const unsigned char* __restrict__ src, unsigned char* __restrict__ out) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < k) out[i] = src[rows[i]];
