@@ -447,6 +447,22 @@ int kt_check_pending_rows(kt_ctx* ctx, uint32_t flags, int64_t k, const int64_t*
  * (single GPU only). */
 int kt_match_pods(kt_ctx* ctx, int64_t k, const int64_t* labels /*[L][k]*/, const int32_t* ns_id /*[k]*/,
                   uint32_t* words /*[k][words_per_row]*/);
+/* PreFilter of k pods that live only in this call (plugin.go:148-215): the manifest of a PreFilter, Reserve or Unreserve, checked
+ * against the tables, observed status and reservations as they are now, with no pass over the pending table.  Entry i is bit
+ * for bit what kt_evaluate(ctx, 0, KT_EVAL_GIVEN_STATUS | KT_EVAL_SKIP_RECONCILE | flags) followed by
+ * kt_get_match_rows(KT_PODS_PENDING) (words) and kt_get_check_rows (codes, admit) would deliver for a pending row holding
+ * labels[.][i], req[.][i], present[i] and ns_id[i] -- columns laid out as in kt_upload_pods / kt_update_pod_rows: a
+ * KT_TERM_POD_INVALID term switches the later terms off, only the non-zero present requests are compared (Q5), requests may be
+ * negative, and a namespace id the tables do not cover gives an all-zero row with admit = 1.  The pass reads no flags of a
+ * pending row (they matter to the running rows only), so the call takes none.  flags is 0 or KT_EVAL_ON_EQUAL
+ * (KT_ERR_INVALID otherwise); k = 0 is valid; KT_ERR_INVALID for k < 0 or a null input column with k > 0; any output may be NULL.
+ * Needs kt_upload_throttles and kt_upload_status (KT_ERR_STATE before either) and no pod rows at all.  It reads no resident pod
+ * row and writes nothing another call reads (every getter answers as before it, and one that fails before kt_evaluate still
+ * fails).  Value domain: kt_evaluate's.  One staged copy in, two launches (pre-records, check), one copy out, one
+ * synchronisation.  KT_ERR_STATE with a communicator (single GPU only). */
+int kt_check_pods(kt_ctx* ctx, uint32_t flags, int64_t k, const int64_t* labels /*[L][k]*/, const int64_t* req /*[R][k]*/,
+                  const uint32_t* present /*[k]*/, const int32_t* ns_id /*[k]*/, uint32_t* words /*[k][words_per_row] or NULL*/,
+                  uint32_t* codes /*[k][2*words_per_row] or NULL*/, uint8_t* admit /*[k] or NULL*/);
 
 /* Device-side status diff (replaces the apiequality.Semantic.DeepEqual(thr.Status, *newStatus) of every reconcile,
  * throttle_controller.go:157 / clusterthrottle_controller.go:160): when an observed status is uploaded (kt_upload_status) every

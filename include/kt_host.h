@@ -115,9 +115,13 @@ const char* kth_get_status_manifest(kth_plugin* p, const char* ns, const char* n
 /* PreFilter(ctx, state, pod) -- plugin.go:148-215.
  * {"code":"Success"|"UnschedulableAndUnresolvable"|"Error","reasons":[...],"event":{...}?,
  *  "throttle":{"active":[..],"insufficient":[..],"podRequestsExceedsThreshold":[..],"affected":[..]},
- *  "clusterthrottle":{...}}                       reasons are in the reference's fixed order (Q10). */
+ *  "clusterthrottle":{...}}                       reasons are in the reference's fixed order (Q10).
+ * Cost: after the state sync every entry point does, ONE device call (kt_check_pods) that evaluates the words of the pod's own
+ * namespace -- it grows with the throttles that namespace can reach, not with the length of the resident scheduling queue; no
+ * pod row is uploaded and no pass runs.  (Linked against an engine without kt_check_pods, the pod takes a scratch row behind
+ * the queue and one pass over both.) */
 const char* kth_pre_filter(kth_plugin* p, const char* pod_json);
-/* The same for a whole scheduling queue in ONE device pass: pods_json is a JSON array of pods, the
+/* The same for a whole scheduling queue in ONE device call: pods_json is a JSON array of pods, the
  * result a JSON array of PreFilter results (each pod checked against the same snapshot, independently). */
 const char* kth_pre_filter_batch(kth_plugin* p, const char* pods_json);
 
@@ -163,10 +167,12 @@ const char* kth_queue_stats(kth_plugin* p);
  * checked against, plugin.go:148-238) -- but in as few device passes as the conflicts between the pods allow: a pass
  * decides every undecided pod none of whose affected throttles was reserved on earlier in the same pass.
  * {"rounds":k,"admitted":n,"results":[{"pod":"ns/name","round":i,"preFilter":{...as kth_pre_filter...}}...]} in queue order;
- * the admitted pods stay reserved (kth_unreserve / a reconcile that observes them bound releases them). */
+ * the admitted pods stay reserved (kth_unreserve / a reconcile that observes them bound releases them).  Each round of the
+ * host-orchestrated form is one kt_check_pods call over the round's undecided pods. */
 const char* kth_admit_queue(kth_plugin* p, const char* pods_json);
 
-/* Reserve / Unreserve -- plugin.go:217-257: {"code":"Success"} or {"code":"Error","reasons":[...]}. */
+/* Reserve / Unreserve -- plugin.go:217-257: {"code":"Success"} or {"code":"Error","reasons":[...]}.  The pod's affected
+ * throttles come from one kt_check_pods call, as for kth_pre_filter: the cost follows the pod's namespace, not the queue. */
 const char* kth_reserve(kth_plugin* p, const char* pod_json);
 const char* kth_unreserve(kth_plugin* p, const char* pod_json);
 /* reservedResourceAmount(nn) of one controller's cache (kind 0 = Throttle, 1 = ClusterThrottle):

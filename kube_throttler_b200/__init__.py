@@ -44,7 +44,7 @@ EXPORTS = [
     "kt_create", "kt_destroy", "kt_last_error", "kt_version", "kt_set_stream", "kt_sync", "kt_enable_timing",
     "kt_enable_trace", "kt_get_trace", "kt_host_alloc", "kt_host_alloc_upload", "kt_host_free", "kt_upload_pods", "kt_upload_pods_compact", "kt_upload_pods_packed", "kt_set_async_uploads", "kt_update_pod_rows", "kt_upload_namespaces",
     "kt_upload_throttles", "kt_upload_status", "kt_set_reserved", "kt_update_status_rows", "kt_update_reserved_rows", "kt_evaluate", "kt_get_reconcile",
-    "kt_match_words", "kt_get_match_bitmap", "kt_get_match_rows", "kt_get_match_columns", "kt_get_check_summary", "kt_reconcile_throttles", "kt_get_check", "kt_set_sparse_check", "kt_get_check_sparse", "kt_get_check_rows", "kt_check_pending_rows", "kt_match_pods", "kt_get_changed", "kt_get_reconcile_rows", "kt_step_submit", "kt_step_wait", "kt_admit_queue", "kt_get_timing", "kt_comm_unique_id",
+    "kt_match_words", "kt_get_match_bitmap", "kt_get_match_rows", "kt_get_match_columns", "kt_get_check_summary", "kt_reconcile_throttles", "kt_get_check", "kt_set_sparse_check", "kt_get_check_sparse", "kt_get_check_rows", "kt_check_pending_rows", "kt_match_pods", "kt_check_pods", "kt_get_changed", "kt_get_reconcile_rows", "kt_step_submit", "kt_step_wait", "kt_admit_queue", "kt_get_timing", "kt_comm_unique_id",
     "kt_comm_init", "kt_comm_destroy", "kt_debug_compile_tables", "kt_debug_set_pass_plan", "kt_debug_get_pass_plan",
     "kt_debug_set_row_order", "kt_debug_get_row_order",
 ]
@@ -89,6 +89,7 @@ def lib():
         L.kt_get_match_rows.argtypes = [vp, C.c_int, C.c_int64, vp, vp]
         L.kt_check_pending_rows.argtypes = [vp, C.c_uint32, C.c_int64, vp, vp, vp, vp]
         L.kt_match_pods.argtypes = [vp, C.c_int64, vp, vp, vp]
+        L.kt_check_pods.argtypes = [vp, C.c_uint32, C.c_int64, vp, vp, vp, vp, vp, vp, vp]
         L.kt_get_changed.argtypes = [vp, vp, C.c_int64, C.POINTER(C.c_int64), vp]
         L.kt_get_reconcile_rows.argtypes = [vp, C.c_int64, vp, C.POINTER(abi.ReconcileOut)]
         L.kt_update_pod_rows.argtypes = [vp, C.c_int, C.c_int64, vp, vp, vp, vp, vp, vp]
@@ -419,6 +420,25 @@ class Engine:
         words = np.zeros((k, self.words_per_row), np.uint32)
         self._ck(self._L.kt_match_pods(self._h, k, abi.ptr(labels), abi.ptr(ns_id), abi.ptr(words)))
         return words
+
+    def check_pods(self, labels, req, present, ns_id, on_equal: bool = False):
+        """PreFilter of k pods given by value (label codes [L][k], requests [R][k], presence bits [k], namespace ids [k]: the
+        columns of upload_pods without the flags, which the pass never reads for a pending row), checked against the tables,
+        observed status and reservations as they are now, with no pending row read: (words[k][W], codes[k][2W], admit[k]) --
+        what check_pending_rows returns for pending rows holding the same values."""
+        labels = np.ascontiguousarray(labels, np.int64).reshape(self.Lslots, -1)
+        ns_id = np.ascontiguousarray(ns_id, np.int32)
+        k = ns_id.shape[0]
+        req = np.ascontiguousarray(req, np.int64).reshape(self.R, -1)
+        present = np.ascontiguousarray(present, np.uint32)
+        if labels.shape[1] != k or req.shape[1] != k or present.shape[0] != k:
+            raise ValueError(f"column lengths differ: labels {labels.shape[1]}, req {req.shape[1]}, present {present.shape[0]}, ns_id {k}")
+        W = self.words_per_row
+        words, codes, admit = np.zeros((k, W), np.uint32), np.zeros((k, 2 * W), np.uint32), np.zeros(k, np.uint8)
+        flags = abi.EVAL_ON_EQUAL if on_equal else 0
+        self._ck(self._L.kt_check_pods(self._h, flags, k, abi.ptr(labels), abi.ptr(req), abi.ptr(present), abi.ptr(ns_id),
+                                       abi.ptr(words), abi.ptr(codes), abi.ptr(admit)))
+        return words, codes, admit
 
     def match_rows(self, kind: int, rows: np.ndarray) -> np.ndarray:
         """words[k][words_per_row]: the match bitmap rows of the listed rows of a kind, gathered on the device."""

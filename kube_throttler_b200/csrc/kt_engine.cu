@@ -1790,6 +1790,27 @@ int kt_get_reconcile_rows(kt_ctx* c, int64_t k, const int32_t* idx, const kt_rec
 }
 
 // ---- PreFilter for k listed pending rows (kt_keyed.cuh) -------------------------------------------------------------
+// The pre-records of every throttle into d_chk_pre: the pass's prep half, GIVEN_STATUS (no clock is read).
+int rows_prep(kt_ctx* c, uint32_t eval_flags) {
+  const int M = c->M, R = c->lim.n_resources;
+  if (M == 0) return KT_OK;
+  KT_CUDA(c, c->d_chk_pre.reserve((size_t)M * pre_record_bytes(R) + 16));
+  int G = 1;
+  while (G < R + 1) G <<= 1;
+  const long long lanes = (long long)M * G;
+  k_rows_prep<<<(unsigned)((lanes + 127) / 128), 128, 0, c->stream>>>(throttle_view(c), M, R, G, eval_flags, c->d_chk_pre.as<unsigned char>());
+  KT_CUDA(c, cudaGetLastError());
+  return KT_OK;
+}
+// The block the keyed checks fetch from: admit[k] (padded to 16 B) | codes[k][2 Wp] | words[k][Wp], zeroed on the device so that
+// every word outside a pod's namespace list reads 0; `fetch` is the prefix that holds the outputs the caller asked for.
+struct CheckBlock {
+  size_t adm_bytes, code_bytes, word_bytes, fetch;
+  CheckBlock(int64_t k, int Wp, bool words, bool codes)
+      : adm_bytes(((size_t)k + 15) & ~(size_t)15), code_bytes((size_t)k * 2 * Wp * 4), word_bytes((size_t)k * Wp * 4),
+        fetch(words ? adm_bytes + code_bytes + word_bytes : codes ? adm_bytes + code_bytes : adm_bytes) {}
+  size_t bytes() const { return adm_bytes + code_bytes + word_bytes; }
+};
 int kt_check_pending_rows(kt_ctx* c, uint32_t flags, int64_t k, const int64_t* rows, uint32_t* words, uint32_t* codes, uint8_t* admit) {
   if (!c || k < 0 || (k > 0 && !rows)) return KT_ERR_INVALID;
   std::lock_guard<std::mutex> lk(c->mu);
@@ -1803,24 +1824,15 @@ int kt_check_pending_rows(kt_ctx* c, uint32_t flags, int64_t k, const int64_t* r
   int rc = set_device(c);
   if (rc) return rc;
   if ((rc = ensure_roff(c, pend))) return rc;  // rows or tables changed since the offsets were translated (what the next pass does first)
-  const int M = c->M, R = c->lim.n_resources, Wp = c->ht.Wp;
+  const int R = c->lim.n_resources, Wp = c->ht.Wp;
   const uint32_t eval_flags = KT_EVAL_GIVEN_STATUS | KT_EVAL_SKIP_RECONCILE | flags;
-  // the output block: admit[k] (padded to 16 B) | codes[k][2 Wp] | words[k][Wp] -- one copy fetches the prefix the caller asked for
-  const size_t adm_bytes = ((size_t)k + 15) & ~(size_t)15, code_bytes = (size_t)k * 2 * Wp * 4, word_bytes = (size_t)k * Wp * 4;
-  const size_t out_bytes = adm_bytes + code_bytes + word_bytes;
-  const size_t fetch = words ? out_bytes : codes ? adm_bytes + code_bytes : adm_bytes;
+  const CheckBlock blk(k, Wp, words, codes);
+  const size_t adm_bytes = blk.adm_bytes, code_bytes = blk.code_bytes, word_bytes = blk.word_bytes;
   if ((rc = upload(c, c->d_call_in, rows, (size_t)k))) return rc;
-  KT_CUDA(c, c->d_call_out.reserve(out_bytes + 16));
-  KT_CUDA(c, c->h_call.reserve(fetch));
-  KT_CUDA(c, cudaMemsetAsync(c->d_call_out.p, 0, out_bytes, c->stream));
-  if (M > 0) {  // the pre-records of every throttle (the pass's prep half, GIVEN_STATUS: no clock is read)
-    KT_CUDA(c, c->d_chk_pre.reserve((size_t)M * pre_record_bytes(R) + 16));
-    int G = 1;
-    while (G < R + 1) G <<= 1;
-    const long long lanes = (long long)M * G;
-    k_rows_prep<<<(unsigned)((lanes + 127) / 128), 128, 0, c->stream>>>(throttle_view(c), M, R, G, eval_flags, c->d_chk_pre.as<unsigned char>());
-    KT_CUDA(c, cudaGetLastError());
-  }
+  KT_CUDA(c, c->d_call_out.reserve(blk.bytes() + 16));
+  KT_CUDA(c, c->h_call.reserve(blk.fetch));
+  KT_CUDA(c, cudaMemsetAsync(c->d_call_out.p, 0, blk.bytes(), c->stream));
+  if ((rc = rows_prep(c, eval_flags))) return rc;
   unsigned char* ob = c->d_call_out.as<unsigned char>();
   RowsArgs a{};
   a.pods = pod_view(pend);
@@ -1835,12 +1847,65 @@ int kt_check_pending_rows(kt_ctx* c, uint32_t flags, int64_t k, const int64_t* r
   KT_CUDA(c, with_variant(c, true, [&](auto tpc, auto b, auto, auto reg) {
     return launch(c, k_check_rows<tpc, b, reg>, (unsigned)((k + kRowsTile - 1) / kRowsTile), kRowsTile, rows_smem_bytes(a.L, R, reg), false, a);
   }));
-  KT_CUDA(c, cudaMemcpyAsync(c->h_call.p, ob, fetch, cudaMemcpyDeviceToHost, c->stream));
+  KT_CUDA(c, cudaMemcpyAsync(c->h_call.p, ob, blk.fetch, cudaMemcpyDeviceToHost, c->stream));
   KT_CUDA(c, cudaStreamSynchronize(c->stream));
   const unsigned char* hb = c->h_call.as<unsigned char>();
   if (admit) std::memcpy(admit, hb, (size_t)k);
   if (codes) std::memcpy(codes, hb + adm_bytes, code_bytes);
   if (words) std::memcpy(words, hb + adm_bytes + code_bytes, word_bytes);
+  return KT_OK;
+}
+
+// ---- PreFilter of k pods given by value (kt_keyed.cuh) ----------------------------------------------------------------
+int kt_check_pods(kt_ctx* c, uint32_t flags, int64_t k, const int64_t* labels, const int64_t* req, const uint32_t* present, const int32_t* ns_id,
+                  uint32_t* words, uint32_t* codes, uint8_t* admit) {
+  if (!c || k < 0) return KT_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(c->mu);
+  const int L = c->lim.label_slots, R = c->lim.n_resources;
+  if (k > 0 && (!labels || !req || !present || !ns_id)) return fail(c, KT_ERR_INVALID, "kt_check_pods: null input column with k = %lld", (long long)k);
+  if (flags & ~KT_EVAL_ON_EQUAL) return fail(c, KT_ERR_INVALID, "kt_check_pods: flags must be 0 or KT_EVAL_ON_EQUAL, not %u", flags);
+  if (int rc = check_single_gpu(c, __func__)) return rc;
+  if (!c->have_throttles) return fail(c, KT_ERR_STATE, "kt_check_pods before kt_upload_throttles");
+  if (!c->have_status) return fail(c, KT_ERR_STATE, "kt_check_pods checks against the observed status: kt_upload_status first");
+  if (k == 0) return KT_OK;
+  int rc = set_device(c);
+  if (rc) return rc;
+  const int Wp = c->ht.Wp;
+  // the inputs in one copy: labels [L][k] | req [R][k] | present [k] | ns [k]
+  const size_t lab_bytes = (size_t)L * k * 8, req_bytes = (size_t)R * k * 8;
+  std::vector<unsigned char> hin(lab_bytes + req_bytes + (size_t)k * 8);
+  std::memcpy(hin.data(), labels, lab_bytes);
+  std::memcpy(hin.data() + lab_bytes, req, req_bytes);
+  std::memcpy(hin.data() + lab_bytes + req_bytes, present, (size_t)k * 4);
+  std::memcpy(hin.data() + lab_bytes + req_bytes + (size_t)k * 4, ns_id, (size_t)k * 4);
+  if ((rc = upload_vec(c, c->d_call_in, hin))) return rc;
+  const CheckBlock blk(k, Wp, words, codes);
+  KT_CUDA(c, c->d_call_out.reserve(blk.bytes() + 16));
+  KT_CUDA(c, c->h_call.reserve(blk.fetch));
+  KT_CUDA(c, cudaMemsetAsync(c->d_call_out.p, 0, blk.bytes(), c->stream));
+  if ((rc = rows_prep(c, KT_EVAL_GIVEN_STATUS | KT_EVAL_SKIP_RECONCILE | flags))) return rc;
+  const unsigned char* ib = c->d_call_in.as<unsigned char>();
+  unsigned char* ob = c->d_call_out.as<unsigned char>();
+  PodsArgs a{};
+  a.tb = table_view(c);
+  a.L = L; a.R = R; a.k = k;
+  a.labels = reinterpret_cast<const int64_t*>(ib);
+  a.req = reinterpret_cast<const int64_t*>(ib + lab_bytes);
+  a.present = reinterpret_cast<const uint32_t*>(ib + lab_bytes + req_bytes);
+  a.ns = reinterpret_cast<const int32_t*>(ib + lab_bytes + req_bytes + (size_t)k * 4);
+  a.pre = c->d_chk_pre.as<unsigned char>();
+  a.admit = ob;
+  a.codes = reinterpret_cast<uint32_t*>(ob + blk.adm_bytes);
+  a.words = reinterpret_cast<uint32_t*>(ob + blk.adm_bytes + blk.code_bytes);
+  KT_CUDA(c, with_variant(c, true, [&](auto tpc, auto b, auto, auto reg) {
+    return launch(c, k_check_pods<tpc, b, reg>, (unsigned)((k + kRowsTile - 1) / kRowsTile), kRowsTile, rows_smem_bytes(L, R, reg), false, a);
+  }));
+  KT_CUDA(c, cudaMemcpyAsync(c->h_call.p, ob, blk.fetch, cudaMemcpyDeviceToHost, c->stream));
+  KT_CUDA(c, cudaStreamSynchronize(c->stream));
+  const unsigned char* hb = c->h_call.as<unsigned char>();
+  if (admit) std::memcpy(admit, hb, (size_t)k);
+  if (codes) std::memcpy(codes, hb + blk.adm_bytes, blk.code_bytes);
+  if (words) std::memcpy(words, hb + blk.adm_bytes + blk.code_bytes, blk.word_bytes);
   return KT_OK;
 }
 

@@ -33,6 +33,7 @@
 #pragma weak kt_reconcile_throttles
 #pragma weak kt_check_pending_rows
 #pragma weak kt_match_pods
+#pragma weak kt_check_pods            // without it (older engine doubles) check_pending runs a pass over queue + scratch rows
 #pragma weak kt_get_check_summary
 #pragma weak kt_update_status_rows    // without them (older engine doubles) sync_status / sync_reserved upload whole tables
 #pragma weak kt_update_reserved_rows
@@ -1865,6 +1866,20 @@ struct kth_plugin {
     PendingResult(size_t k, int Wp) : bitmap(k * (size_t)Wp, 0), codes(k * 2 * (size_t)Wp, 0), admit(k, 1), Wp(Wp) {}
     RowView row(size_t i) const { return RowView{bitmap.data() + i * (size_t)Wp, codes.data() + i * 2 * (size_t)Wp, admit[i], Wp}; }
   };
+  // The PENDING table's capacities for the queue and k scratch rows.  A capacity that grows means a full upload, which re-packs
+  // every row and so voids the cached verdicts -- at once, also on the paths that check a batch without uploading it
+  // (check_pending), so that the queue cache keeps one rule whichever path checked the batch.
+  void size_pending(int64_t k) {
+    int64_t want_q = std::max<int64_t>(64, pend_capacity), want_s = std::max<int64_t>(16, scratch_capacity);
+    while (want_q < (int64_t)pend_pod.size()) want_q *= 2;
+    while (want_s < k) want_s *= 2;
+    if (want_q != pend_capacity || want_s != scratch_capacity) {
+      pend_capacity = want_q;
+      scratch_capacity = want_s;
+      pend_full_upload = true;
+    }
+    if (pend_full_upload) queue.valid = false;
+  }
   // The device's PENDING table = the resident queue rows + `k` scratch rows holding `batch` (pods that are not in the informer
   // cache), brought up to date together with the state a PreFilter view reads (sync_state).  Row deltas; a full upload only
   // when a capacity grows or the packing changed.
@@ -1872,19 +1887,16 @@ struct kth_plugin {
     sync_state();
     const int L = lim.label_slots, R = lim.n_resources;
     const int64_t k = (int64_t)batch.size();
-    int64_t want_q = std::max<int64_t>(64, pend_capacity), want_s = std::max<int64_t>(16, scratch_capacity);
-    while (want_q < (int64_t)pend_pod.size()) want_q *= 2;
-    while (want_s < k) want_s *= 2;
-    if (want_q != pend_capacity || want_s != scratch_capacity) pend_full_upload = true;
+    size_pending(k);
     const bool full = pend_full_upload;
-    const int64_t first_scratch = full ? want_q : pend_capacity;
+    const int64_t first_scratch = pend_capacity;
     std::vector<int64_t> rows;  // the rows a delta packs (a full upload packs every row)
     if (!full) {
       rows.assign(pend_dirty.begin(), pend_dirty.end());
       const int64_t n_scratch = std::max(k, scratch_used);  // this batch, and what the last one left behind
       for (int64_t i = 0; i < n_scratch; ++i) rows.push_back(pend_capacity + i);
     }
-    const size_t n = full ? (size_t)(want_q + want_s) : rows.size();
+    const size_t n = full ? (size_t)(pend_capacity + scratch_capacity) : rows.size();
     if (n) {
       PodObj tomb;
       auto pod_at = [&](int64_t row) -> const PodObj& {
@@ -1903,12 +1915,7 @@ struct kth_plugin {
         check(kt_update_pod_rows(ctx, KT_PODS_PENDING, (int64_t)n, rows.data(), lab.data(), req.data(), present.data(), flags.data(), nsid.data()),
               "kt_update_pod_rows(pending)");
     }
-    if (full) {
-      pend_capacity = want_q;
-      scratch_capacity = want_s;
-      pend_full_upload = false;
-      queue.valid = false;
-    }
+    if (full) pend_full_upload = false;
     pend_dirty.clear();
     scratch_used = k;
   }
@@ -1989,9 +1996,32 @@ struct kth_plugin {
     fetch_queue_results();
   }
 
+  // PreFilter of pods given by value (manifests, and informer pods checked like one).  With kt_check_pods the batch is packed and
+  // checked in one call that costs the words of each pod's namespace: no row is uploaded and no pass runs, so the device keeps
+  // the codes of the last pass, which kth_affected_pods and kth_queue_report only reuse at an unchanged `epoch` (every
+  // non-reading entry point moves it).  Without it (older engine doubles) the batch takes scratch rows behind the queue and one
+  // pass over both.  Either way the state is synced first and the capacities are sized for the batch (size_pending), so that the
+  // statuses, reservations, cached verdicts and errors come out the same.
   PendingResult check_pending(const std::vector<PodObj>& batch, uint32_t extra_flags) {
-    run_pending_pass(batch, extra_flags);
-    return scratch_rows(batch.size());
+    if (!kt_check_pods) {
+      run_pending_pass(batch, extra_flags);
+      return scratch_rows(batch.size());
+    }
+    sync_state();
+    size_pending((int64_t)batch.size());
+    const size_t k = batch.size();
+    const int L = lim.label_slots, R = lim.n_resources;
+    std::vector<int64_t> lab((size_t)L * k), req((size_t)R * k);
+    std::vector<uint32_t> present(k), flags(k);
+    std::vector<int32_t> nsid(k);
+    for (size_t i = 0; i < k; ++i) pack_pod(batch[i], lab, req, present, flags, nsid, k, i);
+    if (namespaces_dirty || throttles_dirty) sync_state();  // packing introduced new namespace ids
+    PendingResult out(k, kt_match_words(ctx));
+    if (throttles.empty() || k == 0) return out;
+    check(kt_check_pods(ctx, extra_flags, (int64_t)k, lab.data(), req.data(), present.data(), nsid.data(), out.bitmap.data(), out.codes.data(),
+                        out.admit.data()),
+          "kt_check_pods");
+    return out;
   }
   // PreFilter of a pod of the resident queue: from the cached verdicts when they are current, else after ONE pass that
   // refreshes the whole queue's.

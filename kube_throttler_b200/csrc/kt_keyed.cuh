@@ -1,6 +1,7 @@
 // kt_keyed.cuh -- reconcile(key) for k listed throttles on the device (kt_reconcile_throttles), PreFilter for k listed
-// pending rows (kt_check_pending_rows), the affected throttles of k pods given by value (kt_match_pods) and the scheduling queue
-// summarised per throttle (kt_get_check_summary), the last three at the end of this file.
+// pending rows (kt_check_pending_rows), the affected throttles of k pods given by value (kt_match_pods), PreFilter of k pods given
+// by value (kt_check_pods) and the scheduling queue summarised per throttle (kt_get_check_summary), the last four at the end of
+// this file.
 //
 // The reference reconciles one key at a time (throttle_controller.go:84-211, clusterthrottle_controller.go:87-214): a key costs
 // the pods of the namespaces its throttle reaches (affectedPods, :221-246), not the whole snapshot.  Here the listed throttles'
@@ -257,6 +258,43 @@ __host__ __device__ inline size_t rows_smem_bytes(int L, int R, bool reg_rows) {
   return (size_t)R * kRowsTile * 8 + (reg_rows ? 0 : (size_t)((L + 7) & ~7) * kRowsTile * 4);
 }
 
+// ResourceAmountOfPod(pod) of the column `p` of req [R][n] into s_req[r * stride]: the non-zero requests are the only ones
+// IsThrottledFor looks at (Q5), so their bits are returned
+__device__ __forceinline__ uint32_t stage_requests(const int64_t* req, int64_t n, int64_t p, uint32_t present, int R, long long* s_req, int stride) {
+  uint32_t nz = 0;
+  for (int r = 0; r < R; ++r) {
+    long long v = __ldg(&req[(int64_t)r * n + p]);
+    if (!((present >> r) & 1)) v = 0;
+    s_req[r * stride] = v;
+    if (v != 0) nz |= 1u << r;
+  }
+  return nz;
+}
+
+// The check of one pending pod, one lane: the words of its namespace's list (winfo) evaluated with the pass's eval_word, each
+// non-zero word stored and decided pair by pair from the pre-records (decide_word_direct_codes; GIVEN_STATUS reads no sums).
+// wrow [Wp] / crow [2 Wp] must be zero: only the non-zero words are written.  Returns the admit byte.
+template <int TPC, int B, bool REG>
+__device__ __forceinline__ unsigned char check_words(const TableView& tb, const PodRows<REG>& rows, int Lpad, int ns, uint32_t winfo,
+                                                     const unsigned char* pre, int R, const DecidePod& pod, uint32_t* wrow, uint32_t* crow) {
+  WordCursor wc;
+  wc.init(tb, winfo, ns, (unsigned)ns < (unsigned)tb.NS);  // a namespace out of range affects nothing
+  const PartExchange px{};  // GIVEN_STATUS: the pre-records carry everything, no sums are read
+  const size_t rec = pre_record_bytes(R);
+  unsigned char ok = 1;
+#pragma unroll 1
+  for (int q = 0; q < wc.cnt; ++q) {
+    const int w = wc.at(tb, q);
+    const uint32_t word = eval_word<TPC, B, REG>(tb, rows, Lpad, ns, w);
+    if (!word) continue;
+    wrow[w] = word;
+    const uint2 c = decide_word_direct_codes(word, w, pre, px, rec, R, tb.M, pod);
+    *reinterpret_cast<uint2*>(&crow[2 * w]) = c;
+    if (c.x | c.y) ok = 0;
+  }
+  return ok;
+}
+
 template <int TPC, int B, bool REG>
 __global__ void __launch_bounds__(kRowsTile) k_check_rows(const RowsArgs a) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -272,36 +310,12 @@ __global__ void __launch_bounds__(kRowsTile) k_check_rows(const RowsArgs a) {
   const int ns = __ldg(&pods.ns[p]);
   const uint32_t present = __ldg(&pods.present[p]);
   const uint32_t winfo = __ldg(&pods.winfo[p]);
-  // ResourceAmountOfPod(pod): the non-zero requests are the only ones IsThrottledFor looks at (Q5)
-  uint32_t nz = 0;
-  for (int r = 0; r < R; ++r) {
-    long long v = __ldg(&pods.req[(int64_t)r * pods.n + p]);
-    if (!((present >> r) & 1)) v = 0;
-    s_req[r * kRowsTile + tid] = v;
-    if (v != 0) nz |= 1u << r;
-  }
+  const uint32_t nz = stage_requests(pods.req, pods.n, p, present, R, s_req + tid, kRowsTile);
   const DecidePod pod{s_req + tid, kRowsTile, nz, p};
   PodRows<REG> rows;
   rows.init(s_rowid, tid, kRowsTile);
   load_rows<REG>(pods.roff, pods.n, p, a.L, rows);
-  WordCursor wc;
-  wc.init(a.tb, winfo, ns, (unsigned)ns < (unsigned)a.tb.NS);  // a namespace out of range affects nothing
-  const PartExchange px{};  // GIVEN_STATUS: the pre-records carry everything, no sums are read
-  const size_t rec = pre_record_bytes(R);
-  uint32_t* wrow = a.words + i * Wp;
-  uint32_t* crow = a.codes + i * 2 * Wp;
-  unsigned char ok = 1;
-#pragma unroll 1
-  for (int q = 0; q < wc.cnt; ++q) {
-    const int w = wc.at(a.tb, q);
-    const uint32_t word = eval_word<TPC, B, REG>(a.tb, rows, Lpad, ns, w);
-    if (!word) continue;
-    wrow[w] = word;
-    const uint2 c = decide_word_direct_codes(word, w, a.pre, px, rec, R, a.tb.M, pod);
-    *reinterpret_cast<uint2*>(&crow[2 * w]) = c;
-    if (c.x | c.y) ok = 0;
-  }
-  a.admit[i] = ok;
+  a.admit[i] = check_words<TPC, B, REG>(a.tb, rows, Lpad, ns, winfo, a.pre, R, pod, a.words + i * Wp, a.codes + i * 2 * Wp);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -320,6 +334,36 @@ struct MatchArgs {
   const int32_t* ns;      // [k]
   uint32_t* words;        // [k][Wp]
 };
+
+// The label codes of column i of labels [L][k] as row offsets into the current tables, in the lane's rows (translate8, the chunk
+// k_unpack_packed translates while it is in registers); slots L..Lpad read empty as the resident rows' padding does.
+template <bool REG>
+__device__ __forceinline__ void translate_labels(const TableView& tb, const int64_t* labels, int64_t k, int64_t i, int L, PodRows<REG>& rows) {
+  const int Lpad = (L + 7) & ~7;
+#pragma unroll 1
+  for (int s0 = 0; s0 < Lpad; s0 += 8) {
+    int64_t lab[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) lab[j] = s0 + j < L ? __ldg(&labels[(int64_t)(s0 + j) * k + i]) : KT_LABEL_EMPTY;
+    uint4 ke[8];
+    uint32_t o[8];
+    translate8_keys(tb, lab, ke);
+    translate8_rows(tb, lab, ke, o);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      if constexpr (REG) rows.off[j] = o[j];  // (REG: L <= 8, one chunk)
+      else rows.col[(s0 + j) * rows.stride] = o[j];
+    }
+  }
+}
+
+// The words that can apply to namespace ns, as k_translate_rows packs them for a resident row (0 for a namespace out of range)
+__device__ __forceinline__ uint32_t ns_winfo(const TableView& tb, int ns) {
+  if ((unsigned)ns >= (unsigned)tb.NS) return 0u;
+  const int lo = __ldg(&tb.nsw_off[ns]);
+  const int cnt = __ldg(&tb.nsw_off[ns + 1]) - lo;
+  return cnt == 0 ? 0u : winfo_pack(cnt, __ldg(&tb.nsw_idx[lo]), cnt > 1 ? __ldg(&tb.nsw_idx[lo + 1]) : 0, tb.W);
+}
 
 __host__ __device__ inline size_t match_smem_bytes(int L, bool reg_rows) { return reg_rows ? 0 : (size_t)((L + 7) & ~7) * kRowsTile * 4; }
 
@@ -342,25 +386,8 @@ __global__ void __launch_bounds__(kRowsTile) k_match_pods(const MatchArgs a) {
   if ((unsigned)ns >= (unsigned)a.tb.NS) return;  // a namespace out of range affects nothing
   PodRows<REG> rows;
   rows.init(reinterpret_cast<int32_t*>(smem_raw), tid, kRowsTile);
-#pragma unroll 1
-  for (int s0 = 0; s0 < Lpad; s0 += 8) {
-    int64_t lab[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) lab[j] = s0 + j < a.L ? __ldg(&a.labels[(int64_t)(s0 + j) * a.k + i]) : KT_LABEL_EMPTY;
-    uint4 ke[8];
-    uint32_t o[8];
-    translate8_keys(a.tb, lab, ke);
-    translate8_rows(a.tb, lab, ke, o);
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      if constexpr (REG) rows.off[j] = o[j];  // (REG: L <= 8, one chunk)
-      else rows.col[(s0 + j) * rows.stride] = o[j];
-    }
-  }
-  // the words that can apply to the namespace, as k_translate_rows packs them for a resident row
-  const int lo = __ldg(&a.tb.nsw_off[ns]);
-  const int cnt = __ldg(&a.tb.nsw_off[ns + 1]) - lo;
-  const uint32_t winfo = cnt == 0 ? 0u : winfo_pack(cnt, cnt > 0 ? __ldg(&a.tb.nsw_idx[lo]) : 0, cnt > 1 ? __ldg(&a.tb.nsw_idx[lo + 1]) : 0, a.tb.W);
+  translate_labels<REG>(a.tb, a.labels, a.k, i, a.L, rows);
+  const uint32_t winfo = ns_winfo(a.tb, ns);
   WordCursor wc;
   wc.init(a.tb, winfo, ns, true);
   uint32_t* wrow = a.words + i * Wp;
@@ -370,6 +397,45 @@ __global__ void __launch_bounds__(kRowsTile) k_match_pods(const MatchArgs a) {
     const uint32_t word = eval_word<TPC, B, REG>(a.tb, rows, Lpad, ns, w);
     if (word) wrow[w] = word;
   }
+}
+
+// ------------------------------------------------------------------------------------------------
+// PreFilter of k pods given by value (kt_check_pods): a manifest PreFilter, Reserve or Unreserve costs the words of the pod's
+// namespace, with no row of the pending table read or written.  The front half is k_match_pods' (the label slots translated in
+// the lane's rows, the namespace's word list from winfo_pack), the back half k_check_rows' (the requests in shared memory, each
+// non-zero word decided from the pre-records k_rows_prep wrote for this call).  The pass reads no flags of a pending row, so the
+// pods carry none.  Outputs go to the call's own block, zeroed before the launch, as in k_check_rows.
+// ------------------------------------------------------------------------------------------------
+struct PodsArgs {
+  TableView tb;
+  int L, R;
+  int64_t k;
+  const int64_t* labels;     // [L][k] label codes
+  const int64_t* req;        // [R][k]
+  const uint32_t* present;   // [k]
+  const int32_t* ns;         // [k]
+  const unsigned char* pre;  // [M][pre_record_bytes(R)] from k_rows_prep
+  uint32_t* words;           // [k][Wp]
+  uint32_t* codes;           // [k][2 Wp]
+  unsigned char* admit;      // [k]
+};
+
+template <int TPC, int B, bool REG>
+__global__ void __launch_bounds__(kRowsTile) k_check_pods(const PodsArgs a) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  const int tid = threadIdx.x;
+  const int64_t i = (int64_t)blockIdx.x * kRowsTile + tid;
+  if (i >= a.k) return;  // (no barrier and no warp collective below: each lane works alone)
+  const int R = a.R, Wp = a.tb.Wp, Lpad = (a.L + 7) & ~7;
+  long long* s_req = reinterpret_cast<long long*>(smem_raw);                              // [R][TILE]
+  int32_t* s_rowid = reinterpret_cast<int32_t*>(smem_raw + (size_t)R * kRowsTile * 8);   // [Lpad][TILE] (!REG)
+  const int ns = __ldg(&a.ns[i]);
+  const uint32_t nz = stage_requests(a.req, a.k, i, __ldg(&a.present[i]), R, s_req + tid, kRowsTile);
+  const DecidePod pod{s_req + tid, kRowsTile, nz, i};
+  PodRows<REG> rows;
+  rows.init(s_rowid, tid, kRowsTile);
+  translate_labels<REG>(a.tb, a.labels, a.k, i, a.L, rows);
+  a.admit[i] = check_words<TPC, B, REG>(a.tb, rows, Lpad, ns, ns_winfo(a.tb, ns), a.pre, R, pod, a.words + i * Wp, a.codes + i * 2 * Wp);
 }
 
 // ------------------------------------------------------------------------------------------------
