@@ -280,6 +280,17 @@ int kt_update_pod_rows(kt_ctx* ctx, int kind, int64_t k, const int64_t* rows,
                        const uint32_t* flags, const int32_t* ns_id);
 /* Namespace rows (namespaceInformer, clusterthrottle_controller.go:224-247). */
 int kt_upload_namespaces(kt_ctx* ctx, int32_t n_ns, const int64_t* labels /*[LN][n_ns]*/);
+/* Row deltas of the namespace rows, for a caller that keeps the snapshot resident: a Namespace created, relabelled or deleted
+ * changes its own row, and only the namespace masks and word lists of the tables depend on it (the pod-label tables do not).
+ * Afterwards every call answers exactly as after a kt_upload_namespaces(ctx, n_ns, all_rows), where all_rows holds the previous
+ * rows with the k listed ones replaced by labels[.][i] ([LN][k]); rows between the previous count and n_ns that are not listed
+ * are label-less.  n_ns never shrinks; idx entries distinct and in [0, n_ns); k >= 0; no null idx, and no null labels when
+ * LN > 0, with k > 0 (KT_ERR_INVALID otherwise); k = 0 with an unchanged n_ns is a no-op.  Before kt_upload_throttles only the
+ * stored rows change, as with the full call.  Otherwise the listed rows (and the rows n_ns grew by) are evaluated against every
+ * term on the device and the word lists are rebuilt there; no table compile, no re-upload of the pod-label tables, one staged
+ * copy and one synchronisation.  The state flags move as the full call moves them: kt_evaluate is needed again before the
+ * getters that read a pass.  Multi-GPU: the tables are replicated, so the call is local -- every rank applies the same updates. */
+int kt_update_namespace_rows(kt_ctx* ctx, int32_t n_ns, int64_t k, const int32_t* idx, const int64_t* labels /*[LN][k]*/);
 /* Throttle + ClusterThrottle specs; compiles the selectors into the bit-sliced match tables. */
 int kt_upload_throttles(kt_ctx* ctx, int32_t m, const kt_throttle_cols* cols,
                         const kt_selector_table* sel);
@@ -515,6 +526,10 @@ typedef struct kt_pass_plan {
 #define KT_PLAN_DECIDE_PER_POD 2
 int kt_debug_set_pass_plan(kt_ctx* ctx, const kt_pass_plan* plan);
 int kt_debug_get_pass_plan(kt_ctx* ctx, kt_pass_plan* last);
+/* The namespace side of the resident tables, as the passes read it (test seam: after kt_update_namespace_rows it must equal what
+ * kt_debug_compile_tables gives for the same rows).  dims[5] = {NS, n_nsw, max_ns_words, W, TPpad}; nsmask [NS][W][TPpad], nsw_off [NS+1],
+ * nsw_idx [n_nsw] may each be NULL (first call with NULL arrays to size them).  KT_ERR_STATE before kt_upload_throttles. */
+int kt_debug_get_ns_tables(kt_ctx* ctx, int32_t dims[5], uint32_t* nsmask, int32_t* nsw_off, int32_t* nsw_idx);
 
 /* ---- row order of the pod tables ------------------------------------------------------ */
 /* A pass costs far more when the 32 rows of a warp belong to many namespaces than when they share one.  So the engine may STORE

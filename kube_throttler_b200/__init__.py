@@ -30,7 +30,7 @@ class KtError(RuntimeError):
 
 def build(force: bool = False) -> str:
     """Compile csrc/ for sm_90a in-tree (nvcc cross-compiles without a GPU)."""
-    srcs = [os.path.join(_HERE, "csrc", f) for f in ("kt_engine.cu", "kt_tables.cc", "kt_host.cc", "kt_kernels.cuh", "kt_admit.cuh", "kt_keyed.cuh", "kt_order.cuh", "kt_tables.h", "kt_json.h", "kt_quantity.h")]
+    srcs = [os.path.join(_HERE, "csrc", f) for f in ("kt_engine.cu", "kt_tables.cc", "kt_host.cc", "kt_kernels.cuh", "kt_admit.cuh", "kt_keyed.cuh", "kt_nsrows.cuh", "kt_order.cuh", "kt_tables.h", "kt_json.h", "kt_quantity.h")]
     srcs.append(os.path.join(_HERE, "..", "include", "kt_b200.h"))
     srcs.append(os.path.join(_HERE, "..", "include", "kt_host.h"))
     newest = max(os.path.getmtime(s) for s in srcs)
@@ -42,10 +42,10 @@ def build(force: bool = False) -> str:
 
 EXPORTS = [
     "kt_create", "kt_destroy", "kt_last_error", "kt_version", "kt_set_stream", "kt_sync", "kt_enable_timing",
-    "kt_enable_trace", "kt_get_trace", "kt_host_alloc", "kt_host_alloc_upload", "kt_host_free", "kt_upload_pods", "kt_upload_pods_compact", "kt_upload_pods_packed", "kt_set_async_uploads", "kt_update_pod_rows", "kt_upload_namespaces",
+    "kt_enable_trace", "kt_get_trace", "kt_host_alloc", "kt_host_alloc_upload", "kt_host_free", "kt_upload_pods", "kt_upload_pods_compact", "kt_upload_pods_packed", "kt_set_async_uploads", "kt_update_pod_rows", "kt_upload_namespaces", "kt_update_namespace_rows",
     "kt_upload_throttles", "kt_upload_status", "kt_set_reserved", "kt_update_status_rows", "kt_update_reserved_rows", "kt_evaluate", "kt_get_reconcile",
     "kt_match_words", "kt_get_match_bitmap", "kt_get_match_rows", "kt_get_match_columns", "kt_get_check_summary", "kt_reconcile_throttles", "kt_get_check", "kt_set_sparse_check", "kt_get_check_sparse", "kt_get_check_rows", "kt_check_pending_rows", "kt_match_pods", "kt_check_pods", "kt_get_changed", "kt_get_reconcile_rows", "kt_step_submit", "kt_step_wait", "kt_admit_queue", "kt_get_timing", "kt_comm_unique_id",
-    "kt_comm_init", "kt_comm_destroy", "kt_debug_compile_tables", "kt_debug_set_pass_plan", "kt_debug_get_pass_plan",
+    "kt_comm_init", "kt_comm_destroy", "kt_debug_compile_tables", "kt_debug_set_pass_plan", "kt_debug_get_pass_plan", "kt_debug_get_ns_tables",
     "kt_debug_set_row_order", "kt_debug_get_row_order",
 ]
 
@@ -94,6 +94,7 @@ def lib():
         L.kt_get_reconcile_rows.argtypes = [vp, C.c_int64, vp, C.POINTER(abi.ReconcileOut)]
         L.kt_update_pod_rows.argtypes = [vp, C.c_int, C.c_int64, vp, vp, vp, vp, vp, vp]
         L.kt_upload_namespaces.argtypes = [vp, C.c_int32, vp]
+        L.kt_update_namespace_rows.argtypes = [vp, C.c_int32, C.c_int64, vp, vp]
         L.kt_upload_throttles.argtypes = [vp, C.c_int32, C.POINTER(abi.ThrottleCols), C.POINTER(abi.SelectorTable)]
         L.kt_upload_status.argtypes = [vp, C.POINTER(abi.StatusCols)]
         L.kt_set_reserved.argtypes = [vp, vp, vp, vp]
@@ -116,6 +117,7 @@ def lib():
                                               vp, vp, vp, vp, vp, vp, vp, vp, vp]
         L.kt_debug_set_pass_plan.argtypes = [vp, C.POINTER(abi.PassPlan)]
         L.kt_debug_get_pass_plan.argtypes = [vp, C.POINTER(abi.PassPlan)]
+        L.kt_debug_get_ns_tables.argtypes = [vp, vp, vp, vp, vp]
         L.kt_debug_set_row_order.argtypes = [vp, C.c_int, C.c_int]
         L.kt_debug_get_row_order.argtypes = [vp, C.c_int, vp, C.POINTER(C.c_int32)]
         _lib = L
@@ -255,6 +257,22 @@ class Engine:
 
     def upload_namespaces(self, ns_labels: np.ndarray):
         self._ck(self._L.kt_upload_namespaces(self._h, ns_labels.shape[1], abi.ptr(ns_labels)))
+
+    def ns_tables(self):
+        """Test seam: the resident namespace masks and word lists, {NS, nsmask[NS][W][TPpad], nsw_off[NS+1], nsw_idx, max_ns_words}."""
+        dims = np.zeros(5, np.int32)
+        self._ck(self._L.kt_debug_get_ns_tables(self._h, abi.ptr(dims), None, None, None))
+        NS, nnsw, mx, W, TPpad = (int(x) for x in dims)
+        mask, off, idx = np.zeros((NS, W, TPpad), np.uint32), np.zeros(NS + 1, np.int32), np.zeros(max(nnsw, 1), np.int32)
+        self._ck(self._L.kt_debug_get_ns_tables(self._h, abi.ptr(dims), abi.ptr(mask), abi.ptr(off), abi.ptr(idx)))
+        return dict(NS=NS, nsmask=mask, nsw_off=off, nsw_idx=idx[:nnsw], max_ns_words=mx)
+
+    def update_namespace_rows(self, n_ns: int, idx: np.ndarray, labels: np.ndarray):
+        """kt_update_namespace_rows: the rows of the listed namespaces replaced by labels[LN][k], the count grown to n_ns (rows
+        it grows by that are not listed are label-less); the tables' namespace masks and word lists are rebuilt on the device."""
+        idx = np.ascontiguousarray(idx, np.int32)
+        labels = abi._arr(labels, np.int64, (self.LN, idx.shape[0]))
+        self._ck(self._L.kt_update_namespace_rows(self._h, int(n_ns), idx.shape[0], abi.ptr(idx), abi.ptr(labels)))
 
     def upload_throttles(self, snap: Snapshot):
         cols, sel = snap.throttle_cols(), snap.selector_table()

@@ -20,6 +20,7 @@
 #include "kt_kernels.cuh"
 #include "kt_admit.cuh"
 #include "kt_keyed.cuh"
+#include "kt_nsrows.cuh"
 #include "kt_order.cuh"
 #include "kt_tables.h"
 
@@ -151,6 +152,12 @@ struct kt_ctx {
   SelectorSpec spec;
   HostTables ht;
   DevBuf d_hash, d_keydir, d_valrow, d_table, d_need, d_nsmask, d_nsw_off, d_nsw_idx;
+  // After kt_update_namespace_rows the device copies of nsmask / nsw_off / nsw_idx are the current ones (ht keeps the vectors of
+  // the last compile, ht.NS and ht.max_ns_words follow the device).  nsw_total: entries of d_nsw_idx in use.
+  int32_t nsw_total = 0;
+  DevBuf d_nsspec;  // NsSpecView (kt_nsrows.cuh): the namespace side of the selector spec, one block staged by kt_upload_throttles
+  size_t nsspec_at[8] = {};
+  std::vector<unsigned char> h_nsspec;
   DevBuf d_kind, d_tflags, d_thr, d_thr_present, d_thr_cnt, d_ovr_off, d_ovr_begin, d_ovr_end, d_ovr_flags, d_ovr_thr,
       d_ovr_present, d_ovr_cnt;
   bool have_status = false;
@@ -287,6 +294,7 @@ int recompile_tables(kt_ctx* c) {
   if ((rc = upload_vec(c, c->d_nsmask, c->ht.nsmask))) return rc;
   if ((rc = upload_vec(c, c->d_nsw_off, c->ht.nsw_off))) return rc;
   if ((rc = upload_vec(c, c->d_nsw_idx, c->ht.nsw_idx))) return rc;
+  c->nsw_total = (int32_t)c->ht.nsw_idx.size();
   KT_CUDA(c, cudaStreamSynchronize(c->stream));  // host vectors may be rebuilt right after
   for (auto& s : c->pods) s.roff_valid = s.bitmap_clean = false;  // row offsets point into the tables that were just replaced; word lists changed
   return KT_OK;
@@ -897,7 +905,7 @@ void kt_destroy(kt_ctx* c) {
                    &c->d_st_used, &c->d_st_used_present, &c->d_st_used_cnt, &c->d_st_throttled, &c->d_reserved, &c->d_reserved_present,
                    &c->d_reserved_cnt, &c->d_part, &c->d_sync, &c->d_trace, &c->d_pre, &c->d_changed, &c->d_col_idx, &c->d_col_cnt, &c->d_col_off,
                    &c->d_col_rows, &c->d_adm_state, &c->d_adm_fail, &c->d_adm_counters, &c->d_out, &c->d_codes, &c->d_admit,
-                   &c->d_key_reach, &c->d_key_scratch, &c->d_key_acc, &c->d_chk_pre, &c->d_call_in, &c->d_call_out};
+                   &c->d_key_reach, &c->d_key_scratch, &c->d_key_acc, &c->d_chk_pre, &c->d_call_in, &c->d_call_out, &c->d_nsspec};
   c->h_call.release();
   c->h_step.release();
   if (c->ev_step) cudaEventDestroy(c->ev_step);
@@ -1188,6 +1196,43 @@ int kt_update_pod_rows(kt_ctx* c, int kind, int64_t k, const int64_t* rows, cons
   return KT_OK;
 }
 
+namespace {
+// The namespace side of the selector spec (NsSpecView, kt_nsrows.cuh) in one device block, after the tables of a throttle upload
+// were compiled (term_unsat comes from there).  Read by kt_update_namespace_rows only.
+int stage_ns_spec(kt_ctx* c) {
+  const SelectorSpec& s = c->spec;
+  const size_t M = (size_t)s.m, nt = s.term_flags.size(), nq = s.req_key.size(), nv = s.req_vals.size();
+  std::vector<uint8_t> tf(nt);
+  for (size_t i = 0; i < nt; ++i)
+    tf[i] = (uint8_t)((s.term_flags[i] & (KT_TERM_NS_INVALID | KT_TERM_POD_INVALID)) | (c->ht.term_unsat[i] ? kTermUnsat : 0));
+  const struct {
+    const void* p;
+    size_t bytes;
+  } part[8] = {{s.term_off.data(), (M + 1) * 4}, {s.ns_req_off.data(), s.ns_req_off.size() * 4}, {tf.data(), nt}, {s.req_key.data(), nq * 4},
+               {s.req_op.data(), nq}, {s.req_val_off.data(), s.req_val_off.size() * 4}, {s.req_vals.data(), nv * 4}, {s.ns_id.data(), M * 4}};
+  size_t total = 0;
+  for (int i = 0; i < 8; ++i) {
+    c->nsspec_at[i] = total;
+    total += (part[i].bytes + 15) & ~(size_t)15;
+  }
+  c->h_nsspec.assign(total, 0);
+  for (int i = 0; i < 8; ++i)
+    if (part[i].bytes) std::memcpy(c->h_nsspec.data() + c->nsspec_at[i], part[i].p, part[i].bytes);
+  return upload_vec(c, c->d_nsspec, c->h_nsspec);
+}
+NsSpecView ns_spec_view(const kt_ctx* c) {
+  const unsigned char* b = c->d_nsspec.as<unsigned char>();
+  NsSpecView v;
+  v.term_off = reinterpret_cast<const int32_t*>(b + c->nsspec_at[0]); v.ns_req_off = reinterpret_cast<const int32_t*>(b + c->nsspec_at[1]);
+  v.term_flags = b + c->nsspec_at[2]; v.req_key = reinterpret_cast<const uint32_t*>(b + c->nsspec_at[3]); v.req_op = b + c->nsspec_at[4];
+  v.req_val_off = reinterpret_cast<const int32_t*>(b + c->nsspec_at[5]); v.req_vals = reinterpret_cast<const uint32_t*>(b + c->nsspec_at[6]);
+  v.ns_id = reinterpret_cast<const int32_t*>(b + c->nsspec_at[7]);
+  v.kind = c->d_kind.as<uint8_t>(); v.flags = c->d_tflags.as<uint8_t>();
+  v.M = c->ht.M; v.W = c->ht.W; v.TPpad = c->ht.TPpad;
+  return v;
+}
+}  // namespace
+
 int kt_upload_namespaces(kt_ctx* c, int32_t n_ns, const int64_t* labels) {
   if (!c) return KT_ERR_INVALID;
   std::lock_guard<std::mutex> lk(c->mu);
@@ -1245,7 +1290,8 @@ int kt_upload_throttles(kt_ctx* c, int32_t m, const kt_throttle_cols* cols, cons
   c->have_reserved = false;
   c->evaluated = false;
   c->have_codes = false;
-  return recompile_tables(c);
+  if ((rc = recompile_tables(c))) return rc;
+  return stage_ns_spec(c);
 }
 
 int kt_upload_status(kt_ctx* c, const kt_status_cols* st) {
@@ -1385,6 +1431,100 @@ int kt_update_reserved_rows(kt_ctx* c, int64_t k, const int32_t* idx, const int6
   KT_CUDA(c, cudaStreamSynchronize(c->stream));  // the caller may reuse its buffers as soon as we return
   c->have_reserved = true;
   c->evaluated = false;
+  return KT_OK;
+}
+
+// ---- namespace row deltas (kt_nsrows.cuh) ---------------------------------------------------------------------------
+int kt_update_namespace_rows(kt_ctx* c, int32_t n_ns, int64_t k, const int32_t* idx, const int64_t* labels) {
+  if (!c) return KT_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(c->mu);
+  const int LN = c->lim.ns_label_slots;
+  if (k < 0) return fail(c, KT_ERR_INVALID, "kt_update_namespace_rows: k = %lld", (long long)k);
+  if (k > 0 && (!idx || (LN > 0 && !labels))) return fail(c, KT_ERR_INVALID, "kt_update_namespace_rows: null column with k = %lld", (long long)k);
+  if (n_ns < c->n_ns) return fail(c, KT_ERR_INVALID, "kt_update_namespace_rows: n_ns %d < %d (namespace rows are never removed)", n_ns, c->n_ns);
+  for (int64_t i = 0; i < k; ++i)
+    if (idx[i] < 0 || idx[i] >= n_ns) return fail(c, KT_ERR_INVALID, "kt_update_namespace_rows: namespace %d out of range [0,%d)", idx[i], n_ns);
+  {
+    std::vector<int32_t> s(idx, idx + k);
+    std::sort(s.begin(), s.end());
+    auto d = std::adjacent_find(s.begin(), s.end());
+    if (d != s.end()) return fail(c, KT_ERR_INVALID, "kt_update_namespace_rows: namespace %d listed twice", *d);
+  }
+  const int32_t old_n = c->n_ns;
+  if (k == 0 && n_ns == old_n) return KT_OK;
+  // the stored rows, as kt_upload_namespaces would hold them: [LN][n_ns], rows the count grew by label-less
+  if (n_ns != old_n) {
+    std::vector<int64_t> grown((size_t)LN * n_ns, KT_LABEL_EMPTY);
+    for (int s = 0; s < LN; ++s)
+      std::copy(c->ns_labels.begin() + (size_t)s * old_n, c->ns_labels.begin() + (size_t)(s + 1) * old_n, grown.begin() + (size_t)s * n_ns);
+    c->ns_labels.swap(grown);
+  }
+  for (int64_t i = 0; i < k; ++i)
+    for (int s = 0; s < LN; ++s) c->ns_labels[(size_t)s * n_ns + idx[i]] = labels[(size_t)s * k + i];
+  c->n_ns = n_ns;
+  c->evaluated = false;
+  if (!c->have_throttles) return KT_OK;  // the next kt_upload_throttles compiles these rows
+  int rc = set_device(c);
+  if (rc) return rc;
+  // the rows to evaluate: the listed ones and the unlisted ones the count grew by
+  std::vector<int32_t> rows(idx, idx + k);
+  {
+    std::vector<char> listed((size_t)(n_ns - old_n), 0);
+    for (int64_t i = 0; i < k; ++i)
+      if (idx[i] >= old_n) listed[(size_t)(idx[i] - old_n)] = 1;
+    for (int32_t ns = old_n; ns < n_ns; ++ns)
+      if (!listed[(size_t)(ns - old_n)]) rows.push_back(ns);
+  }
+  const int32_t kd = (int32_t)rows.size();
+  std::vector<int64_t> lab((size_t)LN * kd);
+  for (int s = 0; s < LN; ++s)
+    for (int32_t i = 0; i < kd; ++i) lab[(size_t)s * kd + i] = c->ns_labels[(size_t)s * n_ns + rows[(size_t)i]];
+  const int32_t W = c->ht.W, TPpad = c->ht.TPpad, old_NS = c->ht.NS, NS = std::max(n_ns, old_NS);
+  const size_t row_bytes = (size_t)W * TPpad * 4;
+  const size_t cap_rows = c->d_nsmask.cap > 16 ? (c->d_nsmask.cap - 16) / row_bytes : 0;
+  if ((size_t)NS > cap_rows) {  // grow by doubling; the rows above old_NS are all evaluated below
+    DevBuf grown;
+    KT_CUDA(c, grown.reserve(std::max<size_t>((size_t)NS, 2 * (size_t)old_NS) * row_bytes + 16));
+    if (old_NS > 0) KT_CUDA(c, cudaMemcpyAsync(grown.p, c->d_nsmask.p, (size_t)old_NS * row_bytes, cudaMemcpyDeviceToDevice, c->stream));
+    std::swap(c->d_nsmask, grown);
+    grown.release();
+  }
+  KT_CUDA(c, c->d_nsw_off.reserve(((size_t)NS + 1) * 4 + 16));
+  // unchanged rows keep their counts, an evaluated row has at most W words
+  KT_CUDA(c, c->d_nsw_idx.reserve(std::min((size_t)NS * W, (size_t)c->nsw_total + (size_t)kd * W) * 4 + 16));
+  KT_CUDA(c, c->d_call_out.reserve(((size_t)NS + 4) * 4 + 16));
+  static const int32_t result_slot[4] = {};
+  size_t at[3];
+  if ((rc = stage_pieces(c, {{rows.data(), (size_t)kd * 4}, {lab.data(), lab.size() * 8}, {result_slot, sizeof result_slot}}, at))) return rc;
+  const unsigned char* in = c->d_call_in.as<unsigned char>();
+  int32_t* out = c->d_call_out.as<int32_t>();  // {total, longest list, -, -}, then cnt[NS]
+  const NsSpecView sp = ns_spec_view(c);
+  for (int32_t y0 = 0; y0 < kd; y0 += 65535) {
+    const dim3 grid((unsigned)((W + 7) / 8), (unsigned)std::min(kd - y0, 65535));
+    k_ns_rows<<<grid, 256, 0, c->stream>>>(sp, y0, kd, reinterpret_cast<const int32_t*>(in + at[0]), reinterpret_cast<const int64_t*>(in + at[1]), LN,
+                                           n_ns, c->d_nsmask.as<uint32_t>());
+    KT_CUDA(c, cudaGetLastError());
+  }
+  const unsigned ns_blocks = (unsigned)((NS + 7) / 8);
+  k_ns_count<<<ns_blocks, 256, 0, c->stream>>>(NS, W, TPpad, c->d_nsmask.as<uint32_t>(), out + 4);
+  KT_CUDA(c, cudaGetLastError());
+  k_ns_scan<<<1, kNsScanThreads, 0, c->stream>>>(NS, out + 4, c->d_nsw_off.as<int32_t>(), out);
+  KT_CUDA(c, cudaGetLastError());
+  k_ns_fill<<<ns_blocks, 256, 0, c->stream>>>(NS, W, TPpad, c->d_nsmask.as<uint32_t>(), c->d_nsw_off.as<int32_t>(), c->d_nsw_idx.as<int32_t>());
+  KT_CUDA(c, cudaGetLastError());
+  c->ht.NS = NS;
+  for (auto& s : c->pods) {  // the row offsets stay valid (the pod-label tables are unchanged); the inlined words may not
+    if (s.roff_valid && s.n > 0) {
+      k_ns_winfo<<<(unsigned)((s.n + 255) / 256), 256, 0, c->stream>>>(s.n, table_view(c), s.ns.as<int32_t>(), s.winfo.as<uint32_t>());
+      KT_CUDA(c, cudaGetLastError());
+    }
+    s.bitmap_clean = false;  // the word lists changed
+  }
+  int32_t* res = reinterpret_cast<int32_t*>(c->h_call.as<unsigned char>() + at[2]);
+  KT_CUDA(c, cudaMemcpyAsync(res, out, 2 * sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
+  KT_CUDA(c, cudaStreamSynchronize(c->stream));  // the caller may reuse its buffers; the pass plan needs the longest list
+  c->nsw_total = res[0];
+  c->ht.max_ns_words = res[1];
   return KT_OK;
 }
 
@@ -2282,6 +2422,21 @@ int kt_debug_get_pass_plan(kt_ctx* c, kt_pass_plan* last) {
   std::lock_guard<std::mutex> lk(c->mu);
   if (!c->have_ran) return fail(c, KT_ERR_STATE, "kt_debug_get_pass_plan before the first fused pass");
   *last = c->ran;
+  return KT_OK;
+}
+
+int kt_debug_get_ns_tables(kt_ctx* c, int32_t dims[5], uint32_t* nsmask, int32_t* nsw_off, int32_t* nsw_idx) {
+  if (!c || !dims) return KT_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(c->mu);
+  if (!c->have_throttles) return fail(c, KT_ERR_STATE, "kt_debug_get_ns_tables before kt_upload_throttles");
+  int rc = set_device(c);
+  if (rc) return rc;
+  const size_t NS = (size_t)c->ht.NS;
+  dims[0] = c->ht.NS; dims[1] = c->nsw_total; dims[2] = c->ht.max_ns_words; dims[3] = c->ht.W; dims[4] = c->ht.TPpad;
+  if (nsmask && NS) KT_CUDA(c, cudaMemcpyAsync(nsmask, c->d_nsmask.p, NS * c->ht.W * c->ht.TPpad * 4, cudaMemcpyDeviceToHost, c->stream));
+  if (nsw_off) KT_CUDA(c, cudaMemcpyAsync(nsw_off, c->d_nsw_off.p, (NS + 1) * 4, cudaMemcpyDeviceToHost, c->stream));
+  if (nsw_idx && c->nsw_total) KT_CUDA(c, cudaMemcpyAsync(nsw_idx, c->d_nsw_idx.p, (size_t)c->nsw_total * 4, cudaMemcpyDeviceToHost, c->stream));
+  KT_CUDA(c, cudaStreamSynchronize(c->stream));
   return KT_OK;
 }
 

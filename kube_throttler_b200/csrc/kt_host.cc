@@ -37,6 +37,7 @@
 #pragma weak kt_get_check_summary
 #pragma weak kt_update_status_rows    // without them (older engine doubles) sync_status / sync_reserved upload whole tables
 #pragma weak kt_update_reserved_rows
+#pragma weak kt_update_namespace_rows  // without it (older engine doubles) every Namespace event uploads all namespace rows
 
 namespace {
 
@@ -539,6 +540,10 @@ struct kth_plugin {
   // status_dirty / reserved_dirty: the next sync uploads every column (the engine holds none, or the columns' layout or scale
   // changed).  Otherwise the columns listed in status_cols / reserved_cols go alone (kt_update_status_rows / _reserved_rows).
   bool throttles_dirty = true, namespaces_dirty = true, status_dirty = true, reserved_dirty = true;
+  // namespaces_dirty: the next sync sends namespace rows -- all of them with namespaces_full (the engine holds none, the label
+  // encoding changed, or the tables are compiled again anyway), else only the rows in ns_dirty (kt_update_namespace_rows).
+  bool namespaces_full = true;
+  std::set<int32_t> ns_dirty;
   struct ColumnSet {  // throttle columns, each listed once
     std::vector<size_t> list;
     std::vector<char> in;
@@ -755,14 +760,27 @@ struct kth_plugin {
     if ((size_t)row < queue.row_ok.size()) queue.row_ok[(size_t)row] = 0;
   }
 
-  int32_t ns_id(const std::string& ns_name) {
+  // A namespace first met through a Namespace event is one more row (the caller marks it: namespace_changed); one first met
+  // through a pod or a throttle compiles the tables again, as everything else about the throttle set does.
+  int32_t ns_id(const std::string& ns_name, bool namespace_event = false) {
     const uint32_t id = ns_dict.id(ns_name);
     if (namespaces.size() <= id) {
       namespaces.resize(id + 1);
       namespaces[id].name = ns_name;
-      namespaces_dirty = throttles_dirty = true;  // Throttle namespace equality is part of the compiled tables
+      if (!namespace_event) namespaces_dirty = namespaces_full = throttles_dirty = true;  // Throttle namespace equality is part of the compiled tables
     }
     return (int32_t)id;
+  }
+
+  // Namespace `id` was created, relabelled or deleted: its row goes to the device with the next sync, and the cached verdicts
+  // of the queued pods in it are void -- no other pod's verdict reads that row.
+  void namespace_changed(int32_t id) {
+    namespaces_dirty = true;
+    ns_dirty.insert(id);
+    if (!queue.valid) return;
+    const std::string& nm = namespaces[(size_t)id].name;
+    for (size_t row = 0; row < pend_pod.size() && row < queue.row_ok.size(); ++row)
+      if (pend_pod[row] >= 0 && pods[(size_t)pend_pod[row]].ns == nm) queue.row_ok[row] = 0;
   }
 
   // ---- engine --------------------------------------------------------------------------------------
@@ -771,7 +789,7 @@ struct kth_plugin {
     ctx = nullptr;
     sparse_cap = 0;
     queue.valid = false;
-    pods_full_upload = pend_full_upload = throttles_dirty = namespaces_dirty = status_dirty = reserved_dirty = true;
+    pods_full_upload = pend_full_upload = throttles_dirty = namespaces_dirty = namespaces_full = status_dirty = reserved_dirty = true;
   }
   void check(int rc, const char* what) {
     if (rc != KT_OK) fail(std::string(what) + ": " + (ctx ? kt_last_error(ctx) : "no engine") + " (" + std::to_string(rc) + ")");
@@ -875,27 +893,41 @@ struct kth_plugin {
       if (col_abs[c] >= ((__int128)1 << 62)) fail("resource '" + cols[c].name + "': the column sum can overflow int64 at scale 1e" + std::to_string(cols[c].scale_exp));
   }
 
+  // Namespace i's row into column `col` of lab [LN][stride].
+  void pack_namespace(size_t i, int64_t* lab, size_t stride, size_t col) {
+    int s = 0;
+    for (auto& kv : namespaces[i].labels) {
+      const int64_t code = labels.encode(kv.first, kv.second);
+      if (code != KT_LABEL_EMPTY) lab[(size_t)(s++) * stride + col] = code;
+    }
+    // A namespace the lister does not hold (never seen, or deleted) is not in the list affectedPods walks
+    // (clusterthrottle_controller.go:227) -- no ClusterThrottle term may match it, not even one whose namespaceSelector is
+    // empty.  Existing namespaces carry one internal label (a key no real label can have) that every term requires.
+    if (namespaces[i].exists && labels.encode(kNsExistsKey, "1") != KT_LABEL_EMPTY) lab[(size_t)(s++) * stride + col] = labels.encode(kNsExistsKey, "1");
+  }
+  // A Namespace event changes one row, and only the namespace masks of the tables depend on it: the dirty rows go alone, and
+  // only their queued pods lost their cached verdicts (namespace_changed).  Everything is sent again -- and every cached verdict
+  // voided -- for the first upload, a new engine, a change of the label encoding, or when the throttles are uploaded anyway.
   void sync_namespaces() {
     ensure_engine();
     if (!namespaces_dirty) return;
-    queue_void();  // (see sync_throttles)
     words_stat = -1;
     const int LN = lim.ns_label_slots;
     const size_t n = namespaces.size();
-    std::vector<int64_t> lab((size_t)LN * std::max<size_t>(n, 1), KT_LABEL_EMPTY);
-    for (size_t i = 0; i < n; ++i) {
-      int s = 0;
-      for (auto& kv : namespaces[i].labels) {
-        const int64_t code = labels.encode(kv.first, kv.second);
-        if (code != KT_LABEL_EMPTY) lab[(size_t)(s++) * n + i] = code;
-      }
-      // A namespace the lister does not hold (never seen, or deleted) is not in the list affectedPods walks
-      // (clusterthrottle_controller.go:227) -- no ClusterThrottle term may match it, not even one whose namespaceSelector is
-      // empty.  Existing namespaces carry one internal label (a key no real label can have) that every term requires.
-      if (namespaces[i].exists && labels.encode(kNsExistsKey, "1") != KT_LABEL_EMPTY) lab[(size_t)(s++) * n + i] = labels.encode(kNsExistsKey, "1");
+    if (namespaces_full || throttles_dirty || !kt_update_namespace_rows) {
+      queue_void();  // (see sync_throttles)
+      std::vector<int64_t> lab((size_t)LN * std::max<size_t>(n, 1), KT_LABEL_EMPTY);
+      for (size_t i = 0; i < n; ++i) pack_namespace(i, lab.data(), n, i);
+      check(kt_upload_namespaces(ctx, (int32_t)n, lab.data()), "kt_upload_namespaces");
+    } else {
+      const std::vector<int32_t> idx(ns_dirty.begin(), ns_dirty.end());
+      const size_t k = idx.size();
+      std::vector<int64_t> lab((size_t)LN * std::max<size_t>(k, 1), KT_LABEL_EMPTY);
+      for (size_t i = 0; i < k; ++i) pack_namespace((size_t)idx[i], lab.data(), k, i);
+      check(kt_update_namespace_rows(ctx, (int32_t)n, (int64_t)k, idx.data(), lab.data()), "kt_update_namespace_rows");
     }
-    check(kt_upload_namespaces(ctx, (int32_t)n, lab.data()), "kt_upload_namespaces");
-    namespaces_dirty = false;
+    namespaces_dirty = namespaces_full = false;
+    ns_dirty.clear();
   }
 
   // ---- device columns in NAMESPACE order ----------------------------------------------------------------------------
@@ -1227,7 +1259,7 @@ struct kth_plugin {
       if (p.row >= 0) dirty_rows.insert(p.row);
       if (p.pend_row >= 0) pend_dirty.insert(p.pend_row);
     }
-    namespaces_dirty = true;  // (a handful of rows: packed whole)
+    namespaces_dirty = namespaces_full = true;  // (a handful of rows: packed whole)
   }
   void sync_all() {
     sync_vocabulary();
@@ -1978,7 +2010,7 @@ struct kth_plugin {
   }
   // Is the cached verdict of queue row `row` still the truth?
   bool queue_row_current(int64_t row) const {
-    if (!queue.valid || throttles_dirty || namespaces_dirty || pend_full_upload) return false;
+    if (!queue.valid || throttles_dirty || (namespaces_dirty && namespaces_full) || pend_full_upload) return false;
     if (row < 0 || (size_t)row >= queue.row_ok.size() || !queue.row_ok[(size_t)row] || pend_dirty.count(row)) return false;
     const uint32_t* bm = &queue.bitmap[(size_t)row * (size_t)queue.Wp];
     for (int w = 0; w < queue.Wp; ++w)
@@ -2546,7 +2578,7 @@ struct kth_plugin {
   }
   void delete_namespace(const std::string& nm) {
     const int id = ns_dict.find(nm);
-    if (id >= 0) { namespaces[(size_t)id].exists = false; namespaces[(size_t)id].labels.clear(); namespaces_dirty = true; }
+    if (id >= 0) { namespaces[(size_t)id].exists = false; namespaces[(size_t)id].labels.clear(); namespace_changed(id); }
   }
 
   // ---- informer events in batches (kth_apply_events) ----------------------------------------------------------------
@@ -2767,7 +2799,7 @@ struct kth_plugin {
     // refuse before touching any state: the object is rejected, the plugin stays usable
     if ((int)lab.obj.size() > KT_MAX_LABEL_SLOTS - 1)  // one slot is the internal "exists" label
       fail("namespace " + nm + " has more than " + std::to_string(KT_MAX_LABEL_SLOTS - 1) + " labels");
-    const int32_t id = ns_id(nm);
+    const int32_t id = ns_id(nm, true);
     NamespaceObj& n = namespaces[(size_t)id];
     n.exists = true;
     n.labels.clear();
@@ -2776,7 +2808,7 @@ struct kth_plugin {
       max_ns_labels = (int)n.labels.size();
       if (ctx && max_ns_labels + 1 > lim.ns_label_slots) drop_engine();
     }
-    namespaces_dirty = true;
+    namespace_changed(id);
   }
   // Everything of two throttles of one key that the compiled tables and the per-column spec on the device are made of.
   static bool same_selector(const CompiledSelector& a, const CompiledSelector& b) {

@@ -1,0 +1,174 @@
+// kt_nsrows.cuh -- namespace row deltas on the device (kt_update_namespace_rows).
+//
+// A namespace's labels feed two things of the compiled tables: its own nsmask row ([W][TPpad], which throttle terms can apply to
+// its pods) and its entry in the per-namespace word lists (nsw_off / nsw_idx).  The pod-label tables (table, need, keydir, valrow,
+// hash) do not depend on namespaces.  So a Namespace event re-evaluates the listed rows here, from a device copy of the namespace
+// side of the selector spec (NsSpecView, staged by kt_upload_throttles), and rebuilds the word lists from the nsmask rows:
+//   1. k_ns_rows     one warp per (listed namespace, 32-throttle word), one lane per throttle: its terms in order, as
+//                    compile_tables (kt_tables.cc) builds the row -- a ClusterThrottle term's namespaceSelector over the row's
+//                    labels, a Throttle term's namespace equality, a KT_TERM_POD_INVALID term switching the later terms off
+//                    where it applies -- one ballot per term plane
+//   2. k_ns_count    one warp per namespace: how many of its words have a non-zero plane
+//   3. k_ns_scan     one CTA: the counts -> nsw_off, plus the total and the longest list (brought back to the host)
+//   4. k_ns_fill     one warp per namespace: the non-zero words in ascending order into nsw_idx
+//   5. k_ns_winfo    one lane per resident pod row: the words inlined with the row (winfo_pack), from the new lists
+#pragma once
+#include "kt_keyed.cuh"
+
+namespace kt {
+
+constexpr uint8_t kTermUnsat = 0x80u;  // staged term flag: the podSelector needs more keys than a pod row holds (HostTables::term_unsat)
+constexpr int kNsScanThreads = 1024;
+
+// What compile_tables reads to build the namespace masks, on the device
+struct NsSpecView {
+  const int32_t* term_off;     // [M+1]
+  const int32_t* ns_req_off;   // [n_terms+1]
+  const uint8_t* term_flags;   // [n_terms] KT_TERM_NS_INVALID | KT_TERM_POD_INVALID | kTermUnsat
+  const uint32_t* req_key;     // [n_reqs]
+  const uint8_t* req_op;       // [n_reqs]
+  const int32_t* req_val_off;  // [n_reqs+1]
+  const uint32_t* req_vals;    // [n_vals]
+  const int32_t* ns_id;        // [M]
+  const uint8_t* kind;         // [M] (the throttle columns)
+  const uint8_t* flags;        // [M]
+  int32_t M, W, TPpad;
+};
+
+// The namespaceSelector of one term over one namespace row (labels[s * stride], LN slots): kt_tables.cc ns_term_matches
+__device__ __forceinline__ bool ns_term_holds(const NsSpecView& sp, int term, uint8_t tf, const int64_t* labels, int64_t stride, int LN) {
+  if (tf & KT_TERM_NS_INVALID) return false;
+  const int q1 = __ldg(&sp.ns_req_off[term + 1]);
+  for (int q = __ldg(&sp.ns_req_off[term]); q < q1; ++q) {
+    const uint32_t key = __ldg(&sp.req_key[q]);
+    const uint8_t op = __ldg(&sp.req_op[q]);
+    bool has = false;
+    uint32_t val = 0;
+    for (int s = 0; s < LN; ++s) {
+      const int64_t l = __ldg(&labels[(int64_t)s * stride]);
+      if (l == KT_LABEL_EMPTY) continue;
+      if ((uint32_t)((uint64_t)l >> 32) == key) { has = true; val = (uint32_t)((uint64_t)l & 0xffffffffu); break; }
+    }
+    bool ok;
+    if (!has) {
+      ok = op == KT_OP_NOTIN || op == KT_OP_DOESNOTEXIST;
+    } else if (op == KT_OP_IN || op == KT_OP_NOTIN) {
+      bool in = false;
+      const int v1 = __ldg(&sp.req_val_off[q + 1]);
+      for (int v = __ldg(&sp.req_val_off[q]); v < v1 && !in; ++v) in = __ldg(&sp.req_vals[v]) == val;
+      ok = (op == KT_OP_IN) == in;
+    } else {
+      ok = op == KT_OP_EXISTS;
+    }
+    if (!ok) return false;
+  }
+  return true;
+}
+
+// nsmask rows of the kd listed namespaces ns_ids[i], labels [LN][kd]; n_ns: the namespace count (a ClusterThrottle term applies to
+// namespaces below it only).  grid (ceil(W / 8), up to 65535 rows from y0), 256 threads: warp = word.
+__global__ void __launch_bounds__(256) k_ns_rows(const NsSpecView sp, int32_t y0, int32_t kd, const int32_t* __restrict__ ns_ids,
+                                                 const int64_t* __restrict__ labels, int LN, int32_t n_ns, uint32_t* __restrict__ nsmask) {
+  const int w = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (w >= sp.W) return;  // whole warps
+  const int i = y0 + blockIdx.y;
+  const int ns = __ldg(&ns_ids[i]);
+  const int t = w * 32 + lane;
+  int term0 = 0, nterm = 0;
+  bool cluster = false, own = false;
+  if (t < sp.M) {
+    const uint8_t f = __ldg(&sp.flags[t]);
+    if ((f & KT_THR_RESPONSIBLE) && !(f & KT_THR_SELECTOR_ERROR)) {
+      term0 = __ldg(&sp.term_off[t]);
+      nterm = __ldg(&sp.term_off[t + 1]) - term0;
+    }
+    cluster = __ldg(&sp.kind[t]) != KT_KIND_THROTTLE;
+    own = __ldg(&sp.ns_id[t]) == ns;
+  }
+  bool blocked = false;  // a KT_TERM_POD_INVALID term of this throttle applies to the namespace: the later terms are off
+  uint32_t* row = nsmask + ((size_t)ns * sp.W + w) * sp.TPpad;
+  for (int s = 0; s < sp.TPpad; ++s) {
+    bool bit = false;
+    if (s < nterm) {
+      const int term = term0 + s;
+      const uint8_t tf = __ldg(&sp.term_flags[term]);
+      if ((tf & KT_TERM_POD_INVALID) || !(tf & kTermUnsat)) {
+        const bool applies = cluster ? ns < n_ns && ns_term_holds(sp, term, tf, labels + i, kd, LN) : own;
+        if (tf & KT_TERM_POD_INVALID) blocked |= applies;
+        else bit = applies && !blocked;
+      }
+    }
+    const uint32_t word = __ballot_sync(kFull, bit);
+    if (lane == 0) row[s] = word;
+  }
+}
+
+__device__ __forceinline__ bool ns_word_live(const uint32_t* __restrict__ nsmask, int ns, int w, int W, int TPpad) {
+  const uint32_t* e = nsmask + ((size_t)ns * W + w) * TPpad;
+  uint32_t any = 0;
+  for (int s = 0; s < TPpad; ++s) any |= __ldg(&e[s]);
+  return any != 0;
+}
+
+// cnt[ns] = the words of namespace ns with a non-zero plane.  One warp per namespace, 8 per CTA.
+__global__ void __launch_bounds__(256) k_ns_count(int32_t NS, int W, int TPpad, const uint32_t* __restrict__ nsmask, int32_t* __restrict__ cnt) {
+  const int ns = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (ns >= NS) return;
+  int c = 0;
+  for (int w0 = 0; w0 < W; w0 += 32) {
+    const int w = w0 + lane;
+    c += __popc(__ballot_sync(kFull, w < W && ns_word_live(nsmask, ns, w, W, TPpad)));
+  }
+  if (lane == 0) cnt[ns] = c;
+}
+
+// off[0..NS] = exclusive scan of cnt[0..NS); out = {total, longest list}.  One CTA, each thread a run of consecutive namespaces.
+__global__ void __launch_bounds__(kNsScanThreads) k_ns_scan(int32_t NS, const int32_t* __restrict__ cnt, int32_t* __restrict__ off, int32_t* __restrict__ out) {
+  __shared__ int32_t part[kNsScanThreads];
+  __shared__ int32_t longest;
+  const int tid = threadIdx.x;
+  const int per = (NS + kNsScanThreads - 1) / kNsScanThreads;
+  const int lo = min(NS, tid * per), hi = min(NS, lo + per);
+  int32_t sum = 0, mx = 0;
+  for (int i = lo; i < hi; ++i) { sum += cnt[i]; mx = max(mx, cnt[i]); }
+  if (tid == 0) longest = 0;
+  part[tid] = sum;
+  __syncthreads();
+  atomicMax(&longest, mx);
+  for (int d = 1; d < kNsScanThreads; d <<= 1) {  // inclusive scan of the per-thread sums
+    const int32_t v = tid >= d ? part[tid - d] : 0;
+    __syncthreads();
+    part[tid] += v;
+    __syncthreads();
+  }
+  int32_t at = part[tid] - sum;
+  for (int i = lo; i < hi; ++i) { off[i] = at; at += cnt[i]; }
+  if (tid == kNsScanThreads - 1) {
+    off[NS] = part[tid];
+    out[0] = part[tid];
+    out[1] = longest;
+  }
+}
+
+// nsw_idx[off[ns] ..] = the live words of namespace ns in ascending order.  One warp per namespace.
+__global__ void __launch_bounds__(256) k_ns_fill(int32_t NS, int W, int TPpad, const uint32_t* __restrict__ nsmask, const int32_t* __restrict__ off,
+                                                 int32_t* __restrict__ idx) {
+  const int ns = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (ns >= NS) return;
+  int at = off[ns];
+  for (int w0 = 0; w0 < W; w0 += 32) {
+    const int w = w0 + lane;
+    const bool live = w < W && ns_word_live(nsmask, ns, w, W, TPpad);
+    const uint32_t b = __ballot_sync(kFull, live);
+    if (live) idx[at + __popc(b & ((1u << lane) - 1u))] = w;
+    at += __popc(b);
+  }
+}
+
+// The words inlined with each resident pod row, from the new word lists (k_translate_rows' winfo; the row offsets stay valid)
+__global__ void __launch_bounds__(256) k_ns_winfo(int64_t n, const TableView tb, const int32_t* __restrict__ ns_col, uint32_t* __restrict__ winfo) {
+  const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (p < n) winfo[p] = ns_winfo(tb, __ldg(&ns_col[p]));
+}
+
+}  // namespace kt

@@ -155,7 +155,7 @@ std::string compile_tables(const kt_limits& lim, const SelectorSpec& s, int32_t 
   h.table.assign((size_t)h.W * rows * TPp * 2, 0);
   for (size_t i = 0; i < h.table.size(); i += 2) h.table[i] = 0xffffffffu;  // sat = all ones, pos = 0
   std::vector<int32_t> need((size_t)M * TP, 0);
-  std::vector<uint8_t> unsat((size_t)M * TP, 0);
+  h.term_unsat.assign((size_t)n_terms, 0);
   int32_t max_need = 0;
   for (int32_t t = 0; t < M; ++t) {
     const int32_t w = t >> 5;
@@ -177,7 +177,7 @@ std::string compile_tables(const kt_limits& lim, const SelectorSpec& s, int32_t 
           if (positive) h.table[e + 1] |= bit;
         }
       }
-      if (nd > lim.label_slots) { unsat[(size_t)t * TP + sidx] = 1; nd = 0; }  // needs more keys than a pod row can hold
+      if (nd > lim.label_slots) { h.term_unsat[(size_t)term] = 1; nd = 0; }  // needs more keys than a pod row can hold
       need[(size_t)t * TP + sidx] = nd;
       max_need = std::max(max_need, nd);
     }
@@ -225,7 +225,7 @@ std::string compile_tables(const kt_limits& lim, const SelectorSpec& s, int32_t 
         }
         continue;
       }
-      if (unsat[(size_t)t * TP + sidx]) continue;
+      if (h.term_unsat[(size_t)term]) continue;
       if (s.kind[t] == KT_KIND_THROTTLE) {
         int32_t ns = s.ns_id[t];
         if (ns >= 0 && ns < NS && !(any_blocked && blocked[(size_t)ns])) h.nsmask[((size_t)ns * h.W + w) * TPp + sidx] |= bit;

@@ -48,6 +48,7 @@ struct HostTables {
   std::vector<uint32_t> valrow;
   std::vector<uint32_t> table;   // [W][rows][TPpad][2]: {sat, pos}
   std::vector<uint32_t> need;    // [W][TPpad][B]
+  std::vector<uint8_t> term_unsat;  // [n_terms] 1: the podSelector needs more keys than a pod row holds (the term matches nobody)
   std::vector<uint32_t> nsmask;  // [NS][W][TPpad]
   std::vector<int32_t> nsw_off;  // [NS+1]
   std::vector<int32_t> nsw_idx;  // non-zero words per namespace
