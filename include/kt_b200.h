@@ -316,6 +316,21 @@ int kt_set_reserved(kt_ctx* ctx, const int64_t* reserved /*[R][m]*/,
 int kt_update_status_rows(kt_ctx* ctx, int64_t k, const int32_t* idx, const kt_status_cols* st);
 int kt_update_reserved_rows(kt_ctx* ctx, int64_t k, const int32_t* idx, const int64_t* reserved /*[R][k]*/,
                             const uint32_t* present /*[k]*/, const int64_t* cnt /*[k]*/);
+/* Column deltas of the spec's thresholds: an edit of spec.threshold or spec.temporaryThresholdOverrides changes a few columns, and
+ * no compiled table reads either.  cols is shaped for the k listed columns: thr[R][k], thr_present[k], thr_cnt[k]; ovr_off[k+1]
+ * with n_ovr == ovr_off[k], and that many ovr_begin / ovr_end / ovr_flags / ovr_present / ovr_cnt entries and ovr_thr[R][n_ovr],
+ * in spec order.  kind, ns_id and flags feed the tables and must be NULL.  Afterwards every call answers exactly as after a
+ * kt_upload_throttles whose spec columns are the previous ones with these k replaced, followed by re-uploading the status and
+ * the reservations held before the call (when they were held): both are kept, and so are the pod rows' table offsets.  The
+ * state flags move as kt_upload_throttles moves them (a pass is needed again before the getters that read one).
+ * KT_ERR_INVALID: k < 0; a null idx or column with k > 0; a non-null kind, ns_id or flags; an index out of [0, M) or listed
+ * twice; an ovr_off that does not span [0, n_ovr] monotonically.  KT_ERR_STATE before kt_upload_throttles; k = 0 is a no-op.
+ * One staged copy and one synchronisation (the caller may reuse its buffers on return); no table compile and no re-upload of
+ * the other columns.  When no listed column changes its number of overrides the columns are scattered in place and the copy
+ * carries O(k) data; otherwise every override entry moves (n_ovr and the stride of ovr_thr change): the new offsets, derived on
+ * the host, travel with the copy (O(M) bytes) and the override columns are rebuilt on the device.  Multi-GPU: the call is
+ * local, not collective -- every rank must apply the same updates. */
+int kt_update_threshold_rows(kt_ctx* ctx, int64_t k, const int32_t* idx, const kt_throttle_cols* cols);
 
 /* ---- the pass ------------------------------------------------------------------- */
 /* One batched pass: reconcile every throttle (throttle_controller.go:84-133) and check

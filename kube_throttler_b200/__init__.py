@@ -43,7 +43,7 @@ def build(force: bool = False) -> str:
 EXPORTS = [
     "kt_create", "kt_destroy", "kt_last_error", "kt_version", "kt_set_stream", "kt_sync", "kt_enable_timing",
     "kt_enable_trace", "kt_get_trace", "kt_host_alloc", "kt_host_alloc_upload", "kt_host_free", "kt_upload_pods", "kt_upload_pods_compact", "kt_upload_pods_packed", "kt_set_async_uploads", "kt_update_pod_rows", "kt_upload_namespaces", "kt_update_namespace_rows",
-    "kt_upload_throttles", "kt_upload_status", "kt_set_reserved", "kt_update_status_rows", "kt_update_reserved_rows", "kt_evaluate", "kt_get_reconcile",
+    "kt_upload_throttles", "kt_upload_status", "kt_set_reserved", "kt_update_status_rows", "kt_update_reserved_rows", "kt_update_threshold_rows", "kt_evaluate", "kt_get_reconcile",
     "kt_match_words", "kt_get_match_bitmap", "kt_get_match_rows", "kt_get_match_columns", "kt_get_check_summary", "kt_reconcile_throttles", "kt_get_check", "kt_set_sparse_check", "kt_get_check_sparse", "kt_get_check_rows", "kt_check_pending_rows", "kt_match_pods", "kt_check_pods", "kt_get_changed", "kt_get_reconcile_rows", "kt_step_submit", "kt_step_wait", "kt_admit_queue", "kt_get_timing", "kt_comm_unique_id",
     "kt_comm_init", "kt_comm_destroy", "kt_debug_compile_tables", "kt_debug_set_pass_plan", "kt_debug_get_pass_plan", "kt_debug_get_ns_tables",
     "kt_debug_set_row_order", "kt_debug_get_row_order",
@@ -100,6 +100,7 @@ def lib():
         L.kt_set_reserved.argtypes = [vp, vp, vp, vp]
         L.kt_update_status_rows.argtypes = [vp, C.c_int64, vp, C.POINTER(abi.StatusCols)]
         L.kt_update_reserved_rows.argtypes = [vp, C.c_int64, vp, vp, vp, vp]
+        L.kt_update_threshold_rows.argtypes = [vp, C.c_int64, vp, C.POINTER(abi.ThrottleCols)]
         L.kt_evaluate.argtypes = [vp, C.c_int64, C.c_uint32]
         L.kt_get_reconcile.argtypes = [vp, C.POINTER(abi.ReconcileOut)]
         L.kt_match_words.argtypes = [vp]
@@ -297,6 +298,25 @@ class Engine:
                     used_cnt=abi._arr(status["used_cnt"], np.int64), throttled=abi._arr(status["throttled"], np.uint32))
         st = abi.StatusCols(*(abi.ptr(cols[f]) for f in ("calculated", "calc_thr", "calc_present", "calc_cnt", "used", "used_present", "used_cnt", "throttled")))
         self._ck(self._L.kt_update_status_rows(self._h, k, abi.ptr(idx), C.byref(st)))
+
+    def update_threshold_rows(self, idx: np.ndarray, cols: dict):
+        """kt_update_threshold_rows: spec.threshold and the temporaryThresholdOverrides of the listed throttle columns, replaced
+        without recompiling the tables.  `cols` holds the k listed columns, named and shaped like the Snapshot fields: thr[R][k],
+        thr_present[k], thr_cnt[k], ovr_off[k+1], and ovr_begin / ovr_end / ovr_flags / ovr_present / ovr_cnt [n_ovr] and
+        ovr_thr[R][n_ovr] with n_ovr = ovr_off[k]; idx entries distinct and in [0, m)."""
+        idx = np.ascontiguousarray(idx, np.int32)
+        k, R = idx.shape[0], self.R
+        off = abi._arr(cols["ovr_off"], np.int32)
+        n = int(off[-1]) if off.shape[0] else 0
+        a = dict(thr=abi._arr(cols["thr"], np.int64, (R, k)), thr_present=abi._arr(cols["thr_present"], np.uint32),
+                 thr_cnt=abi._arr(cols["thr_cnt"], np.int64), ovr_off=off, ovr_begin=abi._arr(cols["ovr_begin"], np.int64),
+                 ovr_end=abi._arr(cols["ovr_end"], np.int64), ovr_flags=abi._arr(cols["ovr_flags"], np.uint8),
+                 ovr_thr=abi._arr(cols["ovr_thr"], np.int64, (R, n)), ovr_present=abi._arr(cols["ovr_present"], np.uint32),
+                 ovr_cnt=abi._arr(cols["ovr_cnt"], np.int64))
+        tc = abi.ThrottleCols(None, None, None, abi.ptr(a["thr"]), abi.ptr(a["thr_present"]), abi.ptr(a["thr_cnt"]), abi.ptr(off), n,
+                              abi.ptr(a["ovr_begin"]), abi.ptr(a["ovr_end"]), abi.ptr(a["ovr_flags"]), abi.ptr(a["ovr_thr"]),
+                              abi.ptr(a["ovr_present"]), abi.ptr(a["ovr_cnt"]))
+        self._ck(self._L.kt_update_threshold_rows(self._h, k, abi.ptr(idx), C.byref(tc)))
 
     def update_reserved_rows(self, idx: np.ndarray, reserved: np.ndarray, present: np.ndarray, cnt: np.ndarray):
         """kt_update_reserved_rows: reserved[R][k], present[k], cnt[k] of the listed throttle columns, replaced in place (the

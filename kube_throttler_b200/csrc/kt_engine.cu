@@ -160,6 +160,10 @@ struct kt_ctx {
   std::vector<unsigned char> h_nsspec;
   DevBuf d_kind, d_tflags, d_thr, d_thr_present, d_thr_cnt, d_ovr_off, d_ovr_begin, d_ovr_end, d_ovr_flags, d_ovr_thr,
       d_ovr_present, d_ovr_cnt;
+  // kt_update_threshold_rows: the resident ovr_off (host copy) and a spare set of override columns that a change of the
+  // override counts rebuilds into before the two sets swap
+  std::vector<int32_t> h_ovr_off;
+  DevBuf s_ovr_off, s_ovr_begin, s_ovr_end, s_ovr_flags, s_ovr_thr, s_ovr_present, s_ovr_cnt;
   bool have_status = false;
   DevBuf d_st_calculated, d_st_calc_thr, d_st_calc_present, d_st_calc_cnt, d_st_used, d_st_used_present, d_st_used_cnt,
       d_st_throttled;
@@ -251,6 +255,10 @@ int upload(kt_ctx* c, DevBuf& b, const T* src, size_t count) {
 }
 template <class T>
 int upload_vec(kt_ctx* c, DevBuf& b, const std::vector<T>& v) { return upload(c, b, v.data(), v.size()); }
+template <class T>
+const T* staged(const kt_ctx* c, size_t at) {  // piece at `at` of a call's staged copy (stage_pieces), on the device
+  return reinterpret_cast<const T*>(c->d_call_in.as<unsigned char>() + at);
+}
 
 // The library's last launch on each stream, while that launch is a fused k_pass: evaluate_locked lets the next fused pass start
 // its first phase early only behind one (k_pass).  Every other library call that queues work on a stream forgets the stream's
@@ -905,7 +913,8 @@ void kt_destroy(kt_ctx* c) {
                    &c->d_st_used, &c->d_st_used_present, &c->d_st_used_cnt, &c->d_st_throttled, &c->d_reserved, &c->d_reserved_present,
                    &c->d_reserved_cnt, &c->d_part, &c->d_sync, &c->d_trace, &c->d_pre, &c->d_changed, &c->d_col_idx, &c->d_col_cnt, &c->d_col_off,
                    &c->d_col_rows, &c->d_adm_state, &c->d_adm_fail, &c->d_adm_counters, &c->d_out, &c->d_codes, &c->d_admit,
-                   &c->d_key_reach, &c->d_key_scratch, &c->d_key_acc, &c->d_chk_pre, &c->d_call_in, &c->d_call_out, &c->d_nsspec};
+                   &c->d_key_reach, &c->d_key_scratch, &c->d_key_acc, &c->d_chk_pre, &c->d_call_in, &c->d_call_out, &c->d_nsspec,
+                   &c->s_ovr_off, &c->s_ovr_begin, &c->s_ovr_end, &c->s_ovr_flags, &c->s_ovr_thr, &c->s_ovr_present, &c->s_ovr_cnt};
   c->h_call.release();
   c->h_step.release();
   if (c->ev_step) cudaEventDestroy(c->ev_step);
@@ -1263,6 +1272,8 @@ int kt_upload_throttles(kt_ctx* c, int32_t m, const kt_throttle_cols* cols, cons
   const int R = c->lim.n_resources;
   c->M = m;
   c->n_ovr = n_ovr;
+  if (m > 0) c->h_ovr_off.assign(cols->ovr_off, cols->ovr_off + m + 1);
+  else c->h_ovr_off.assign(1, 0);
   if ((rc = upload(c, c->d_kind, cols->kind, (size_t)m)) || (rc = upload(c, c->d_tflags, cols->flags, (size_t)m)) ||
       (rc = upload(c, c->d_thr, cols->thr, (size_t)R * m)) || (rc = upload(c, c->d_thr_present, cols->thr_present, (size_t)m)) ||
       (rc = upload(c, c->d_thr_cnt, cols->thr_cnt, (size_t)m)) || (rc = upload(c, c->d_ovr_off, cols->ovr_off, (size_t)m + 1)) ||
@@ -1359,7 +1370,10 @@ int stage_pieces(kt_ctx* c, std::initializer_list<Piece> pieces, size_t* at) {
   KT_CUDA(c, c->h_call.reserve(total));
   KT_CUDA(c, c->d_call_in.reserve(total + 16));
   i = 0;
-  for (const Piece& p : pieces) std::memcpy(c->h_call.as<unsigned char>() + at[i++], p.src, p.bytes);
+  for (const Piece& p : pieces) {
+    if (p.bytes) std::memcpy(c->h_call.as<unsigned char>() + at[i], p.src, p.bytes);
+    ++i;
+  }
   KT_CUDA(c, cudaMemcpyAsync(c->d_call_in.p, c->h_call.p, total, cudaMemcpyHostToDevice, c->stream));
   return KT_OK;
 }
@@ -1431,6 +1445,95 @@ int kt_update_reserved_rows(kt_ctx* c, int64_t k, const int32_t* idx, const int6
   KT_CUDA(c, cudaStreamSynchronize(c->stream));  // the caller may reuse its buffers as soon as we return
   c->have_reserved = true;
   c->evaluated = false;
+  return KT_OK;
+}
+
+int kt_update_threshold_rows(kt_ctx* c, int64_t k, const int32_t* idx, const kt_throttle_cols* cols) {
+  if (!c) return KT_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(c->mu);
+  if (k < 0) return fail(c, KT_ERR_INVALID, "kt_update_threshold_rows: k = %lld", (long long)k);
+  if (k > 0 && (!idx || !cols || !cols->thr || !cols->thr_present || !cols->thr_cnt || !cols->ovr_off))
+    return fail(c, KT_ERR_INVALID, "kt_update_threshold_rows: null column with k = %lld", (long long)k);
+  if (cols && (cols->kind || cols->ns_id || cols->flags))
+    return fail(c, KT_ERR_INVALID, "kt_update_threshold_rows: kind, ns_id and flags feed the tables (kt_upload_throttles) and must be NULL");
+  if (!c->have_throttles) return fail(c, KT_ERR_STATE, "kt_update_threshold_rows before kt_upload_throttles");
+  if (k == 0) return KT_OK;
+  if (int rc = check_distinct_throttles(c, __func__, k, idx)) return rc;
+  const int32_t* in_off = cols->ovr_off;
+  const int32_t n_in = in_off[k];
+  if (in_off[0] != 0 || n_in != cols->n_ovr) return fail(c, KT_ERR_INVALID, "kt_update_threshold_rows: ovr_off must span [0, n_ovr]");
+  for (int64_t i = 0; i < k; ++i)
+    if (in_off[i] > in_off[i + 1]) return fail(c, KT_ERR_INVALID, "kt_update_threshold_rows: ovr_off not monotone");
+  if (n_in > 0 && (!cols->ovr_begin || !cols->ovr_end || !cols->ovr_flags || !cols->ovr_thr || !cols->ovr_present || !cols->ovr_cnt))
+    return fail(c, KT_ERR_INVALID, "kt_update_threshold_rows: null override columns");
+  const int R = c->lim.n_resources, M = c->M;
+  const std::vector<int32_t>& old_off = c->h_ovr_off;
+  bool same_counts = true;
+  for (int64_t i = 0; i < k && same_counts; ++i) same_counts = in_off[i + 1] - in_off[i] == old_off[(size_t)idx[i] + 1] - old_off[(size_t)idx[i]];
+  // the new layout when some count changes: every column keeps its count but the listed ones
+  std::vector<int32_t> new_off, sorted, pos;
+  if (!same_counts) {
+    std::vector<int64_t> cnt((size_t)M);
+    for (int t = 0; t < M; ++t) cnt[(size_t)t] = old_off[(size_t)t + 1] - old_off[(size_t)t];
+    for (int64_t i = 0; i < k; ++i) cnt[(size_t)idx[i]] = in_off[i + 1] - in_off[i];
+    new_off.assign((size_t)M + 1, 0);
+    int64_t run = 0;
+    for (int t = 0; t < M; ++t) {
+      run += cnt[(size_t)t];
+      if (run > INT32_MAX) return fail(c, KT_ERR_INVALID, "kt_update_threshold_rows: more than 2^31-1 overrides");
+      new_off[(size_t)t + 1] = (int32_t)run;
+    }
+    std::vector<std::pair<int32_t, int32_t>> by_col((size_t)k);
+    for (int64_t i = 0; i < k; ++i) by_col[(size_t)i] = {idx[i], (int32_t)i};
+    std::sort(by_col.begin(), by_col.end());
+    for (auto& p : by_col) { sorted.push_back(p.first); pos.push_back(p.second); }
+  }
+  int rc = set_device(c);
+  if (rc) return rc;
+  const size_t K = (size_t)k, N = (size_t)n_in;
+  size_t at[14];
+  if ((rc = stage_pieces(c, {{idx, K * 4}, {cols->thr, (size_t)R * K * 8}, {cols->thr_present, K * 4}, {cols->thr_cnt, K * 8}, {in_off, (K + 1) * 4},
+                             {cols->ovr_begin, N * 8}, {cols->ovr_end, N * 8}, {cols->ovr_flags, N}, {cols->ovr_thr, (size_t)R * N * 8},
+                             {cols->ovr_present, N * 4}, {cols->ovr_cnt, N * 8}, {new_off.data(), new_off.size() * 4}, {sorted.data(), sorted.size() * 4},
+                             {pos.data(), pos.size() * 4}}, at)))
+    return rc;
+  OverrideCols src{staged<int64_t>(c, at[5]), staged<int64_t>(c, at[6]), staged<uint8_t>(c, at[7]), staged<int64_t>(c, at[8]),
+                   staged<uint32_t>(c, at[9]), staged<int64_t>(c, at[10]), n_in};
+  OverrideOut resident{c->d_ovr_begin.as<int64_t>(), c->d_ovr_end.as<int64_t>(), c->d_ovr_flags.as<uint8_t>(), c->d_ovr_thr.as<int64_t>(),
+                       c->d_ovr_present.as<uint32_t>(), c->d_ovr_cnt.as<int64_t>(), c->n_ovr};
+  k_scatter_thresholds<<<(unsigned)((k + 127) / 128), 128, 0, c->stream>>>(
+      k, staged<int32_t>(c, at[0]), R, M, staged<int64_t>(c, at[1]), staged<uint32_t>(c, at[2]), staged<int64_t>(c, at[3]),
+      staged<int32_t>(c, at[4]), src, c->d_ovr_off.as<int32_t>(), same_counts, c->d_thr.as<int64_t>(), c->d_thr_present.as<uint32_t>(),
+      c->d_thr_cnt.as<int64_t>(), resident);
+  KT_CUDA(c, cudaGetLastError());
+  if (!same_counts) {
+    const int32_t n_new = new_off[(size_t)M];
+    const size_t n = (size_t)n_new;
+    KT_CUDA(c, c->s_ovr_off.reserve(((size_t)M + 1) * 4 + 16));
+    KT_CUDA(c, c->s_ovr_begin.reserve(n * 8 + 16));
+    KT_CUDA(c, c->s_ovr_end.reserve(n * 8 + 16));
+    KT_CUDA(c, c->s_ovr_flags.reserve(n + 16));
+    KT_CUDA(c, c->s_ovr_thr.reserve((size_t)R * n * 8 + 16));
+    KT_CUDA(c, c->s_ovr_present.reserve(n * 4 + 16));
+    KT_CUDA(c, c->s_ovr_cnt.reserve(n * 8 + 16));
+    const OverrideCols old{resident.begin, resident.end, resident.flags, resident.thr, resident.present, resident.cnt, resident.n};
+    const OverrideOut out{c->s_ovr_begin.as<int64_t>(), c->s_ovr_end.as<int64_t>(), c->s_ovr_flags.as<uint8_t>(), c->s_ovr_thr.as<int64_t>(),
+                          c->s_ovr_present.as<uint32_t>(), c->s_ovr_cnt.as<int64_t>(), n_new};
+    k_rebuild_overrides<<<(unsigned)((M + 1 + 127) / 128), 128, 0, c->stream>>>(
+        M, R, k, staged<int32_t>(c, at[12]), staged<int32_t>(c, at[13]), staged<int32_t>(c, at[11]), c->d_ovr_off.as<int32_t>(), old,
+        staged<int32_t>(c, at[4]), src, c->s_ovr_off.as<int32_t>(), out);
+    KT_CUDA(c, cudaGetLastError());
+    std::swap(c->d_ovr_off, c->s_ovr_off); std::swap(c->d_ovr_begin, c->s_ovr_begin); std::swap(c->d_ovr_end, c->s_ovr_end);
+    std::swap(c->d_ovr_flags, c->s_ovr_flags); std::swap(c->d_ovr_thr, c->s_ovr_thr); std::swap(c->d_ovr_present, c->s_ovr_present);
+    std::swap(c->d_ovr_cnt, c->s_ovr_cnt);
+    c->n_ovr = n_new;
+    c->h_ovr_off.swap(new_off);
+  }
+  KT_CUDA(c, cudaStreamSynchronize(c->stream));  // the caller may reuse its buffers as soon as we return
+  // as after kt_upload_throttles: a pass is needed again before the getters that read one (status and reservations are kept)
+  c->evaluated = false;
+  c->have_codes = false;
+  c->have_diff = false;
   return KT_OK;
 }
 

@@ -38,6 +38,7 @@
 #pragma weak kt_update_status_rows    // without them (older engine doubles) sync_status / sync_reserved upload whole tables
 #pragma weak kt_update_reserved_rows
 #pragma weak kt_update_namespace_rows  // without it (older engine doubles) every Namespace event uploads all namespace rows
+#pragma weak kt_update_threshold_rows  // without it (older engine doubles) every threshold or override edit recompiles the tables
 
 namespace {
 
@@ -539,6 +540,8 @@ struct kth_plugin {
   }
   // status_dirty / reserved_dirty: the next sync uploads every column (the engine holds none, or the columns' layout or scale
   // changed).  Otherwise the columns listed in status_cols / reserved_cols go alone (kt_update_status_rows / _reserved_rows).
+  // spec_cols: the columns whose threshold or overrides changed and nothing else of the spec (kt_update_threshold_rows, unless
+  // the throttles are uploaded whole anyway).
   bool throttles_dirty = true, namespaces_dirty = true, status_dirty = true, reserved_dirty = true;
   // namespaces_dirty: the next sync sends namespace rows -- all of them with namespaces_full (the engine holds none, the label
   // encoding changed, or the tables are compiled again anyway), else only the rows in ns_dirty (kt_update_namespace_rows).
@@ -555,7 +558,7 @@ struct kth_plugin {
       for (size_t t : list) in[t] = 0;
       list.clear();
     }
-  } status_cols, reserved_cols;
+  } status_cols, reserved_cols, spec_cols;
   uint64_t col_epoch = 0;  // bumped whenever a resource column is added or changes its scale: every packed column may change
   std::vector<size_t> broken;  // columns of the throttles with a podSelector that does not convert (controller_error)
   bool broken_valid = false;
@@ -1022,16 +1025,9 @@ struct kth_plugin {
     queue_void();
     words_stat = -1;
     reorder_columns();
-    const int R = lim.n_resources;
     const size_t m = throttles.size();
     std::vector<uint8_t> kind(m), flags(m);
-    std::vector<int32_t> nsid(m), ovr_off(m + 1, 0);
-    std::vector<int64_t> thr((size_t)R * std::max<size_t>(m, 1), 0), thr_cnt(m, 0);
-    std::vector<uint32_t> thr_present(m, 0);
-    std::vector<int64_t> ovr_begin, ovr_end, ovr_cnt;
-    std::vector<uint8_t> ovr_flags;
-    std::vector<uint32_t> ovr_present;
-    std::vector<std::vector<int64_t>> ovr_vals;  // per override: R values
+    std::vector<int32_t> nsid(m);
     std::vector<int32_t> term_off(m + 1, 0), pod_req_off{0}, ns_req_off, req_val_off{0};
     std::vector<uint8_t> term_flags, req_op;
     std::vector<uint32_t> req_key, req_vals;
@@ -1045,40 +1041,12 @@ struct kth_plugin {
         req_val_off.push_back((int32_t)req_vals.size());
       }
     };
-    auto amount_cols = [&](const ResAmount& a, int64_t* vals, size_t stride, uint32_t* present, int64_t* cnt) {
-      *present = 0;
-      *cnt = 0;
-      if (a.has_counts) { *present |= KT_COUNT_BIT; *cnt = a.pod; }
-      for (auto& kv : a.requests) {
-        vals[(size_t)kv.first * stride] = at_scale(kv.first, kv.second);
-        *present |= 1u << kv.first;
-      }
-    };
     for (size_t t = 0; t < m; ++t) {
       const ThrottleObj& o = throttles[t];
       kind[t] = (uint8_t)o.kind;
       nsid[t] = o.kind == KT_KIND_THROTTLE ? ns_id(o.ns) : -1;
       flags[t] = 0;
       if (o.live && o.throttler_name == name) flags[t] |= KT_THR_RESPONSIBLE;  // isResponsibleFor, throttle_controller.go:213-215
-      amount_cols(o.threshold, &thr[t], m, &thr_present[t], &thr_cnt[t]);
-      for (size_t i = 0; i < o.overrides.size(); ++i) {
-        const Override& ov = o.overrides[i];
-        GoTime b, e;
-        uint8_t f = 0;
-        if (!ov.begin.empty() && !parse_rfc3339(ov.begin, &b).empty()) f = KT_OVR_PARSE_ERROR;
-        if (!ov.end.empty() && !parse_rfc3339(ov.end, &e).empty()) f = KT_OVR_PARSE_ERROR;
-        ovr_begin.push_back(b.zero ? KT_TIME_OPEN_BEGIN : clamp_ns(b.ns()));
-        ovr_end.push_back(e.zero ? KT_TIME_OPEN_END : clamp_ns(e.ns()));
-        ovr_flags.push_back(f);
-        std::vector<int64_t> vals((size_t)R, 0);
-        uint32_t pr;
-        int64_t cnt;
-        amount_cols(ov.threshold, vals.data(), 1, &pr, &cnt);
-        ovr_vals.push_back(std::move(vals));
-        ovr_present.push_back(pr);
-        ovr_cnt.push_back(cnt);
-      }
-      ovr_off[t + 1] = (int32_t)ovr_begin.size();
       for (auto& term : o.terms) {
         // a podSelector that does not convert: the term matches nobody and shadows the LATER terms for exactly the pods that
         // reach it (KT_TERM_POD_INVALID; the table compiler scopes that by namespace / namespaceSelector)
@@ -1104,14 +1072,9 @@ struct kth_plugin {
       push_reqs(reqs);
       ns_req_off.push_back((int32_t)req_key.size());
     }
-    const size_t n_ovr = ovr_begin.size();
-    std::vector<int64_t> ovr_thr((size_t)R * std::max<size_t>(n_ovr, 1), 0);
-    for (size_t i = 0; i < n_ovr; ++i)
-      for (int r = 0; r < R; ++r) ovr_thr[(size_t)r * n_ovr + i] = ovr_vals[i][(size_t)r];
-    kt_throttle_cols tc{};
-    tc.kind = kind.data(); tc.ns_id = nsid.data(); tc.flags = flags.data(); tc.thr = thr.data(); tc.thr_present = thr_present.data();
-    tc.thr_cnt = thr_cnt.data(); tc.ovr_off = ovr_off.data(); tc.n_ovr = (int32_t)n_ovr; tc.ovr_begin = ovr_begin.data(); tc.ovr_end = ovr_end.data();
-    tc.ovr_flags = ovr_flags.data(); tc.ovr_thr = ovr_thr.data(); tc.ovr_present = ovr_present.data(); tc.ovr_cnt = ovr_cnt.data();
+    const ThresholdColumns tcols = threshold_columns(AllColumns{m});
+    kt_throttle_cols tc = tcols.cols();
+    tc.kind = kind.data(); tc.ns_id = nsid.data(); tc.flags = flags.data();
     kt_selector_table st{};
     st.n_terms = (int32_t)term_flags.size(); st.n_reqs = (int32_t)req_key.size(); st.n_vals = (int32_t)req_vals.size();
     st.term_off = term_off.data(); st.term_flags = term_flags.data(); st.pod_req_off = pod_req_off.data(); st.ns_req_off = ns_req_off.data();
@@ -1120,6 +1083,76 @@ struct kth_plugin {
     check(kt_upload_throttles(ctx, (int32_t)m, &tc, &st), "kt_upload_throttles");
     throttles_dirty = false;
     status_dirty = reserved_dirty = true;  // kt_upload_throttles forgets both
+    spec_cols.clear();
+  }
+  // The spec columns of the listed throttles that no compiled table reads: spec.threshold ([R][k] / [k]) and the
+  // temporaryThresholdOverrides in spec order (ovr_off[k+1], ovr_thr[R][n_ovr]).  kind, ns_id and flags stay null.
+  struct ThresholdColumns {
+    std::vector<int32_t> ovr_off;
+    std::vector<int64_t> thr, thr_cnt, ovr_begin, ovr_end, ovr_thr, ovr_cnt;
+    std::vector<uint32_t> thr_present, ovr_present;
+    std::vector<uint8_t> ovr_flags;
+    kt_throttle_cols cols() const {
+      kt_throttle_cols tc{};
+      tc.thr = thr.data(); tc.thr_present = thr_present.data(); tc.thr_cnt = thr_cnt.data(); tc.ovr_off = ovr_off.data();
+      tc.n_ovr = ovr_off.back(); tc.ovr_begin = ovr_begin.data(); tc.ovr_end = ovr_end.data(); tc.ovr_flags = ovr_flags.data();
+      tc.ovr_thr = ovr_thr.data(); tc.ovr_present = ovr_present.data(); tc.ovr_cnt = ovr_cnt.data();
+      return tc;
+    }
+  };
+  template <class List>
+  ThresholdColumns threshold_columns(const List& list) const {
+    const int R = lim.n_resources;
+    const size_t k = list.size();
+    ThresholdColumns tc;
+    tc.ovr_off.assign(k + 1, 0);
+    tc.thr.assign((size_t)R * std::max<size_t>(k, 1), 0); tc.thr_cnt.assign(k, 0); tc.thr_present.assign(k, 0);
+    std::vector<std::vector<int64_t>> ovr_vals;  // per override: R values
+    auto amount_cols = [&](const ResAmount& a, int64_t* vals, size_t stride, uint32_t* present, int64_t* cnt) {
+      *present = 0;
+      *cnt = 0;
+      if (a.has_counts) { *present |= KT_COUNT_BIT; *cnt = a.pod; }
+      for (auto& kv : a.requests) {
+        vals[(size_t)kv.first * stride] = at_scale(kv.first, kv.second);
+        *present |= 1u << kv.first;
+      }
+    };
+    for (size_t i = 0; i < k; ++i) {
+      const ThrottleObj& o = throttles[list[i]];
+      amount_cols(o.threshold, &tc.thr[i], k, &tc.thr_present[i], &tc.thr_cnt[i]);
+      for (const Override& ov : o.overrides) {
+        GoTime b, e;
+        uint8_t f = 0;
+        if (!ov.begin.empty() && !parse_rfc3339(ov.begin, &b).empty()) f = KT_OVR_PARSE_ERROR;
+        if (!ov.end.empty() && !parse_rfc3339(ov.end, &e).empty()) f = KT_OVR_PARSE_ERROR;
+        tc.ovr_begin.push_back(b.zero ? KT_TIME_OPEN_BEGIN : clamp_ns(b.ns()));
+        tc.ovr_end.push_back(e.zero ? KT_TIME_OPEN_END : clamp_ns(e.ns()));
+        tc.ovr_flags.push_back(f);
+        std::vector<int64_t> vals((size_t)R, 0);
+        uint32_t pr;
+        int64_t cnt;
+        amount_cols(ov.threshold, vals.data(), 1, &pr, &cnt);
+        ovr_vals.push_back(std::move(vals));
+        tc.ovr_present.push_back(pr);
+        tc.ovr_cnt.push_back(cnt);
+      }
+      tc.ovr_off[i + 1] = (int32_t)tc.ovr_begin.size();
+    }
+    const size_t n_ovr = tc.ovr_begin.size();
+    tc.ovr_thr.assign((size_t)R * std::max<size_t>(n_ovr, 1), 0);
+    for (size_t i = 0; i < n_ovr; ++i)
+      for (int r = 0; r < R; ++r) tc.ovr_thr[(size_t)r * n_ovr + i] = ovr_vals[i][(size_t)r];
+    return tc;
+  }
+  // Threshold and override edits that left the tables alone: one kt_update_threshold_rows for the listed columns.  No "more than
+  // half dirty" rule here: the alternative is a table recompile, never cheaper.
+  void sync_thresholds() {
+    if (spec_cols.list.empty()) return;
+    const ThresholdColumns tcols = threshold_columns(spec_cols.list);
+    const kt_throttle_cols tc = tcols.cols();
+    const std::vector<int32_t> idx(spec_cols.list.begin(), spec_cols.list.end());
+    check(kt_update_threshold_rows(ctx, (int64_t)idx.size(), idx.data(), &tc), "kt_update_threshold_rows");
+    spec_cols.clear();
   }
 
   // Whether the dirty columns go as a delta (the callers check first that no full upload is pending): the engine has the call and
@@ -1266,6 +1299,7 @@ struct kth_plugin {
     sync_pods();
     sync_namespaces();
     sync_throttles();
+    sync_thresholds();  // (after sync_throttles, which sends these columns too when it uploads the throttles)
   }
   // Everything a PreFilter view reads: the tables, the informer copy of the statuses and the reservations.  A table change voids
   // the cached queue verdicts on the way (sync_namespaces / sync_throttles); afterwards no dirty flag is set.
@@ -2817,14 +2851,19 @@ struct kth_plugin {
       if (a.reqs[i].key != b.reqs[i].key || a.reqs[i].op != b.reqs[i].op || a.reqs[i].values != b.reqs[i].values) return false;
     return true;
   }
-  static bool same_spec(const ThrottleObj& a, const ThrottleObj& b) {
-    if (a.kind != b.kind || a.ns != b.ns || a.throttler_name != b.throttler_name || !amount_equal(a.threshold, b.threshold)) return false;
-    if (a.overrides.size() != b.overrides.size() || a.terms.size() != b.terms.size()) return false;
+  // What compile_tables and the column layout read: kind, namespace, throttlerName (the responsibility flag) and the terms.
+  static bool same_tables(const ThrottleObj& a, const ThrottleObj& b) {
+    if (a.kind != b.kind || a.ns != b.ns || a.throttler_name != b.throttler_name || a.terms.size() != b.terms.size()) return false;
+    for (size_t i = 0; i < a.terms.size(); ++i)
+      if (!same_selector(a.terms[i].pod_sel, b.terms[i].pod_sel) || !same_selector(a.terms[i].ns_sel, b.terms[i].ns_sel)) return false;
+    return true;
+  }
+  // What threshold_columns reads: spec.threshold and the temporaryThresholdOverrides.
+  static bool same_threshold_columns(const ThrottleObj& a, const ThrottleObj& b) {
+    if (!amount_equal(a.threshold, b.threshold) || a.overrides.size() != b.overrides.size()) return false;
     for (size_t i = 0; i < a.overrides.size(); ++i)
       if (a.overrides[i].begin != b.overrides[i].begin || a.overrides[i].end != b.overrides[i].end || !amount_equal(a.overrides[i].threshold, b.overrides[i].threshold))
         return false;
-    for (size_t i = 0; i < a.terms.size(); ++i)
-      if (!same_selector(a.terms[i].pod_sel, b.terms[i].pod_sel) || !same_selector(a.terms[i].ns_sel, b.terms[i].ns_sel)) return false;
     return true;
   }
   // apiequality.Semantic.DeepEqual on two ThrottleStatus values (empty maps are nil maps)
@@ -2901,15 +2940,21 @@ struct kth_plugin {
         o.st_calc = old.st_calc; o.st_calc_at_set = old.st_calc_at_set; o.st_calc_at = old.st_calc_at; o.st_messages = old.st_messages;
         o.st_thr_pod = old.st_thr_pod; o.st_thr_req = old.st_thr_req; o.st_thr_req_nil = old.st_thr_req_nil; o.st_used = old.st_used;
       }
-      // The same spec (a status echoed back by the informer after reconcile's UpdateStatus, or written by another replica): the
-      // tables and the spec columns stay; only this column's status is sent again, and only the cached verdicts of the pods this
-      // throttle affects are void.
-      const bool spec_kept = epoch == col_epoch && same_spec(old, o), status_kept = same_status(old, o);
+      // The same tables (a status echoed back by the informer after reconcile's UpdateStatus, or written by another replica; an
+      // edit of the threshold or the overrides): the tables stay; only this column's status and threshold columns are sent
+      // again, when they changed, and only the cached verdicts of the pods this throttle affects are void.
+      const size_t t = (size_t)it->second;
+      const bool tables_kept = epoch == col_epoch && same_tables(old, o), thresholds_kept = same_threshold_columns(old, o),
+                 status_kept = same_status(old, o);
       old = std::move(o);
-      if (spec_kept) {
+      if (tables_kept && (thresholds_kept || (kt_update_threshold_rows && !throttles_dirty))) {
+        if (!thresholds_kept) {
+          spec_cols.add(t);
+          throttle_state_changed(t);
+        }
         if (!status_kept) {
-          status_cols.add((size_t)it->second);
-          throttle_state_changed((size_t)it->second);
+          status_cols.add(t);
+          throttle_state_changed(t);
         }
         return;
       }

@@ -2159,6 +2159,61 @@ __global__ void __launch_bounds__(128) k_scatter_reserved(int64_t k, const int32
   present[t] = src_present[i];
   cnt[t] = src_cnt[i];
 }
+// Threshold column deltas (kt_update_threshold_rows).  The override entries of a set of columns: n entries, ovr_thr strided by n.
+struct OverrideCols {
+  const int64_t* begin; const int64_t* end; const uint8_t* flags; const int64_t* thr; const uint32_t* present; const int64_t* cnt;
+  int32_t n;
+};
+struct OverrideOut {
+  int64_t* begin; int64_t* end; uint8_t* flags; int64_t* thr; uint32_t* present; int64_t* cnt;
+  int32_t n;
+};
+__device__ __forceinline__ void copy_override(const OverrideOut& d, int32_t j, const OverrideCols& s, int32_t e, int R) {
+  d.begin[j] = s.begin[e];
+  d.end[j] = s.end[e];
+  d.flags[j] = s.flags[e];
+  d.present[j] = s.present[e];
+  d.cnt[j] = s.cnt[e];
+  for (int r = 0; r < R; ++r) d.thr[(size_t)r * d.n + j] = s.thr[(size_t)r * s.n + e];
+}
+// Column i of k staged columns -> column idx[i]: spec.threshold, and -- when `ovr` is set (no listed column changes its number of
+// overrides, so every entry keeps its position) -- its overrides in place at the resident offsets.  The idx are distinct.
+__global__ void __launch_bounds__(128) k_scatter_thresholds(int64_t k, const int32_t* __restrict__ idx, int R, int M, const int64_t* __restrict__ src_thr,
+                                                            const uint32_t* __restrict__ src_present, const int64_t* __restrict__ src_cnt,
+                                                            const int32_t* __restrict__ src_off, const OverrideCols src, const int32_t* __restrict__ ovr_off,
+                                                            bool ovr, int64_t* thr, uint32_t* present, int64_t* cnt, const OverrideOut dst) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= k) return;
+  const int t = idx[i];
+  for (int r = 0; r < R; ++r) thr[(size_t)r * M + t] = src_thr[(size_t)r * k + i];
+  present[t] = src_present[i];
+  cnt[t] = src_cnt[i];
+  if (!ovr) return;
+  for (int32_t e = src_off[i], j = ovr_off[t]; e < src_off[i + 1]; ++e, ++j) copy_override(dst, j, src, e, R);
+}
+// Some listed column changes its number of overrides: every entry may move.  Column t of the new layout (new_off[M+1]) takes its
+// entries from the staged input when it is listed (sorted[] holds the listed columns in ascending order, pos[] each one's index in
+// the staged input, whose offsets are src_off[k+1]), else from its old position (old_off); they land in a spare set of columns.
+__global__ void __launch_bounds__(128) k_rebuild_overrides(int M, int R, int64_t k, const int32_t* __restrict__ sorted, const int32_t* __restrict__ pos,
+                                                           const int32_t* __restrict__ new_off, const int32_t* __restrict__ old_off, const OverrideCols old,
+                                                           const int32_t* __restrict__ src_off, const OverrideCols src, int32_t* out_off, const OverrideOut out) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t > M) return;
+  out_off[t] = new_off[t];
+  if (t == M) return;
+  int64_t lo = 0, hi = k;  // first listed column >= t
+  while (lo < hi) {
+    const int64_t mid = (lo + hi) >> 1;
+    if (sorted[mid] < t) lo = mid + 1;
+    else hi = mid;
+  }
+  const int32_t j0 = new_off[t], j1 = new_off[t + 1];
+  if (lo < k && sorted[lo] == t) {
+    for (int32_t j = j0, e = src_off[pos[lo]]; j < j1; ++j, ++e) copy_override(out, j, src, e, R);
+  } else {
+    for (int32_t j = j0, e = old_off[t]; j < j1; ++j, ++e) copy_override(out, j, old, e, R);
+  }
+}
 
 __global__ void __launch_bounds__(256) k_gather_bytes(int64_t k, const int64_t* __restrict__ rows, const unsigned char* __restrict__ src, unsigned char* __restrict__ out) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
