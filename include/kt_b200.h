@@ -331,6 +331,26 @@ int kt_update_reserved_rows(kt_ctx* ctx, int64_t k, const int32_t* idx, const in
  * the host, travel with the copy (O(M) bytes) and the override columns are rebuilt on the device.  Multi-GPU: the call is
  * local, not collective -- every rank must apply the same updates. */
 int kt_update_threshold_rows(kt_ctx* ctx, int64_t k, const int32_t* idx, const kt_throttle_cols* cols);
+/* Column deltas of the compiled side of the spec: a deletion (zero terms, flags 0), a podSelector / namespaceSelector edit or a
+ * throttlerName change (KT_THR_RESPONSIBLE) of a few columns, with M and every column's position kept.  cols carries kind[k],
+ * ns_id[k] and flags[k] of the k listed columns; its threshold and override pointers belong to kt_update_threshold_rows and must
+ * be NULL.  sel is a CSR over the k listed columns, in idx order, shaped as for kt_upload_throttles.  Afterwards every call
+ * answers exactly as after a kt_upload_throttles whose spec is the previous one with the listed columns' kind, ns_id, flags and
+ * selector terms replaced (threshold and override columns kept), followed by re-uploading the status and the reservations held
+ * before the call (when they were held).  The state flags move as kt_upload_throttles moves them (a pass is needed again before
+ * the getters that read one, and the next pass zero-fills its bitmap rows).  *recompiled (may be NULL) is 1 when the call
+ * compiled the tables again, 0 when it patched them in place.
+ * KT_ERR_INVALID: k < 0; a null idx, kind, ns_id, flags, sel or term_off with k > 0; a non-null threshold or override pointer;
+ * an index out of [0, M) or listed twice; a malformed CSR.  KT_ERR_STATE before kt_upload_throttles; k = 0 is a no-op.
+ * In place when every listed column fits the resident tables -- its podSelector keys and (key, value) pairs have table rows,
+ * its term count fits TPpad, its need fits the counter planes, a Throttle's namespace is below the resident namespace count --:
+ * the listed columns' table and need bits are recompiled on the host (the code compile_tables uses for one column) and only
+ * their 32-throttle word slices cross, in one staged copy; the namespace masks of those words are evaluated again for every
+ * namespace on the device and the word lists rebuilt; the pod rows keep their table offsets.  Otherwise the tables are
+ * compiled again from the patched spec, as kt_upload_namespaces does.  One synchronisation; the caller may reuse its buffers on
+ * return.  Multi-GPU: the call is local, not collective -- every rank must apply the same updates. */
+int kt_update_selector_rows(kt_ctx* ctx, int64_t k, const int32_t* idx, const kt_throttle_cols* cols,
+                            const kt_selector_table* sel, int32_t* recompiled);
 
 /* ---- the pass ------------------------------------------------------------------- */
 /* One batched pass: reconcile every throttle (throttle_controller.go:84-133) and check

@@ -159,7 +159,10 @@ int64_t kth_pod_row(kth_plugin* p, const char* ns, const char* name);
 const char* kth_last_error(void);
 /* {"queued":n,"rows":r,"passes":device passes over the queue so far,"hits":by-key calls answered from cached verdicts,
  *  "throttleColumns":device columns the throttles occupy (deleted throttles' columns are reused),"liveThrottles":m,
- *  "labelKeys":k,"labelValues":v (the label dictionaries: what the selectors mention),"resourceColumns":c} */
+ *  "labelKeys":k,"labelValues":v (the label dictionaries: what the selectors mention),"resourceColumns":c,
+ *  "wordsPerNamespaceX100":32-throttle words a namespace's pods visit, x100}.  A deletion or selector edit applied as a column
+ * delta keeps its column until the next whole upload: passes, hits, throttleColumns and wordsPerNamespaceX100 may differ from a
+ * plugin that uploads every change whole (they reflect the last whole upload, holes included); every other result is the same. */
 const char* kth_queue_stats(kth_plugin* p);
 
 /* Queue-ordered admission: PreFilter and, on Success, Reserve for every pod of a SORTED scheduling queue, with exactly

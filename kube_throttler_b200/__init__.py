@@ -43,7 +43,7 @@ def build(force: bool = False) -> str:
 EXPORTS = [
     "kt_create", "kt_destroy", "kt_last_error", "kt_version", "kt_set_stream", "kt_sync", "kt_enable_timing",
     "kt_enable_trace", "kt_get_trace", "kt_host_alloc", "kt_host_alloc_upload", "kt_host_free", "kt_upload_pods", "kt_upload_pods_compact", "kt_upload_pods_packed", "kt_set_async_uploads", "kt_update_pod_rows", "kt_upload_namespaces", "kt_update_namespace_rows",
-    "kt_upload_throttles", "kt_upload_status", "kt_set_reserved", "kt_update_status_rows", "kt_update_reserved_rows", "kt_update_threshold_rows", "kt_evaluate", "kt_get_reconcile",
+    "kt_upload_throttles", "kt_upload_status", "kt_set_reserved", "kt_update_status_rows", "kt_update_reserved_rows", "kt_update_threshold_rows", "kt_update_selector_rows", "kt_evaluate", "kt_get_reconcile",
     "kt_match_words", "kt_get_match_bitmap", "kt_get_match_rows", "kt_get_match_columns", "kt_get_check_summary", "kt_reconcile_throttles", "kt_get_check", "kt_set_sparse_check", "kt_get_check_sparse", "kt_get_check_rows", "kt_check_pending_rows", "kt_match_pods", "kt_check_pods", "kt_get_changed", "kt_get_reconcile_rows", "kt_step_submit", "kt_step_wait", "kt_admit_queue", "kt_get_timing", "kt_comm_unique_id",
     "kt_comm_init", "kt_comm_destroy", "kt_debug_compile_tables", "kt_debug_set_pass_plan", "kt_debug_get_pass_plan", "kt_debug_get_ns_tables",
     "kt_debug_set_row_order", "kt_debug_get_row_order",
@@ -101,6 +101,7 @@ def lib():
         L.kt_update_status_rows.argtypes = [vp, C.c_int64, vp, C.POINTER(abi.StatusCols)]
         L.kt_update_reserved_rows.argtypes = [vp, C.c_int64, vp, vp, vp, vp]
         L.kt_update_threshold_rows.argtypes = [vp, C.c_int64, vp, C.POINTER(abi.ThrottleCols)]
+        L.kt_update_selector_rows.argtypes = [vp, C.c_int64, vp, C.POINTER(abi.ThrottleCols), C.POINTER(abi.SelectorTable), vp]
         L.kt_evaluate.argtypes = [vp, C.c_int64, C.c_uint32]
         L.kt_get_reconcile.argtypes = [vp, C.POINTER(abi.ReconcileOut)]
         L.kt_match_words.argtypes = [vp]
@@ -317,6 +318,26 @@ class Engine:
                               abi.ptr(a["ovr_begin"]), abi.ptr(a["ovr_end"]), abi.ptr(a["ovr_flags"]), abi.ptr(a["ovr_thr"]),
                               abi.ptr(a["ovr_present"]), abi.ptr(a["ovr_cnt"]))
         self._ck(self._L.kt_update_threshold_rows(self._h, k, abi.ptr(idx), C.byref(tc)))
+
+    def update_selector_rows(self, idx: np.ndarray, cols: dict) -> bool:
+        """kt_update_selector_rows: kind, ns_id, flags and the selector terms of the listed throttle columns replaced (a deletion is
+        zero terms and flags 0).  `cols` holds the k listed columns: kind[k], thr_ns[k], thr_flags[k], and a CSR over them in idx
+        order named like the Snapshot fields -- term_off[k+1], term_flags, pod_req_off, ns_req_off, req_key, req_op, req_val_off,
+        req_vals.  Returns whether the engine compiled the tables again (a column did not fit the resident tables)."""
+        idx = np.ascontiguousarray(idx, np.int32)
+        k = idx.shape[0]
+        a = dict(kind=abi._arr(cols["kind"], np.uint8), ns=abi._arr(cols["thr_ns"], np.int32), flags=abi._arr(cols["thr_flags"], np.uint8),
+                 term_off=abi._arr(cols["term_off"], np.int32), term_flags=abi._arr(cols["term_flags"], np.uint8),
+                 pod_req_off=abi._arr(cols["pod_req_off"], np.int32), ns_req_off=abi._arr(cols["ns_req_off"], np.int32),
+                 req_key=abi._arr(cols["req_key"], np.uint32), req_op=abi._arr(cols["req_op"], np.uint8),
+                 req_val_off=abi._arr(cols["req_val_off"], np.int32), req_vals=abi._arr(cols["req_vals"], np.uint32))
+        tc = abi.ThrottleCols(abi.ptr(a["kind"]), abi.ptr(a["ns"]), abi.ptr(a["flags"]), None, None, None, None, 0, None, None, None, None,
+                              None, None)
+        st = abi.SelectorTable(int(a["term_off"][-1]) if a["term_off"].shape[0] else 0, int(a["req_key"].shape[0]), int(a["req_vals"].shape[0]),
+                               *(abi.ptr(a[f]) for f in ("term_off", "term_flags", "pod_req_off", "ns_req_off", "req_key", "req_op", "req_val_off", "req_vals")))
+        out = np.zeros(1, np.int32)
+        self._ck(self._L.kt_update_selector_rows(self._h, k, abi.ptr(idx), C.byref(tc), C.byref(st), abi.ptr(out)))
+        return bool(out[0])
 
     def update_reserved_rows(self, idx: np.ndarray, reserved: np.ndarray, present: np.ndarray, cnt: np.ndarray):
         """kt_update_reserved_rows: reserved[R][k], present[k], cnt[k] of the listed throttle columns, replaced in place (the

@@ -1538,6 +1538,41 @@ int kt_update_threshold_rows(kt_ctx* c, int64_t k, const int32_t* idx, const kt_
 }
 
 // ---- namespace row deltas (kt_nsrows.cuh) ---------------------------------------------------------------------------
+namespace {
+// After some nsmask entries changed on the device: the word lists of all NS namespaces rebuilt from nsmask (the caller reserved
+// d_nsw_off, d_nsw_idx and d_call_out for NS), the words inlined with the resident pod rows refreshed, and the total and the
+// longest list brought back through the call block at res_at with the call's one synchronisation.
+int rebuild_ns_words(kt_ctx* c, int32_t NS, size_t res_at) {
+  const int32_t W = c->ht.W, TPpad = c->ht.TPpad;
+  int32_t* out = c->d_call_out.as<int32_t>();  // {total, longest list, -, -}, then cnt[NS]
+  const unsigned ns_blocks = (unsigned)((NS + 7) / 8);
+  if (NS > 0) {
+    k_ns_count<<<ns_blocks, 256, 0, c->stream>>>(NS, W, TPpad, c->d_nsmask.as<uint32_t>(), out + 4);
+    KT_CUDA(c, cudaGetLastError());
+  }
+  k_ns_scan<<<1, kNsScanThreads, 0, c->stream>>>(NS, out + 4, c->d_nsw_off.as<int32_t>(), out);
+  KT_CUDA(c, cudaGetLastError());
+  if (NS > 0) {
+    k_ns_fill<<<ns_blocks, 256, 0, c->stream>>>(NS, W, TPpad, c->d_nsmask.as<uint32_t>(), c->d_nsw_off.as<int32_t>(), c->d_nsw_idx.as<int32_t>());
+    KT_CUDA(c, cudaGetLastError());
+  }
+  c->ht.NS = NS;
+  for (auto& s : c->pods) {  // the row offsets stay valid (the pod-label tables keep their rows); the inlined words may not
+    if (s.roff_valid && s.n > 0) {
+      k_ns_winfo<<<(unsigned)((s.n + 255) / 256), 256, 0, c->stream>>>(s.n, table_view(c), s.ns.as<int32_t>(), s.winfo.as<uint32_t>());
+      KT_CUDA(c, cudaGetLastError());
+    }
+    s.bitmap_clean = false;  // the word lists changed
+  }
+  int32_t* res = reinterpret_cast<int32_t*>(c->h_call.as<unsigned char>() + res_at);
+  KT_CUDA(c, cudaMemcpyAsync(res, out, 2 * sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
+  KT_CUDA(c, cudaStreamSynchronize(c->stream));  // the caller may reuse its buffers; the pass plan needs the longest list
+  c->nsw_total = res[0];
+  c->ht.max_ns_words = res[1];
+  return KT_OK;
+}
+}  // namespace
+
 int kt_update_namespace_rows(kt_ctx* c, int32_t n_ns, int64_t k, const int32_t* idx, const int64_t* labels) {
   if (!c) return KT_ERR_INVALID;
   std::lock_guard<std::mutex> lk(c->mu);
@@ -1600,7 +1635,6 @@ int kt_update_namespace_rows(kt_ctx* c, int32_t n_ns, int64_t k, const int32_t* 
   size_t at[3];
   if ((rc = stage_pieces(c, {{rows.data(), (size_t)kd * 4}, {lab.data(), lab.size() * 8}, {result_slot, sizeof result_slot}}, at))) return rc;
   const unsigned char* in = c->d_call_in.as<unsigned char>();
-  int32_t* out = c->d_call_out.as<int32_t>();  // {total, longest list, -, -}, then cnt[NS]
   const NsSpecView sp = ns_spec_view(c);
   for (int32_t y0 = 0; y0 < kd; y0 += 65535) {
     const dim3 grid((unsigned)((W + 7) / 8), (unsigned)std::min(kd - y0, 65535));
@@ -1608,27 +1642,131 @@ int kt_update_namespace_rows(kt_ctx* c, int32_t n_ns, int64_t k, const int32_t* 
                                            n_ns, c->d_nsmask.as<uint32_t>());
     KT_CUDA(c, cudaGetLastError());
   }
-  const unsigned ns_blocks = (unsigned)((NS + 7) / 8);
-  k_ns_count<<<ns_blocks, 256, 0, c->stream>>>(NS, W, TPpad, c->d_nsmask.as<uint32_t>(), out + 4);
-  KT_CUDA(c, cudaGetLastError());
-  k_ns_scan<<<1, kNsScanThreads, 0, c->stream>>>(NS, out + 4, c->d_nsw_off.as<int32_t>(), out);
-  KT_CUDA(c, cudaGetLastError());
-  k_ns_fill<<<ns_blocks, 256, 0, c->stream>>>(NS, W, TPpad, c->d_nsmask.as<uint32_t>(), c->d_nsw_off.as<int32_t>(), c->d_nsw_idx.as<int32_t>());
-  KT_CUDA(c, cudaGetLastError());
-  c->ht.NS = NS;
-  for (auto& s : c->pods) {  // the row offsets stay valid (the pod-label tables are unchanged); the inlined words may not
-    if (s.roff_valid && s.n > 0) {
-      k_ns_winfo<<<(unsigned)((s.n + 255) / 256), 256, 0, c->stream>>>(s.n, table_view(c), s.ns.as<int32_t>(), s.winfo.as<uint32_t>());
-      KT_CUDA(c, cudaGetLastError());
+  return rebuild_ns_words(c, NS, at[2]);
+}
+
+// ---- selector column deltas (kt_tables.cc patch_columns, kt_nsrows.cuh k_ns_cols) --------------------------------------
+namespace {
+// The spec with column idx[i] taking column i of d (kind, ns_id, flags and terms), the others as they were.  The CSR is laid out
+// again column by column: every term's podSelector requirements first, then every term's namespaceSelector ones.
+SelectorSpec splice_spec(const SelectorSpec& old, int64_t k, const int32_t* idx, const SelectorSpec& d) {
+  const int32_t M = old.m;
+  std::vector<int32_t> from((size_t)M, -1);
+  for (int64_t i = 0; i < k; ++i) from[(size_t)idx[i]] = (int32_t)i;
+  SelectorSpec s;
+  s.m = M;
+  s.kind = old.kind; s.flags = old.flags; s.ns_id = old.ns_id;
+  s.term_off.assign(1, 0);
+  std::vector<std::pair<const SelectorSpec*, int32_t>> terms;  // (source, term) in the new order
+  for (int32_t t = 0; t < M; ++t) {
+    const int32_t i = from[(size_t)t];
+    const SelectorSpec& src = i >= 0 ? d : old;
+    const int32_t col = i >= 0 ? i : t;
+    if (i >= 0) { s.kind[(size_t)t] = d.kind[(size_t)i]; s.flags[(size_t)t] = d.flags[(size_t)i]; s.ns_id[(size_t)t] = d.ns_id[(size_t)i]; }
+    for (int32_t term = src.term_off[(size_t)col]; term < src.term_off[(size_t)col + 1]; ++term) {
+      terms.emplace_back(&src, term);
+      s.term_flags.push_back(src.term_flags[(size_t)term]);
     }
-    s.bitmap_clean = false;  // the word lists changed
+    s.term_off.push_back((int32_t)terms.size());
   }
-  int32_t* res = reinterpret_cast<int32_t*>(c->h_call.as<unsigned char>() + at[2]);
-  KT_CUDA(c, cudaMemcpyAsync(res, out, 2 * sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
-  KT_CUDA(c, cudaStreamSynchronize(c->stream));  // the caller may reuse its buffers; the pass plan needs the longest list
-  c->nsw_total = res[0];
-  c->ht.max_ns_words = res[1];
-  return KT_OK;
+  s.req_val_off.assign(1, 0);
+  auto push_reqs = [&](const SelectorSpec& src, int32_t q0, int32_t q1) {
+    for (int32_t q = q0; q < q1; ++q) {
+      s.req_key.push_back(src.req_key[(size_t)q]);
+      s.req_op.push_back(src.req_op[(size_t)q]);
+      s.req_vals.insert(s.req_vals.end(), src.req_vals.begin() + src.req_val_off[(size_t)q], src.req_vals.begin() + src.req_val_off[(size_t)q + 1]);
+      s.req_val_off.push_back((int32_t)s.req_vals.size());
+    }
+  };
+  s.pod_req_off.assign(1, 0);
+  for (auto& st : terms) {
+    push_reqs(*st.first, st.first->pod_req_off[(size_t)st.second], st.first->pod_req_off[(size_t)st.second + 1]);
+    s.pod_req_off.push_back((int32_t)s.req_key.size());
+  }
+  s.ns_req_off.assign(1, (int32_t)s.req_key.size());
+  for (auto& st : terms) {
+    push_reqs(*st.first, st.first->ns_req_off[(size_t)st.second], st.first->ns_req_off[(size_t)st.second + 1]);
+    s.ns_req_off.push_back((int32_t)s.req_key.size());
+  }
+  return s;
+}
+}  // namespace
+
+int kt_update_selector_rows(kt_ctx* c, int64_t k, const int32_t* idx, const kt_throttle_cols* cols, const kt_selector_table* sel,
+                            int32_t* recompiled) {
+  if (!c) return KT_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(c->mu);
+  if (recompiled) *recompiled = 0;
+  if (k < 0) return fail(c, KT_ERR_INVALID, "kt_update_selector_rows: k = %lld", (long long)k);
+  if (k > 0 && (!idx || !cols || !cols->kind || !cols->ns_id || !cols->flags || !sel || !sel->term_off))
+    return fail(c, KT_ERR_INVALID, "kt_update_selector_rows: null column with k = %lld", (long long)k);
+  if (cols && (cols->thr || cols->thr_present || cols->thr_cnt || cols->ovr_off || cols->ovr_begin || cols->ovr_end || cols->ovr_flags ||
+               cols->ovr_thr || cols->ovr_present || cols->ovr_cnt))
+    return fail(c, KT_ERR_INVALID, "kt_update_selector_rows: threshold and override columns (kt_update_threshold_rows) must be NULL");
+  if (!c->have_throttles) return fail(c, KT_ERR_STATE, "kt_update_selector_rows before kt_upload_throttles");
+  if (k == 0) return KT_OK;
+  if (int rc = check_distinct_throttles(c, __func__, k, idx)) return rc;
+  SelectorSpec d;
+  const std::string e = copy_selector_spec((int32_t)k, cols, sel, &d);
+  if (!e.empty()) return fail(c, KT_ERR_INVALID, "kt_update_selector_rows: selector table: %s", e.c_str());
+  SelectorSpec spec = splice_spec(c->spec, k, idx, d);
+  int rc = set_device(c);
+  if (rc) return rc;
+  const bool fits = patch_columns(c->lim, c->spec, spec, std::vector<int32_t>(idx, idx + k), &c->ht);
+  c->spec = std::move(spec);
+  // as after kt_upload_throttles: a pass is needed again before the getters that read one (status and reservations are kept)
+  c->evaluated = false;
+  c->have_codes = false;
+  c->have_diff = false;
+  const size_t K = (size_t)k;
+  if (!fits) {  // the listed columns' kind and flags, then the tables compiled again from the patched spec (kt_upload_namespaces)
+    size_t at[3];
+    if ((rc = stage_pieces(c, {{idx, K * 4}, {cols->kind, K}, {cols->flags, K}}, at))) return rc;
+    k_scatter_kind_flags<<<(unsigned)((k + 127) / 128), 128, 0, c->stream>>>(k, staged<int32_t>(c, at[0]), staged<uint8_t>(c, at[1]), staged<uint8_t>(c, at[2]),
+                                                                           c->d_kind.as<uint8_t>(), c->d_tflags.as<uint8_t>());
+    KT_CUDA(c, cudaGetLastError());
+    if ((rc = recompile_tables(c)) || (rc = stage_ns_spec(c))) return rc;
+    KT_CUDA(c, cudaStreamSynchronize(c->stream));
+    if (recompiled) *recompiled = 1;
+    return KT_OK;
+  }
+  // the 32-throttle words the listed columns live in, ascending, and their recompiled table and need slices
+  std::vector<int32_t> words(idx, idx + k);
+  for (int32_t& w : words) w >>= 5;
+  std::sort(words.begin(), words.end());
+  words.erase(std::unique(words.begin(), words.end()), words.end());
+  const HostTables& h = c->ht;
+  const size_t nw = words.size(), tlen = (size_t)h.rows * h.TPpad * 2, nlen = (size_t)h.TPpad * h.B;
+  std::vector<uint32_t> tab(nw * tlen), nd(nw * nlen);
+  for (size_t j = 0; j < nw; ++j) {
+    std::copy(h.table.begin() + (size_t)words[j] * tlen, h.table.begin() + (size_t)(words[j] + 1) * tlen, tab.begin() + j * tlen);
+    std::copy(h.need.begin() + (size_t)words[j] * nlen, h.need.begin() + (size_t)(words[j] + 1) * nlen, nd.begin() + j * nlen);
+  }
+  const int32_t NS = h.NS, W = h.W, LN = c->lim.ns_label_slots;
+  KT_CUDA(c, c->d_nsw_off.reserve(((size_t)NS + 1) * 4 + 16));
+  // the unlisted words keep their entries, a listed word is in at most every list
+  KT_CUDA(c, c->d_nsw_idx.reserve(std::min((size_t)NS * W, (size_t)c->nsw_total + (size_t)NS * nw) * 4 + 16));
+  KT_CUDA(c, c->d_call_out.reserve(((size_t)NS + 4) * 4 + 16));
+  static const int32_t result_slot[4] = {};
+  size_t at[8];
+  if ((rc = stage_pieces(c, {{idx, K * 4}, {cols->kind, K}, {cols->flags, K}, {words.data(), nw * 4}, {tab.data(), tab.size() * 4},
+                             {nd.data(), nd.size() * 4}, {c->ns_labels.data(), c->ns_labels.size() * 8}, {result_slot, sizeof result_slot}}, at)))
+    return rc;
+  k_scatter_kind_flags<<<(unsigned)((k + 127) / 128), 128, 0, c->stream>>>(k, staged<int32_t>(c, at[0]), staged<uint8_t>(c, at[1]), staged<uint8_t>(c, at[2]),
+                                                                         c->d_kind.as<uint8_t>(), c->d_tflags.as<uint8_t>());
+  KT_CUDA(c, cudaGetLastError());
+  const unsigned tblocks = (unsigned)std::min<size_t>((nw * tlen + 255) / 256, 4096), nblocks = (unsigned)std::min<size_t>((nw * nlen + 255) / 256, 4096);
+  k_scatter_words<<<tblocks, 256, 0, c->stream>>>((int64_t)nw, staged<int32_t>(c, at[3]), (int64_t)tlen, staged<uint32_t>(c, at[4]), c->d_table.as<uint32_t>());
+  KT_CUDA(c, cudaGetLastError());
+  k_scatter_words<<<nblocks, 256, 0, c->stream>>>((int64_t)nw, staged<int32_t>(c, at[3]), (int64_t)nlen, staged<uint32_t>(c, at[5]), c->d_need.as<uint32_t>());
+  KT_CUDA(c, cudaGetLastError());
+  if ((rc = stage_ns_spec(c))) return rc;  // term ranges, requirements and ns_id of the patched spec
+  if (NS > 0) {
+    k_ns_cols<<<(unsigned)(((int64_t)NS * (int64_t)nw + 7) / 8), 256, 0, c->stream>>>(ns_spec_view(c), NS, (int32_t)nw, staged<int32_t>(c, at[3]),
+                                                                                       staged<int64_t>(c, at[6]), LN, c->n_ns, c->d_nsmask.as<uint32_t>());
+    KT_CUDA(c, cudaGetLastError());
+  }
+  return rebuild_ns_words(c, NS, at[7]);
 }
 
 int32_t kt_match_words(const kt_ctx* c) { return c && c->have_throttles ? c->ht.Wp : 0; }

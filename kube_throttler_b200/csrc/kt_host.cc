@@ -39,6 +39,7 @@
 #pragma weak kt_update_reserved_rows
 #pragma weak kt_update_namespace_rows  // without it (older engine doubles) every Namespace event uploads all namespace rows
 #pragma weak kt_update_threshold_rows  // without it (older engine doubles) every threshold or override edit recompiles the tables
+#pragma weak kt_update_selector_rows   // without it (older engine doubles) every deletion and selector edit recompiles the tables
 
 namespace {
 
@@ -541,7 +542,8 @@ struct kth_plugin {
   // status_dirty / reserved_dirty: the next sync uploads every column (the engine holds none, or the columns' layout or scale
   // changed).  Otherwise the columns listed in status_cols / reserved_cols go alone (kt_update_status_rows / _reserved_rows).
   // spec_cols: the columns whose threshold or overrides changed and nothing else of the spec (kt_update_threshold_rows, unless
-  // the throttles are uploaded whole anyway).
+  // the throttles are uploaded whole anyway).  sel_cols: the columns deleted, or whose terms or throttlerName changed, in place
+  // (kt_update_selector_rows, likewise).
   bool throttles_dirty = true, namespaces_dirty = true, status_dirty = true, reserved_dirty = true;
   // namespaces_dirty: the next sync sends namespace rows -- all of them with namespaces_full (the engine holds none, the label
   // encoding changed, or the tables are compiled again anyway), else only the rows in ns_dirty (kt_update_namespace_rows).
@@ -558,7 +560,7 @@ struct kth_plugin {
       for (size_t t : list) in[t] = 0;
       list.clear();
     }
-  } status_cols, reserved_cols, spec_cols;
+  } status_cols, reserved_cols, spec_cols, sel_cols;
   uint64_t col_epoch = 0;  // bumped whenever a resource column is added or changes its scale: every packed column may change
   std::vector<size_t> broken;  // columns of the throttles with a podSelector that does not convert (controller_error)
   bool broken_valid = false;
@@ -1026,34 +1028,64 @@ struct kth_plugin {
     words_stat = -1;
     reorder_columns();
     const size_t m = throttles.size();
-    std::vector<uint8_t> kind(m), flags(m);
-    std::vector<int32_t> nsid(m);
-    std::vector<int32_t> term_off(m + 1, 0), pod_req_off{0}, ns_req_off, req_val_off{0};
+    SelectorColumns scols = selector_columns(AllColumns{m});
+    const ThresholdColumns tcols = threshold_columns(AllColumns{m});
+    kt_throttle_cols tc = tcols.cols();
+    scols.put(&tc);
+    const kt_selector_table st = scols.table();
+    sync_namespaces();  // Throttle rows may have introduced namespace ids
+    check(kt_upload_throttles(ctx, (int32_t)m, &tc, &st), "kt_upload_throttles");
+    throttles_dirty = false;
+    status_dirty = reserved_dirty = true;  // kt_upload_throttles forgets both
+    spec_cols.clear();
+    sel_cols.clear();
+  }
+  // What compile_tables reads of the listed throttles: kind, ns_id, flags ([k]) and the selector CSR over them, in list order
+  // (requirement pool: all podSelector requirements in term order, then all namespaceSelector ones).  A deleted throttle's column
+  // has no terms and flags 0.
+  struct SelectorColumns {
+    std::vector<uint8_t> kind, flags;
+    std::vector<int32_t> nsid;
+    std::vector<int32_t> term_off{0}, pod_req_off{0}, ns_req_off, req_val_off{0};
     std::vector<uint8_t> term_flags, req_op;
     std::vector<uint32_t> req_key, req_vals;
+    void put(kt_throttle_cols* tc) const { tc->kind = kind.data(); tc->ns_id = nsid.data(); tc->flags = flags.data(); }
+    kt_selector_table table() const {
+      kt_selector_table st{};
+      st.n_terms = (int32_t)term_flags.size(); st.n_reqs = (int32_t)req_key.size(); st.n_vals = (int32_t)req_vals.size();
+      st.term_off = term_off.data(); st.term_flags = term_flags.data(); st.pod_req_off = pod_req_off.data(); st.ns_req_off = ns_req_off.data();
+      st.req_key = req_key.data(); st.req_op = req_op.data(); st.req_val_off = req_val_off.data(); st.req_vals = req_vals.data();
+      return st;
+    }
+  };
+  template <class List>
+  SelectorColumns selector_columns(const List& list) {
+    const size_t k = list.size();
+    SelectorColumns sc;
+    sc.kind.resize(k); sc.flags.resize(k); sc.nsid.resize(k);
     std::vector<std::vector<Requirement>> ns_reqs_of_term;
     auto push_reqs = [&](const std::vector<Requirement>& reqs) {
       for (auto& r : reqs) {
         const uint32_t kid = labels.key_id(r.key);  // (all of it interned by sync_vocabulary already)
-        req_key.push_back(kid);
-        req_op.push_back(r.op);
-        for (auto& v : r.values) req_vals.push_back(labels.value_id(kid, v));
-        req_val_off.push_back((int32_t)req_vals.size());
+        sc.req_key.push_back(kid);
+        sc.req_op.push_back(r.op);
+        for (auto& v : r.values) sc.req_vals.push_back(labels.value_id(kid, v));
+        sc.req_val_off.push_back((int32_t)sc.req_vals.size());
       }
     };
-    for (size_t t = 0; t < m; ++t) {
-      const ThrottleObj& o = throttles[t];
-      kind[t] = (uint8_t)o.kind;
-      nsid[t] = o.kind == KT_KIND_THROTTLE ? ns_id(o.ns) : -1;
-      flags[t] = 0;
-      if (o.live && o.throttler_name == name) flags[t] |= KT_THR_RESPONSIBLE;  // isResponsibleFor, throttle_controller.go:213-215
+    for (size_t i = 0; i < k; ++i) {
+      const ThrottleObj& o = throttles[list[i]];
+      sc.kind[i] = (uint8_t)o.kind;
+      sc.nsid[i] = o.kind == KT_KIND_THROTTLE ? ns_id(o.ns) : -1;
+      sc.flags[i] = 0;
+      if (o.live && o.throttler_name == name) sc.flags[i] |= KT_THR_RESPONSIBLE;  // isResponsibleFor, throttle_controller.go:213-215
       for (auto& term : o.terms) {
         // a podSelector that does not convert: the term matches nobody and shadows the LATER terms for exactly the pods that
         // reach it (KT_TERM_POD_INVALID; the table compiler scopes that by namespace / namespaceSelector)
-        term_flags.push_back((term.ns_sel.error.empty() ? 0 : KT_TERM_NS_INVALID) |  // Q9: swallowed, the term is false
-                             (term.pod_sel.error.empty() ? 0 : KT_TERM_POD_INVALID));
+        sc.term_flags.push_back((term.ns_sel.error.empty() ? 0 : KT_TERM_NS_INVALID) |  // Q9: swallowed, the term is false
+                                (term.pod_sel.error.empty() ? 0 : KT_TERM_POD_INVALID));
         push_reqs(term.pod_sel.reqs);  // (none when the selector is broken)
-        pod_req_off.push_back((int32_t)req_key.size());
+        sc.pod_req_off.push_back((int32_t)sc.req_key.size());
         std::vector<Requirement> nsr;
         if (o.kind == KT_KIND_CLUSTERTHROTTLE && term.ns_sel.error.empty()) {
           nsr = term.ns_sel.reqs;
@@ -1064,26 +1096,27 @@ struct kth_plugin {
         }
         ns_reqs_of_term.push_back(std::move(nsr));
       }
-      term_off[t + 1] = (int32_t)term_flags.size();
+      sc.term_off.push_back((int32_t)sc.term_flags.size());
     }
-    // requirement pool layout: all podSelector requirements (term order), then all namespaceSelector ones
-    ns_req_off.push_back((int32_t)req_key.size());
+    sc.ns_req_off.push_back((int32_t)sc.req_key.size());
     for (auto& reqs : ns_reqs_of_term) {
       push_reqs(reqs);
-      ns_req_off.push_back((int32_t)req_key.size());
+      sc.ns_req_off.push_back((int32_t)sc.req_key.size());
     }
-    const ThresholdColumns tcols = threshold_columns(AllColumns{m});
-    kt_throttle_cols tc = tcols.cols();
-    tc.kind = kind.data(); tc.ns_id = nsid.data(); tc.flags = flags.data();
-    kt_selector_table st{};
-    st.n_terms = (int32_t)term_flags.size(); st.n_reqs = (int32_t)req_key.size(); st.n_vals = (int32_t)req_vals.size();
-    st.term_off = term_off.data(); st.term_flags = term_flags.data(); st.pod_req_off = pod_req_off.data(); st.ns_req_off = ns_req_off.data();
-    st.req_key = req_key.data(); st.req_op = req_op.data(); st.req_val_off = req_val_off.data(); st.req_vals = req_vals.data();
-    sync_namespaces();  // Throttle rows may have introduced namespace ids
-    check(kt_upload_throttles(ctx, (int32_t)m, &tc, &st), "kt_upload_throttles");
-    throttles_dirty = false;
-    status_dirty = reserved_dirty = true;  // kt_upload_throttles forgets both
-    spec_cols.clear();
+    return sc;
+  }
+  // Deletions and in-place selector / throttlerName edits (delete_throttle, apply_throttle): one kt_update_selector_rows for the
+  // listed columns, with the column layout kept.  The engine patches its tables when the new terms fit them and compiles them
+  // again otherwise; either way the statuses and reservations it holds stay.
+  void sync_selectors() {
+    if (sel_cols.list.empty()) return;
+    const SelectorColumns scols = selector_columns(sel_cols.list);
+    kt_throttle_cols tc{};
+    scols.put(&tc);
+    const kt_selector_table st = scols.table();
+    const std::vector<int32_t> idx(sel_cols.list.begin(), sel_cols.list.end());
+    check(kt_update_selector_rows(ctx, (int64_t)idx.size(), idx.data(), &tc, &st, nullptr), "kt_update_selector_rows");
+    sel_cols.clear();
   }
   // The spec columns of the listed throttles that no compiled table reads: spec.threshold ([R][k] / [k]) and the
   // temporaryThresholdOverrides in spec order (ovr_off[k+1], ovr_thr[R][n_ovr]).  kind, ns_id and flags stay null.
@@ -1299,7 +1332,8 @@ struct kth_plugin {
     sync_pods();
     sync_namespaces();
     sync_throttles();
-    sync_thresholds();  // (after sync_throttles, which sends these columns too when it uploads the throttles)
+    sync_selectors();   // (after sync_throttles, which sends these columns too when it uploads the throttles)
+    sync_thresholds();
   }
   // Everything a PreFilter view reads: the tables, the informer copy of the statuses and the reservations.  A table change voids
   // the cached queue verdicts on the way (sync_namespaces / sync_throttles); afterwards no dirty flag is set.
@@ -2946,8 +2980,16 @@ struct kth_plugin {
       const size_t t = (size_t)it->second;
       const bool tables_kept = epoch == col_epoch && same_tables(old, o), thresholds_kept = same_threshold_columns(old, o),
                  status_kept = same_status(old, o);
+      // Other terms or another throttlerName in the same column (same kind and namespace, no label key or value the dictionaries
+      // lack): the column is recompiled in place, without a new layout (kt_update_selector_rows).
+      const bool selector_in_place = !tables_kept && epoch == col_epoch && old.ns == o.ns && selector_delta() && in_vocabulary(o) &&
+                                     (thresholds_kept || kt_update_threshold_rows);
       old = std::move(o);
-      if (tables_kept && (thresholds_kept || (kt_update_threshold_rows && !throttles_dirty))) {
+      if (selector_in_place) {
+        sel_cols.add(t);
+        selector_changed(t, true);
+      }
+      if (selector_in_place || (tables_kept && (thresholds_kept || (kt_update_threshold_rows && !throttles_dirty)))) {
         if (!thresholds_kept) {
           spec_cols.add(t);
           throttle_state_changed(t);
@@ -2966,7 +3008,8 @@ struct kth_plugin {
     auto it = thr_index.find(thr_key(kind, ns, tname));
     if (it == thr_index.end()) return;
     // the column can never match or be reconciled again; the next new throttle takes it over
-    ThrottleObj& o = throttles[(size_t)it->second];
+    const size_t t = (size_t)it->second;
+    ThrottleObj& o = throttles[t];
     free_thr.push_back(it->second);
     if (o.metrics_pending) { record_metrics(o); o.metrics_pending = false; }  // its series outlive it, as a GaugeVec's do
     o.live = false;
@@ -2974,8 +3017,55 @@ struct kth_plugin {
     // The reservation cache keeps the entry: reserved_resource_amounts.go has no way to drop a throttle, so what was reserved on
     // this name is still counted if a throttle of the same name comes back (until those pods are observed or deleted).
     thr_index.erase(it);
+    // The column becomes a hole that matches nothing (no terms, flags 0) until the next whole upload compacts it -- as long as at
+    // most half the columns are holes.  That bound is a guess, not a measured break-even: past it every pass walks mostly dead
+    // words, and a whole upload lays the columns out again.
+    if (selector_delta() && 2 * free_thr.size() <= throttles.size()) {
+      sel_cols.add(t);
+      selector_changed(t, false);
+      return;
+    }
     throttles_dirty = status_dirty = reserved_dirty = true;
     broken_valid = false;
+  }
+  // Whether a deletion or a selector edit can go as a column delta: the engine has the call and no whole upload is pending.
+  bool selector_delta() const { return kt_update_selector_rows && !throttles_dirty; }
+  // Every label key and value the throttle's selectors mention is in the dictionaries already: sync_vocabulary would intern
+  // nothing, so no pod or namespace row has to be packed again.
+  bool in_vocabulary(const ThrottleObj& o) const {
+    auto known = [&](const std::vector<Requirement>& reqs) {
+      for (auto& r : reqs) {
+        const int kid = labels.keys.find(r.key);
+        if (kid < 0) return false;
+        for (auto& v : r.values)
+          if (labels.vals[(size_t)kid].find(v) < 0) return false;
+      }
+      return true;
+    };
+    for (auto& term : o.terms) {
+      if (!known(term.pod_sel.reqs)) return false;
+      if (o.kind == KT_KIND_CLUSTERTHROTTLE && (!known(term.ns_sel.reqs) || labels.keys.find(kNsExistsKey) < 0)) return false;
+    }
+    return true;
+  }
+  // Column t's terms or flags changed in place: the cached verdicts of the pods it affected are void (the cached match rows say
+  // which), and after an edit also those of the queued pods in the namespaces the new version can reach.
+  void selector_changed(size_t t, bool edit) {
+    throttle_state_changed(t);
+    broken_valid = false;
+    if (!edit || !queue.valid) return;
+    const ThrottleObj& o = throttles[t];
+    const std::string reach = o.kind == KT_KIND_THROTTLE ? std::string() : namespace_set_of(o);
+    for (size_t row = 0; row < pend_pod.size() && row < queue.row_ok.size(); ++row) {
+      if (pend_pod[row] < 0) continue;
+      const std::string& ns = pods[(size_t)pend_pod[row]].ns;
+      bool reached = ns == o.ns;
+      if (o.kind != KT_KIND_THROTTLE) {
+        const int id = ns_dict.find(ns);
+        reached = id >= 0 && (size_t)id < reach.size() && reach[(size_t)id] == '1';
+      }
+      if (reached) queue.row_ok[row] = 0;
+    }
   }
 
   std::string status_json(const std::string& ns, const std::string& tname) {

@@ -1,4 +1,5 @@
-// kt_nsrows.cuh -- namespace row deltas on the device (kt_update_namespace_rows).
+// kt_nsrows.cuh -- namespace row deltas on the device (kt_update_namespace_rows), and the namespace side of selector column
+// deltas (kt_update_selector_rows).
 //
 // A namespace's labels feed two things of the compiled tables: its own nsmask row ([W][TPpad], which throttle terms can apply to
 // its pods) and its entry in the per-namespace word lists (nsw_off / nsw_idx).  The pod-label tables (table, need, keydir, valrow,
@@ -12,6 +13,9 @@
 //   3. k_ns_scan     one CTA: the counts -> nsw_off, plus the total and the longest list (brought back to the host)
 //   4. k_ns_fill     one warp per namespace: the non-zero words in ascending order into nsw_idx
 //   5. k_ns_winfo    one lane per resident pod row: the words inlined with the row (winfo_pack), from the new lists
+// A selector column delta changes the other axis: k_ns_cols re-evaluates the listed 32-throttle words for every namespace with
+// the same per-lane walk as k_ns_rows (ns_word_planes), then steps 2-5 follow.  k_scatter_words / k_scatter_kind_flags land the
+// host-recompiled table and need slices of those words and the listed columns' kind and flags.
 #pragma once
 #include "kt_keyed.cuh"
 
@@ -65,14 +69,12 @@ __device__ __forceinline__ bool ns_term_holds(const NsSpecView& sp, int term, ui
   return true;
 }
 
-// nsmask rows of the kd listed namespaces ns_ids[i], labels [LN][kd]; n_ns: the namespace count (a ClusterThrottle term applies to
-// namespaces below it only).  grid (ceil(W / 8), up to 65535 rows from y0), 256 threads: warp = word.
-__global__ void __launch_bounds__(256) k_ns_rows(const NsSpecView sp, int32_t y0, int32_t kd, const int32_t* __restrict__ ns_ids,
-                                                 const int64_t* __restrict__ labels, int LN, int32_t n_ns, uint32_t* __restrict__ nsmask) {
-  const int w = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
-  if (w >= sp.W) return;  // whole warps
-  const int i = y0 + blockIdx.y;
-  const int ns = __ldg(&ns_ids[i]);
+// One warp's nsmask entry of namespace ns and 32-throttle word w, one lane per throttle: its terms in order, as compile_tables
+// builds them -- a ClusterThrottle term's namespaceSelector over the namespace's labels (slot s at labels[col + s * stride]; read
+// for ns < n_ns only), a Throttle term's namespace equality, a KT_TERM_POD_INVALID term switching the later terms off where it
+// applies -- one ballot per term plane, written by lane 0 to the namespace's entry of that word in nsmask ([NS][W][TPpad]).
+__device__ __forceinline__ void ns_word_planes(const NsSpecView& sp, int w, int lane, int ns, const int64_t* labels, int col, int64_t stride,
+                                               int LN, int32_t n_ns, uint32_t* nsmask) {
   const int t = w * 32 + lane;
   int term0 = 0, nterm = 0;
   bool cluster = false, own = false;
@@ -93,7 +95,7 @@ __global__ void __launch_bounds__(256) k_ns_rows(const NsSpecView sp, int32_t y0
       const int term = term0 + s;
       const uint8_t tf = __ldg(&sp.term_flags[term]);
       if ((tf & KT_TERM_POD_INVALID) || !(tf & kTermUnsat)) {
-        const bool applies = cluster ? ns < n_ns && ns_term_holds(sp, term, tf, labels + i, kd, LN) : own;
+        const bool applies = cluster ? ns < n_ns && ns_term_holds(sp, term, tf, labels + col, stride, LN) : own;
         if (tf & KT_TERM_POD_INVALID) blocked |= applies;
         else bit = applies && !blocked;
       }
@@ -101,6 +103,46 @@ __global__ void __launch_bounds__(256) k_ns_rows(const NsSpecView sp, int32_t y0
     const uint32_t word = __ballot_sync(kFull, bit);
     if (lane == 0) row[s] = word;
   }
+}
+
+// nsmask rows of the kd listed namespaces ns_ids[i], labels [LN][kd]; n_ns: the namespace count (a ClusterThrottle term applies to
+// namespaces below it only).  grid (ceil(W / 8), up to 65535 rows from y0), 256 threads: warp = word.
+__global__ void __launch_bounds__(256) k_ns_rows(const NsSpecView sp, int32_t y0, int32_t kd, const int32_t* __restrict__ ns_ids,
+                                                 const int64_t* __restrict__ labels, int LN, int32_t n_ns, uint32_t* __restrict__ nsmask) {
+  const int w = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (w >= sp.W) return;  // whole warps
+  const int i = y0 + blockIdx.y;
+  const int ns = __ldg(&ns_ids[i]);
+  ns_word_planes(sp, w, lane, ns, labels, i, kd, LN, n_ns, nsmask);
+}
+
+// nsmask entries of the nw listed words (words[]) for all NS namespaces, labels [LN][n_ns] (kt_update_selector_rows: the columns
+// of those words changed).  One warp per (namespace, listed word): warp g takes namespace g % NS of word g / NS, so the warps of
+// a CTA share one word's spec.  grid ceil(NS * nw / 8), 256 threads.
+__global__ void __launch_bounds__(256) k_ns_cols(const NsSpecView sp, int32_t NS, int32_t nw, const int32_t* __restrict__ words,
+                                                 const int64_t* __restrict__ labels, int LN, int32_t n_ns, uint32_t* __restrict__ nsmask) {
+  const int64_t g = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5);
+  if (g >= (int64_t)NS * nw) return;  // whole warps
+  const int lane = threadIdx.x & 31, ns = (int)(g % NS), w = __ldg(&words[g / NS]);
+  ns_word_planes(sp, w, lane, ns, labels, ns, n_ns, LN, n_ns, nsmask);
+}
+
+// Word slices of the listed words: dst[words[j] * len + e] = src[j * len + e] (table / need slices of kt_update_selector_rows)
+__global__ void __launch_bounds__(256) k_scatter_words(int64_t nw, const int32_t* __restrict__ words, int64_t len, const uint32_t* __restrict__ src,
+                                                       uint32_t* __restrict__ dst) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < nw * len; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t j = i / len, e = i - j * len;
+    dst[(int64_t)__ldg(&words[j]) * len + e] = src[i];
+  }
+}
+
+// kind and flags of the k listed throttle columns (kt_update_selector_rows)
+__global__ void __launch_bounds__(128) k_scatter_kind_flags(int64_t k, const int32_t* __restrict__ idx, const uint8_t* __restrict__ src_kind,
+                                                            const uint8_t* __restrict__ src_flags, uint8_t* kind, uint8_t* flags) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= k) return;
+  kind[idx[i]] = src_kind[i];
+  flags[idx[i]] = src_flags[i];
 }
 
 __device__ __forceinline__ bool ns_word_live(const uint32_t* __restrict__ nsmask, int ns, int w, int W, int TPpad) {

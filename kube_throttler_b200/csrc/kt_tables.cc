@@ -69,12 +69,6 @@ std::string copy_selector_spec(int32_t m, const kt_throttle_cols* cols, const kt
 
 namespace {
 
-struct RowRef {
-  int32_t row;
-  bool other;    // the "some other value" row of the key
-  uint32_t val;  // valid when !other
-};
-
 // Does requirement q hold for a label whose key equals the requirement's key and whose value is `val`
 // (or some value no requirement mentions when other==true)?
 inline bool req_holds_present(const SelectorSpec& s, int32_t q, bool other, uint32_t val) {
@@ -110,7 +104,45 @@ inline bool ns_term_matches(const SelectorSpec& s, int32_t term, const int64_t* 
   return true;
 }
 
+// need counts of one column's terms -> its bit in the word's counter planes ([TPpad][B] of the word)
+void put_need(int32_t t, int32_t n_terms, const int32_t* need, int32_t TPp, int32_t B, uint32_t* word_need) {
+  for (int32_t sidx = 0; sidx < n_terms; ++sidx)
+    for (int32_t b = 0; b < B; ++b)
+      if ((need[sidx] >> b) & 1) word_need[(size_t)sidx * B + b] |= 1u << (t & 31);
+}
+
 }  // namespace
+
+// Throttle t's bits in its word's slice of the table ([rows][TPpad][2], which the caller set to sat = 1 / pos = 0 for t), the
+// need count of each of its terms (need[sidx]) and which of them can never match (term_unsat[sidx]); returns the largest need.
+int32_t compile_column(const kt_limits& lim, const SelectorSpec& s, int32_t t, const RowsOfKey& rows_of_key, int32_t rows, int32_t TPp,
+                       uint32_t* word_table, int32_t* need, uint8_t* term_unsat) {
+  const uint32_t bit = 1u << (t & 31);
+  int32_t max_need = 0;
+  for (int32_t term = s.term_off[t], sidx = 0; term < s.term_off[t + 1]; ++term, ++sidx) {
+    // group this term's requirements by key
+    std::map<uint32_t, std::vector<int32_t>> by_key;
+    for (int32_t q = s.pod_req_off[term]; q < s.pod_req_off[term + 1]; ++q) by_key[s.req_key[q]].push_back(q);
+    int32_t nd = 0;
+    for (auto& kv : by_key) {
+      bool positive = false;
+      for (int32_t q : kv.second) positive |= (s.req_op[q] == KT_OP_IN || s.req_op[q] == KT_OP_EXISTS);
+      if (positive) ++nd;
+      for (const RowRef& rr : rows_of_key.at(kv.first)) {
+        bool sat = true;
+        for (int32_t q : kv.second) sat &= req_holds_present(s, q, rr.other, rr.val);
+        size_t e = ((size_t)rr.row * TPp + sidx) * 2;
+        if (!sat) word_table[e] &= ~bit;
+        if (positive) word_table[e + 1] |= bit;
+      }
+    }
+    term_unsat[sidx] = 0;
+    if (nd > lim.label_slots) { term_unsat[sidx] = 1; nd = 0; }  // needs more keys than a pod row can hold
+    need[sidx] = nd;
+    max_need = std::max(max_need, nd);
+  }
+  return max_need;
+}
 
 std::string compile_tables(const kt_limits& lim, const SelectorSpec& s, int32_t n_ns, const int64_t* ns_labels, HostTables* out) {
   HostTables h;
@@ -126,8 +158,8 @@ std::string compile_tables(const kt_limits& lim, const SelectorSpec& s, int32_t 
 
   // ---- row dictionary over the podSelector requirements --------------------------------------
   std::map<uint32_t, int32_t> key_row;                 // key -> "other value" row
-  std::map<uint64_t, int32_t> pair_row;                // (key<<32|val) -> row
-  std::unordered_map<uint32_t, std::vector<RowRef>> rows_of_key;
+  std::map<uint64_t, int32_t>& pair_row = h.pair_row;  // (key<<32|val) -> row
+  RowsOfKey& rows_of_key = h.rows_of_key;
   int32_t next_row = 0;
   const int32_t n_terms = s.term_off.empty() ? 0 : s.term_off[M];
   for (int32_t term = 0; term < n_terms; ++term)
@@ -157,42 +189,15 @@ std::string compile_tables(const kt_limits& lim, const SelectorSpec& s, int32_t 
   std::vector<int32_t> need((size_t)M * TP, 0);
   h.term_unsat.assign((size_t)n_terms, 0);
   int32_t max_need = 0;
-  for (int32_t t = 0; t < M; ++t) {
-    const int32_t w = t >> 5;
-    const uint32_t bit = 1u << (t & 31);
-    for (int32_t term = s.term_off[t], sidx = 0; term < s.term_off[t + 1]; ++term, ++sidx) {
-      // group this term's requirements by key
-      std::map<uint32_t, std::vector<int32_t>> by_key;
-      for (int32_t q = s.pod_req_off[term]; q < s.pod_req_off[term + 1]; ++q) by_key[s.req_key[q]].push_back(q);
-      int32_t nd = 0;
-      for (auto& kv : by_key) {
-        bool positive = false;
-        for (int32_t q : kv.second) positive |= (s.req_op[q] == KT_OP_IN || s.req_op[q] == KT_OP_EXISTS);
-        if (positive) ++nd;
-        for (const RowRef& rr : rows_of_key[kv.first]) {
-          bool sat = true;
-          for (int32_t q : kv.second) sat &= req_holds_present(s, q, rr.other, rr.val);
-          size_t e = (((size_t)w * rows + rr.row) * TPp + sidx) * 2;
-          if (!sat) h.table[e] &= ~bit;
-          if (positive) h.table[e + 1] |= bit;
-        }
-      }
-      if (nd > lim.label_slots) { h.term_unsat[(size_t)term] = 1; nd = 0; }  // needs more keys than a pod row can hold
-      need[(size_t)t * TP + sidx] = nd;
-      max_need = std::max(max_need, nd);
-    }
-  }
+  for (int32_t t = 0; t < M; ++t)
+    max_need = std::max(max_need, compile_column(lim, s, t, h.rows_of_key, rows, TPp, &h.table[(size_t)(t >> 5) * rows * TPp * 2],
+                                                 &need[(size_t)t * TP], h.term_unsat.data() + s.term_off[t]));
   int32_t B = 1;
   while ((1 << B) <= max_need) ++B;
   B = B <= 2 ? 2 : 6;  // the kernels are instantiated for 2 and 6 counter bit-planes (need <= 3 / <= 63)
   h.B = B;
   h.need.assign((size_t)h.W * TPp * B, 0);
-  for (int32_t t = 0; t < M; ++t)
-    for (int32_t sidx = 0; sidx < s.term_off[t + 1] - s.term_off[t]; ++sidx) {
-      int32_t nd = need[(size_t)t * TP + sidx];
-      for (int32_t b = 0; b < B; ++b)
-        if ((nd >> b) & 1) h.need[((size_t)(t >> 5) * TPp + sidx) * B + b] |= 1u << (t & 31);
-    }
+  for (int32_t t = 0; t < M; ++t) put_need(t, s.term_off[t + 1] - s.term_off[t], &need[(size_t)t * TP], TPp, B, &h.need[(size_t)(t >> 5) * TPp * B]);
 
   // ---- namespace masks: which (throttle, term) can apply to pods of namespace ns at all ---------
   int32_t NS = n_ns;
@@ -297,6 +302,45 @@ std::string compile_tables(const kt_limits& lim, const SelectorSpec& s, int32_t 
 
   *out = std::move(h);
   return "";
+}
+
+bool patch_columns(const kt_limits& lim, const SelectorSpec& old_s, const SelectorSpec& s, const std::vector<int32_t>& listed, HostTables* h) {
+  const int32_t M = s.m, TPp = h->TPpad, B = h->B, rows = h->rows;
+  std::vector<char> is_listed((size_t)M, 0);
+  for (int32_t t : listed) {  // does every listed column fit the resident tables?
+    is_listed[(size_t)t] = 1;
+    if (s.term_off[t + 1] - s.term_off[t] > TPp) return false;
+    if (s.kind[t] == KT_KIND_THROTTLE && s.ns_id[t] >= h->NS) return false;
+    for (int32_t term = s.term_off[t]; term < s.term_off[t + 1]; ++term)
+      for (int32_t q = s.pod_req_off[term]; q < s.pod_req_off[term + 1]; ++q) {
+        if (!h->rows_of_key.count(s.req_key[q])) return false;
+        for (int32_t i = s.req_val_off[q]; i < s.req_val_off[q + 1]; ++i)
+          if (!h->pair_row.count(((uint64_t)s.req_key[q] << 32) | s.req_vals[i])) return false;
+      }
+  }
+  // term_unsat follows the new term numbering: the unlisted columns keep theirs
+  std::vector<uint8_t> unsat((size_t)s.term_off[M], 0);
+  for (int32_t t = 0; t < M; ++t)
+    if (!is_listed[(size_t)t])
+      std::copy(h->term_unsat.begin() + old_s.term_off[t], h->term_unsat.begin() + old_s.term_off[t + 1], unsat.begin() + s.term_off[t]);
+  std::vector<int32_t> need((size_t)TPp);
+  for (int32_t t : listed) {
+    const uint32_t bit = 1u << (t & 31);
+    uint32_t* word_table = &h->table[(size_t)(t >> 5) * rows * TPp * 2];
+    uint32_t* word_need = &h->need[(size_t)(t >> 5) * TPp * B];
+    for (size_t e = 0; e < (size_t)rows * TPp * 2; e += 2) {  // as compile_tables starts: sat = 1, pos = 0
+      word_table[e] |= bit;
+      word_table[e + 1] &= ~bit;
+    }
+    for (size_t e = 0; e < (size_t)TPp * B; ++e) word_need[e] &= ~bit;
+    const int32_t nt = s.term_off[t + 1] - s.term_off[t];
+    if (compile_column(lim, s, t, h->rows_of_key, rows, TPp, word_table, need.data(), unsat.data() + s.term_off[t]) >= (1 << B)) return false;
+    put_need(t, nt, need.data(), TPp, B, word_need);
+  }
+  h->term_unsat.swap(unsat);
+  h->TP = 1;
+  for (int32_t t = 0; t < M; ++t) h->TP = std::max(h->TP, s.term_off[t + 1] - s.term_off[t]);
+  return true;
 }
 
 }  // namespace kt

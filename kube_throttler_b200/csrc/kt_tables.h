@@ -8,7 +8,9 @@
 // It contains no pod-evaluation code: matching pods happens only on the GPU.
 #pragma once
 #include <cstdint>
+#include <map>
 #include <string>
+#include <unordered_map>
 #include <vector>
 
 #include "../../include/kt_b200.h"
@@ -24,6 +26,14 @@ struct SelectorSpec {
   std::vector<uint8_t> term_flags, req_op;
   std::vector<uint32_t> req_key, req_vals;
 };
+
+// A table row of a key that some podSelector requirement mentions
+struct RowRef {
+  int32_t row;
+  bool other;    // the "some other value" row of the key
+  uint32_t val;  // valid when !other
+};
+using RowsOfKey = std::unordered_map<uint32_t, std::vector<RowRef>>;
 
 struct HostTables {
   int32_t M = 0;
@@ -53,6 +63,9 @@ struct HostTables {
   std::vector<int32_t> nsw_off;  // [NS+1]
   std::vector<int32_t> nsw_idx;  // non-zero words per namespace
   int32_t max_ns_words = 0;      // longest per-namespace word list
+  // the row dictionary the table was built with: every row of each mentioned key, and the row of each mentioned (key, value)
+  RowsOfKey rows_of_key;
+  std::map<uint64_t, int32_t> pair_row;  // (key << 32 | value) -> row
 };
 
 // Validates the CSR arrays and copies them.  Returns "" or an error description.
@@ -61,6 +74,18 @@ std::string copy_selector_spec(int32_t m, const kt_throttle_cols* cols, const kt
 // Builds the tables.  ns_labels: [LN][n_ns] (may be null when n_ns == 0).
 std::string compile_tables(const kt_limits& lim, const SelectorSpec& spec, int32_t n_ns, const int64_t* ns_labels,
                            HostTables* out);
+
+// One column's table bits, term need counts and unsatisfiable terms (see kt_tables.cc); compile_tables builds every column with it.
+int32_t compile_column(const kt_limits& lim, const SelectorSpec& spec, int32_t t, const RowsOfKey& rows_of_key, int32_t rows,
+                       int32_t TPpad, uint32_t* word_table, int32_t* need, uint8_t* term_unsat);
+
+// The listed columns of h (compiled from old_spec) recompiled in place from `spec`, which equals old_spec but for the listed
+// columns: their table bits, need planes and term_unsat entries, with compile_column.  false when one of them does not fit the
+// resident tables -- a podSelector key or (key, value) without a row, more terms than TPpad, a need beyond the B counter planes,
+// a Throttle namespace beyond NS --; h is then partly patched and must be compiled again.  The namespace masks and word lists
+// are not touched (nsmask, nsw_off, nsw_idx, max_ns_words).
+bool patch_columns(const kt_limits& lim, const SelectorSpec& old_spec, const SelectorSpec& spec, const std::vector<int32_t>& listed,
+                   HostTables* h);
 
 constexpr uint32_t kKeyDirMax = 1u << 16;  // direct key table only for key ids below this
 
