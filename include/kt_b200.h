@@ -351,6 +351,23 @@ int kt_update_threshold_rows(kt_ctx* ctx, int64_t k, const int32_t* idx, const k
  * return.  Multi-GPU: the call is local, not collective -- every rank must apply the same updates. */
 int kt_update_selector_rows(kt_ctx* ctx, int64_t k, const int32_t* idx, const kt_throttle_cols* cols,
                             const kt_selector_table* sel, int32_t* recompiled);
+/* k new throttle columns appended at [M, M+k): a Throttle or ClusterThrottle creation without recompiling the selector tables.
+ * cols and sel are shaped exactly as for kt_upload_throttles(ctx, k, cols, sel): kind, ns_id, flags, thresholds, the override
+ * CSR and the selector CSR of the k new columns.  Afterwards every call answers exactly as after a kt_upload_throttles of the
+ * previous spec with these k columns appended, followed by re-uploading the status and the reservations held before the call,
+ * each widened by k columns of zeros (no calculatedAt, nothing used, nothing reserved); status or reservations not held before
+ * the call are still not held.  The state flags move as kt_update_selector_rows moves them; *recompiled (may be NULL) is as
+ * there.
+ * KT_ERR_INVALID: k < 0; a null column with k > 0; a malformed CSR or ovr_off.  KT_ERR_STATE before kt_upload_throttles;
+ * k = 0 is a no-op.
+ * In place when every new column fits the resident tables (the test of kt_update_selector_rows): the new columns are compiled on
+ * the host into the partly filled last 32-throttle word and the words appended after it, and only those word slices cross, in
+ * one staged copy; the resident per-throttle columns are widened on the device (the override columns rebuilt), the namespace
+ * masks restrided when the word count grows and evaluated for the touched words, the word lists rebuilt; the pod rows keep their
+ * table offsets.  Otherwise the tables are compiled again from the grown spec.  One synchronisation; the caller may reuse its
+ * buffers on return.  Multi-GPU: the call is local, not collective -- every rank must apply the same appends. */
+int kt_append_throttle_rows(kt_ctx* ctx, int64_t k, const kt_throttle_cols* cols, const kt_selector_table* sel,
+                            int32_t* recompiled);
 
 /* ---- the pass ------------------------------------------------------------------- */
 /* One batched pass: reconcile every throttle (throttle_controller.go:84-133) and check

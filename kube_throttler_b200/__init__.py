@@ -43,7 +43,7 @@ def build(force: bool = False) -> str:
 EXPORTS = [
     "kt_create", "kt_destroy", "kt_last_error", "kt_version", "kt_set_stream", "kt_sync", "kt_enable_timing",
     "kt_enable_trace", "kt_get_trace", "kt_host_alloc", "kt_host_alloc_upload", "kt_host_free", "kt_upload_pods", "kt_upload_pods_compact", "kt_upload_pods_packed", "kt_set_async_uploads", "kt_update_pod_rows", "kt_upload_namespaces", "kt_update_namespace_rows",
-    "kt_upload_throttles", "kt_upload_status", "kt_set_reserved", "kt_update_status_rows", "kt_update_reserved_rows", "kt_update_threshold_rows", "kt_update_selector_rows", "kt_evaluate", "kt_get_reconcile",
+    "kt_upload_throttles", "kt_upload_status", "kt_set_reserved", "kt_update_status_rows", "kt_update_reserved_rows", "kt_update_threshold_rows", "kt_update_selector_rows", "kt_append_throttle_rows", "kt_evaluate", "kt_get_reconcile",
     "kt_match_words", "kt_get_match_bitmap", "kt_get_match_rows", "kt_get_match_columns", "kt_get_check_summary", "kt_reconcile_throttles", "kt_get_check", "kt_set_sparse_check", "kt_get_check_sparse", "kt_get_check_rows", "kt_check_pending_rows", "kt_match_pods", "kt_check_pods", "kt_get_changed", "kt_get_reconcile_rows", "kt_step_submit", "kt_step_wait", "kt_admit_queue", "kt_get_timing", "kt_comm_unique_id",
     "kt_comm_init", "kt_comm_destroy", "kt_debug_compile_tables", "kt_debug_set_pass_plan", "kt_debug_get_pass_plan", "kt_debug_get_ns_tables",
     "kt_debug_set_row_order", "kt_debug_get_row_order",
@@ -102,6 +102,7 @@ def lib():
         L.kt_update_reserved_rows.argtypes = [vp, C.c_int64, vp, vp, vp, vp]
         L.kt_update_threshold_rows.argtypes = [vp, C.c_int64, vp, C.POINTER(abi.ThrottleCols)]
         L.kt_update_selector_rows.argtypes = [vp, C.c_int64, vp, C.POINTER(abi.ThrottleCols), C.POINTER(abi.SelectorTable), vp]
+        L.kt_append_throttle_rows.argtypes = [vp, C.c_int64, C.POINTER(abi.ThrottleCols), C.POINTER(abi.SelectorTable), vp]
         L.kt_evaluate.argtypes = [vp, C.c_int64, C.c_uint32]
         L.kt_get_reconcile.argtypes = [vp, C.POINTER(abi.ReconcileOut)]
         L.kt_match_words.argtypes = [vp]
@@ -337,6 +338,33 @@ class Engine:
                                *(abi.ptr(a[f]) for f in ("term_off", "term_flags", "pod_req_off", "ns_req_off", "req_key", "req_op", "req_val_off", "req_vals")))
         out = np.zeros(1, np.int32)
         self._ck(self._L.kt_update_selector_rows(self._h, k, abi.ptr(idx), C.byref(tc), C.byref(st), abi.ptr(out)))
+        return bool(out[0])
+
+    def append_throttle_rows(self, cols: dict) -> bool:
+        """kt_append_throttle_rows: k new throttle columns appended at [m, m+k), their status and reservations zero.  `cols` holds
+        the k new columns named and shaped like the Snapshot fields: kind, thr_ns, thr_flags, thr[R][k], thr_present, thr_cnt,
+        ovr_off[k+1] and the override columns, and the selector CSR (term_off[k+1], term_flags, pod_req_off, ns_req_off, req_key,
+        req_op, req_val_off, req_vals).  Returns whether the engine compiled the tables again (a column did not fit them)."""
+        k, R = int(np.asarray(cols["kind"]).shape[0]), self.R
+        off = abi._arr(cols["ovr_off"], np.int32)
+        n = int(off[-1]) if off.shape[0] else 0
+        a = dict(kind=abi._arr(cols["kind"], np.uint8), ns=abi._arr(cols["thr_ns"], np.int32), flags=abi._arr(cols["thr_flags"], np.uint8),
+                 thr=abi._arr(cols["thr"], np.int64, (R, k)), thr_present=abi._arr(cols["thr_present"], np.uint32),
+                 thr_cnt=abi._arr(cols["thr_cnt"], np.int64), ovr_off=off, ovr_begin=abi._arr(cols["ovr_begin"], np.int64),
+                 ovr_end=abi._arr(cols["ovr_end"], np.int64), ovr_flags=abi._arr(cols["ovr_flags"], np.uint8),
+                 ovr_thr=abi._arr(cols["ovr_thr"], np.int64, (R, n)), ovr_present=abi._arr(cols["ovr_present"], np.uint32),
+                 ovr_cnt=abi._arr(cols["ovr_cnt"], np.int64),
+                 term_off=abi._arr(cols["term_off"], np.int32), term_flags=abi._arr(cols["term_flags"], np.uint8),
+                 pod_req_off=abi._arr(cols["pod_req_off"], np.int32), ns_req_off=abi._arr(cols["ns_req_off"], np.int32),
+                 req_key=abi._arr(cols["req_key"], np.uint32), req_op=abi._arr(cols["req_op"], np.uint8),
+                 req_val_off=abi._arr(cols["req_val_off"], np.int32), req_vals=abi._arr(cols["req_vals"], np.uint32))
+        tc = abi.ThrottleCols(*(abi.ptr(a[f]) for f in ("kind", "ns", "flags", "thr", "thr_present", "thr_cnt", "ovr_off")), n,
+                              *(abi.ptr(a[f]) for f in ("ovr_begin", "ovr_end", "ovr_flags", "ovr_thr", "ovr_present", "ovr_cnt")))
+        st = abi.SelectorTable(int(a["term_off"][-1]) if a["term_off"].shape[0] else 0, int(a["req_key"].shape[0]), int(a["req_vals"].shape[0]),
+                               *(abi.ptr(a[f]) for f in ("term_off", "term_flags", "pod_req_off", "ns_req_off", "req_key", "req_op", "req_val_off", "req_vals")))
+        out = np.zeros(1, np.int32)
+        self._ck(self._L.kt_append_throttle_rows(self._h, k, C.byref(tc), C.byref(st), abi.ptr(out)))
+        self.m += k
         return bool(out[0])
 
     def update_reserved_rows(self, idx: np.ndarray, reserved: np.ndarray, present: np.ndarray, cnt: np.ndarray):

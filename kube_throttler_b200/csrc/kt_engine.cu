@@ -169,6 +169,10 @@ struct kt_ctx {
       d_st_throttled;
   bool have_reserved = false;
   DevBuf d_reserved, d_reserved_present, d_reserved_cnt;
+  // kt_append_throttle_rows: the spare halves the per-throttle arrays are widened into before each pair swaps (append_targets).
+  // Kept for the context's life, so that a creation allocates nothing once they are large enough: after the first append the
+  // per-throttle columns (thresholds, status, reservations: (3R + 10) x 8 bytes per throttle at most) take twice their size.
+  DevBuf w_spare[16];
   // pass state / outputs
   DevBuf d_part;   // 2 x [2R+1][M] u64 by pass parity: a reconciling pass adds into one half and leaves the other zeroed for its successor
   size_t part_stride = 0;  // bytes between the two halves
@@ -922,6 +926,7 @@ void kt_destroy(kt_ctx* c) {
   if (c->h_sparse_count) cudaFreeHost(c->h_sparse_count);
   c->d_sparse.release();
   for (DevBuf* b : all) b->release();
+  for (DevBuf& b : c->w_spare) b.release();
   for (auto& e : c->ev)
     if (e) cudaEventDestroy(e);
   if (c->own_stream) cudaStreamDestroy(c->own_stream);
@@ -1647,15 +1652,17 @@ int kt_update_namespace_rows(kt_ctx* c, int32_t n_ns, int64_t k, const int32_t* 
 
 // ---- selector column deltas (kt_tables.cc patch_columns, kt_nsrows.cuh k_ns_cols) --------------------------------------
 namespace {
-// The spec with column idx[i] taking column i of d (kind, ns_id, flags and terms), the others as they were.  The CSR is laid out
-// again column by column: every term's podSelector requirements first, then every term's namespaceSelector ones.
-SelectorSpec splice_spec(const SelectorSpec& old, int64_t k, const int32_t* idx, const SelectorSpec& d) {
-  const int32_t M = old.m;
+// The spec of m >= old.m columns with column idx[i] taking column i of d (kind, ns_id, flags and terms), the others as they were;
+// every column at or above old.m is listed.  The CSR is laid out again column by column: every term's podSelector requirements
+// first, then every term's namespaceSelector ones.
+SelectorSpec splice_spec(const SelectorSpec& old, int64_t k, const int32_t* idx, const SelectorSpec& d, int32_t m) {
+  const int32_t M = m;
   std::vector<int32_t> from((size_t)M, -1);
   for (int64_t i = 0; i < k; ++i) from[(size_t)idx[i]] = (int32_t)i;
   SelectorSpec s;
   s.m = M;
   s.kind = old.kind; s.flags = old.flags; s.ns_id = old.ns_id;
+  s.kind.resize((size_t)M); s.flags.resize((size_t)M); s.ns_id.resize((size_t)M);
   s.term_off.assign(1, 0);
   std::vector<std::pair<const SelectorSpec*, int32_t>> terms;  // (source, term) in the new order
   for (int32_t t = 0; t < M; ++t) {
@@ -1709,7 +1716,7 @@ int kt_update_selector_rows(kt_ctx* c, int64_t k, const int32_t* idx, const kt_t
   SelectorSpec d;
   const std::string e = copy_selector_spec((int32_t)k, cols, sel, &d);
   if (!e.empty()) return fail(c, KT_ERR_INVALID, "kt_update_selector_rows: selector table: %s", e.c_str());
-  SelectorSpec spec = splice_spec(c->spec, k, idx, d);
+  SelectorSpec spec = splice_spec(c->spec, k, idx, d, c->spec.m);
   int rc = set_device(c);
   if (rc) return rc;
   const bool fits = patch_columns(c->lim, c->spec, spec, std::vector<int32_t>(idx, idx + k), &c->ht);
@@ -1767,6 +1774,198 @@ int kt_update_selector_rows(kt_ctx* c, int64_t k, const int32_t* idx, const kt_t
     KT_CUDA(c, cudaGetLastError());
   }
   return rebuild_ns_words(c, NS, at[7]);
+}
+
+// ---- column appends (kt_tables.cc patch_columns, kt_nsrows.cuh k_widen_cols) ------------------------------------------
+namespace {
+// A resident per-throttle array an append widens: [rows][M] elements of esize bytes, swapped with its spare once widened.
+struct AppendTarget {
+  DevBuf* buf;
+  int64_t rows;
+  int32_t esize;
+  int add;  // index of the staged piece holding its new columns [rows][k], or -1: the new columns are zero
+};
+// The spec's kind and flags and the threshold columns (new columns staged at pieces 0-4), then the status and the reservations
+// when they are held (new columns zero: no calculatedAt, nothing used, nothing reserved).
+std::vector<AppendTarget> append_targets(kt_ctx* c) {
+  const int64_t R = c->lim.n_resources;
+  std::vector<AppendTarget> v = {{&c->d_kind, 1, 1, 0}, {&c->d_tflags, 1, 1, 1}, {&c->d_thr, R, 8, 2}, {&c->d_thr_present, 1, 4, 3},
+                                 {&c->d_thr_cnt, 1, 8, 4}};
+  if (c->have_status)
+    v.insert(v.end(), {{&c->d_st_calculated, 1, 1, -1}, {&c->d_st_calc_thr, R, 8, -1}, {&c->d_st_calc_present, 1, 4, -1},
+                       {&c->d_st_calc_cnt, 1, 8, -1}, {&c->d_st_used, R, 8, -1}, {&c->d_st_used_present, 1, 4, -1},
+                       {&c->d_st_used_cnt, 1, 8, -1}, {&c->d_st_throttled, 1, 4, -1}});
+  if (c->have_reserved)
+    v.insert(v.end(), {{&c->d_reserved, R, 8, -1}, {&c->d_reserved_present, 1, 4, -1}, {&c->d_reserved_cnt, 1, 8, -1}});
+  return v;
+}
+// Reserve b for `bytes`, keeping its first `keep` bytes: a grown buffer replaces b and the old one goes to `old`, to be released
+// once the stream has passed the copy.
+int reserve_keep(kt_ctx* c, DevBuf& b, size_t bytes, size_t keep, DevBuf& old) {
+  if (bytes <= b.cap) return KT_OK;
+  DevBuf grown;
+  KT_CUDA(c, grown.reserve(bytes));
+  if (keep) KT_CUDA(c, cudaMemcpyAsync(grown.p, b.p, keep, cudaMemcpyDeviceToDevice, c->stream));
+  std::swap(b, grown);
+  std::swap(old, grown);
+  return KT_OK;
+}
+}  // namespace
+
+int kt_append_throttle_rows(kt_ctx* c, int64_t k, const kt_throttle_cols* cols, const kt_selector_table* sel, int32_t* recompiled) {
+  if (!c) return KT_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(c->mu);
+  if (recompiled) *recompiled = 0;
+  if (k < 0) return fail(c, KT_ERR_INVALID, "kt_append_throttle_rows: k = %lld", (long long)k);
+  if (k > 0 && (!cols || !cols->kind || !cols->ns_id || !cols->flags || !cols->thr || !cols->thr_present || !cols->thr_cnt || !cols->ovr_off ||
+                !sel || !sel->term_off))
+    return fail(c, KT_ERR_INVALID, "kt_append_throttle_rows: null column with k = %lld", (long long)k);
+  if (!c->have_throttles) return fail(c, KT_ERR_STATE, "kt_append_throttle_rows before kt_upload_throttles");
+  if (k == 0) return KT_OK;
+  const int32_t M0 = c->M;
+  if (k > (int64_t)INT32_MAX - M0) return fail(c, KT_ERR_INVALID, "kt_append_throttle_rows: more than 2^31-1 throttles");
+  const int32_t* in_off = cols->ovr_off;
+  const int32_t n_in = in_off[k];
+  if (in_off[0] != 0 || n_in != cols->n_ovr) return fail(c, KT_ERR_INVALID, "kt_append_throttle_rows: ovr_off must span [0, n_ovr]");
+  for (int64_t i = 0; i < k; ++i)
+    if (in_off[i] > in_off[i + 1]) return fail(c, KT_ERR_INVALID, "kt_append_throttle_rows: ovr_off not monotone");
+  if (n_in > 0 && (!cols->ovr_begin || !cols->ovr_end || !cols->ovr_flags || !cols->ovr_thr || !cols->ovr_present || !cols->ovr_cnt))
+    return fail(c, KT_ERR_INVALID, "kt_append_throttle_rows: null override columns");
+  if ((int64_t)c->n_ovr + n_in > INT32_MAX) return fail(c, KT_ERR_INVALID, "kt_append_throttle_rows: more than 2^31-1 overrides");
+  SelectorSpec d;
+  const std::string e = copy_selector_spec((int32_t)k, cols, sel, &d);
+  if (!e.empty()) return fail(c, KT_ERR_INVALID, "kt_append_throttle_rows: selector table: %s", e.c_str());
+  const int32_t M1 = M0 + (int32_t)k;
+  std::vector<int32_t> idx((size_t)k), pos((size_t)k);
+  for (int32_t i = 0; i < (int32_t)k; ++i) { idx[(size_t)i] = M0 + i; pos[(size_t)i] = i; }
+  int rc = set_device(c);
+  if (rc) return rc;
+  const int32_t W0 = c->ht.W;
+  SelectorSpec spec = splice_spec(c->spec, k, idx.data(), d, M1);
+  const bool fits = patch_columns(c->lim, c->spec, spec, idx, &c->ht);
+  c->spec = std::move(spec);
+  // as after kt_upload_throttles: a pass is needed again before the getters that read one (status and reservations are kept)
+  c->evaluated = false;
+  c->have_codes = false;
+  c->have_diff = false;
+  const int R = c->lim.n_resources;
+  const size_t K = (size_t)k, N = (size_t)n_in;
+  // the override layout: the resident entries keep their offsets, the new columns' follow them
+  std::vector<int32_t> new_off(c->h_ovr_off);
+  new_off.resize((size_t)M1 + 1);
+  for (int64_t i = 0; i < k; ++i) new_off[(size_t)M0 + 1 + i] = c->n_ovr + in_off[i + 1];
+  const int32_t n_new = new_off[(size_t)M1];
+  // pass state sized by M, as kt_upload_throttles reserves it
+  const size_t part_bytes = (size_t)(2 * R + 1) * M1 * sizeof(unsigned long long);
+  c->part_stride = (part_bytes + 255) & ~(size_t)255;
+  KT_CUDA(c, c->d_part.reserve(2 * c->part_stride + 16));
+  KT_CUDA(c, cudaMemsetAsync(c->d_part.p, 0, c->d_part.cap, c->stream));
+  c->part_parity = 0;
+  c->win_stale = c->win != nullptr;  // laid out for the previous M
+  c->pre_stride = (size_t)((M1 + 31) & ~31) * pre_record_bytes(R);
+  KT_CUDA(c, c->d_pre.reserve(2 * c->pre_stride + 16));
+  KT_CUDA(c, c->d_changed.reserve(16 + (size_t)M1 * 5 + 16));
+  KT_CUDA(c, cudaMemsetAsync(c->d_changed.p, 0, 16, c->stream));
+  const size_t out_bytes = status_layout(R, M1).bytes;
+  KT_CUDA(c, c->d_out.reserve(out_bytes + 16));
+  KT_CUDA(c, c->h_call.reserve(out_bytes));  // (before the staged copy: a grown block would drop it)
+  // the widened arrays' spare halves and the spare override set
+  const std::vector<AppendTarget> tg = append_targets(c);
+  for (size_t j = 0; j < tg.size(); ++j) KT_CUDA(c, c->w_spare[j].reserve((size_t)tg[j].rows * M1 * tg[j].esize + 16));
+  KT_CUDA(c, c->s_ovr_off.reserve(((size_t)M1 + 1) * 4 + 16));
+  KT_CUDA(c, c->s_ovr_begin.reserve((size_t)n_new * 8 + 16));
+  KT_CUDA(c, c->s_ovr_end.reserve((size_t)n_new * 8 + 16));
+  KT_CUDA(c, c->s_ovr_flags.reserve((size_t)n_new + 16));
+  KT_CUDA(c, c->s_ovr_thr.reserve((size_t)R * n_new * 8 + 16));
+  KT_CUDA(c, c->s_ovr_present.reserve((size_t)n_new * 4 + 16));
+  KT_CUDA(c, c->s_ovr_cnt.reserve((size_t)n_new * 8 + 16));
+  // In place: the words from the one the first new column lands in up to the new W are recompiled on the host and cross as
+  // slices; when W grows, table and need grow (the existing words keep their place) and nsmask is restrided on the device.
+  const HostTables& h = c->ht;
+  const int32_t w0 = M0 >> 5, W1 = h.W, NS = h.NS, LN = c->lim.ns_label_slots;
+  const size_t tlen = (size_t)h.rows * h.TPpad * 2, nlen = (size_t)h.TPpad * h.B, ns_row0 = (size_t)W0 * h.TPpad, ns_row1 = (size_t)W1 * h.TPpad;
+  std::vector<int32_t> words;
+  DevBuf old_table, old_need, old_nsmask;
+  bool nsmask_widen = false;
+  if (fits) {
+    for (int32_t w = w0; w < W1; ++w) words.push_back(w);
+    if ((rc = reserve_keep(c, c->d_table, (size_t)W1 * tlen * 4 + 16, (size_t)w0 * tlen * 4, old_table)) ||
+        (rc = reserve_keep(c, c->d_need, (size_t)W1 * nlen * 4 + 16, (size_t)w0 * nlen * 4, old_need)))
+      return rc;
+    if (W1 > W0 && NS > 0) {
+      nsmask_widen = true;
+      std::swap(old_nsmask, c->d_nsmask);
+      KT_CUDA(c, c->d_nsmask.reserve((size_t)NS * ns_row1 * 4 + 16));
+    }
+    KT_CUDA(c, c->d_nsw_off.reserve(((size_t)NS + 1) * 4 + 16));
+    // the untouched words keep their entries, a touched word is in at most every list
+    KT_CUDA(c, c->d_nsw_idx.reserve(std::min((size_t)NS * W1, (size_t)c->nsw_total + (size_t)NS * words.size()) * 4 + 16));
+    KT_CUDA(c, c->d_call_out.reserve(((size_t)NS + 4) * 4 + 16));
+  }
+  const size_t nw = words.size();
+  static const int32_t result_slot[4] = {};
+  size_t at[20];
+  if ((rc = stage_pieces(c, {{cols->kind, K}, {cols->flags, K}, {cols->thr, (size_t)R * K * 8}, {cols->thr_present, K * 4}, {cols->thr_cnt, K * 8},
+                             {in_off, (K + 1) * 4}, {cols->ovr_begin, N * 8}, {cols->ovr_end, N * 8}, {cols->ovr_flags, N},
+                             {cols->ovr_thr, (size_t)R * N * 8}, {cols->ovr_present, N * 4}, {cols->ovr_cnt, N * 8}, {new_off.data(), new_off.size() * 4},
+                             {idx.data(), K * 4}, {pos.data(), K * 4}, {fits ? &h.table[(size_t)w0 * tlen] : nullptr, nw * tlen * 4},
+                             {fits ? &h.need[(size_t)w0 * nlen] : nullptr, nw * nlen * 4}, {words.data(), nw * 4},
+                             {c->ns_labels.data(), fits ? c->ns_labels.size() * 8 : 0}, {result_slot, sizeof result_slot}},
+                            at)))
+    return rc;
+  // one launch restrides every widened array (and lands the table and need slices, and restrides nsmask, in place)
+  WidenBatch wb{};
+  int64_t widest = 0;
+  auto add_array = [&](const void* src, const void* add, void* dst, int64_t rows, int64_t m_old, int64_t m_new, int32_t esize) {
+    wb.a[wb.n++] = WidenArray{static_cast<const unsigned char*>(src), static_cast<const unsigned char*>(add), static_cast<unsigned char*>(dst),
+                              rows, m_old, m_new, esize};
+    widest = std::max(widest, rows * m_new);
+  };
+  for (size_t j = 0; j < tg.size(); ++j)
+    add_array(tg[j].buf->p, tg[j].add >= 0 ? staged<unsigned char>(c, at[tg[j].add]) : nullptr, c->w_spare[j].p, tg[j].rows, M0, M1, tg[j].esize);
+  if (fits) {  // the slices of words [w0, W1) over the table and need (reserve_keep kept the words below w0)
+    add_array(nullptr, staged<unsigned char>(c, at[15]), c->d_table.as<uint32_t>() + (size_t)w0 * tlen, 1, 0, (int64_t)(nw * tlen), 4);
+    add_array(nullptr, staged<unsigned char>(c, at[16]), c->d_need.as<uint32_t>() + (size_t)w0 * nlen, 1, 0, (int64_t)(nw * nlen), 4);
+    if (nsmask_widen) add_array(old_nsmask.p, nullptr, c->d_nsmask.p, NS, (int64_t)ns_row0, (int64_t)ns_row1, 4);
+  }
+  const unsigned wblocks = (unsigned)std::min<int64_t>((widest + 255) / 256, 2048);
+  k_widen_cols<<<dim3(std::max(wblocks, 1u), (unsigned)wb.n), 256, 0, c->stream>>>(wb);
+  KT_CUDA(c, cudaGetLastError());
+  for (size_t j = 0; j < tg.size(); ++j) std::swap(*tg[j].buf, c->w_spare[j]);
+  // the override columns rebuilt into the spare set, the new columns' entries appended
+  const OverrideCols src{staged<int64_t>(c, at[6]), staged<int64_t>(c, at[7]), staged<uint8_t>(c, at[8]), staged<int64_t>(c, at[9]),
+                         staged<uint32_t>(c, at[10]), staged<int64_t>(c, at[11]), n_in};
+  const OverrideCols old{c->d_ovr_begin.as<int64_t>(), c->d_ovr_end.as<int64_t>(), c->d_ovr_flags.as<uint8_t>(), c->d_ovr_thr.as<int64_t>(),
+                         c->d_ovr_present.as<uint32_t>(), c->d_ovr_cnt.as<int64_t>(), c->n_ovr};
+  const OverrideOut out{c->s_ovr_begin.as<int64_t>(), c->s_ovr_end.as<int64_t>(), c->s_ovr_flags.as<uint8_t>(), c->s_ovr_thr.as<int64_t>(),
+                        c->s_ovr_present.as<uint32_t>(), c->s_ovr_cnt.as<int64_t>(), n_new};
+  k_rebuild_overrides<<<(unsigned)((M1 + 1 + 127) / 128), 128, 0, c->stream>>>(M1, R, k, staged<int32_t>(c, at[13]), staged<int32_t>(c, at[14]),
+                                                                             staged<int32_t>(c, at[12]), c->d_ovr_off.as<int32_t>(), old,
+                                                                             staged<int32_t>(c, at[5]), src, c->s_ovr_off.as<int32_t>(), out);
+  KT_CUDA(c, cudaGetLastError());
+  std::swap(c->d_ovr_off, c->s_ovr_off); std::swap(c->d_ovr_begin, c->s_ovr_begin); std::swap(c->d_ovr_end, c->s_ovr_end);
+  std::swap(c->d_ovr_flags, c->s_ovr_flags); std::swap(c->d_ovr_thr, c->s_ovr_thr); std::swap(c->d_ovr_present, c->s_ovr_present);
+  std::swap(c->d_ovr_cnt, c->s_ovr_cnt);
+  c->M = M1;
+  c->n_ovr = n_new;
+  c->h_ovr_off.swap(new_off);
+  if (!fits) {  // the tables compiled again from the grown spec (kt_upload_namespaces)
+    if ((rc = recompile_tables(c)) || (rc = stage_ns_spec(c))) return rc;
+    KT_CUDA(c, cudaStreamSynchronize(c->stream));
+    if (recompiled) *recompiled = 1;
+    return KT_OK;
+  }
+  if ((rc = stage_ns_spec(c))) return rc;  // term ranges, requirements and ns_id of the grown spec
+  if (NS > 0) {
+    k_ns_cols<<<(unsigned)(((int64_t)NS * (int64_t)nw + 7) / 8), 256, 0, c->stream>>>(ns_spec_view(c), NS, (int32_t)nw, staged<int32_t>(c, at[17]),
+                                                                                       staged<int64_t>(c, at[18]), LN, c->n_ns, c->d_nsmask.as<uint32_t>());
+    KT_CUDA(c, cudaGetLastError());
+  }
+  if ((rc = rebuild_ns_words(c, NS, at[19]))) return rc;
+  old_table.release();  // the stream has passed every read of the old buffers (rebuild_ns_words synchronised)
+  old_need.release();
+  old_nsmask.release();
+  return KT_OK;
 }
 
 int32_t kt_match_words(const kt_ctx* c) { return c && c->have_throttles ? c->ht.Wp : 0; }

@@ -40,6 +40,7 @@
 #pragma weak kt_update_namespace_rows  // without it (older engine doubles) every Namespace event uploads all namespace rows
 #pragma weak kt_update_threshold_rows  // without it (older engine doubles) every threshold or override edit recompiles the tables
 #pragma weak kt_update_selector_rows   // without it (older engine doubles) every deletion and selector edit recompiles the tables
+#pragma weak kt_append_throttle_rows   // without it (older engine doubles) every creation recompiles the tables, hole fills included
 
 namespace {
 
@@ -535,6 +536,7 @@ struct kth_plugin {
   long long words_stat = -1;  // kth_queue_stats: words per namespace of the current layout (-1: not computed)
   uint64_t thr_seq = 0;
   bool thr_reused = false;  // some column holds a younger throttle than a higher one: column order is not creation order any more
+  size_t m_dev = 0;  // throttle columns the engine holds: [m_dev, throttles.size()) are creations appended by the next sync
   template <class V>
   void creation_order(V& cols_list) const {  // sort a list of throttle columns by creation
     if (thr_reused) std::stable_sort(cols_list.begin(), cols_list.end(), [&](size_t a, size_t b) { return throttles[a].seq < throttles[b].seq; });
@@ -1035,6 +1037,7 @@ struct kth_plugin {
     const kt_selector_table st = scols.table();
     sync_namespaces();  // Throttle rows may have introduced namespace ids
     check(kt_upload_throttles(ctx, (int32_t)m, &tc, &st), "kt_upload_throttles");
+    m_dev = m;
     throttles_dirty = false;
     status_dirty = reserved_dirty = true;  // kt_upload_throttles forgets both
     spec_cols.clear();
@@ -1104,6 +1107,22 @@ struct kth_plugin {
       sc.ns_req_off.push_back((int32_t)sc.req_key.size());
     }
     return sc;
+  }
+  // Creations placed at the end (apply_throttle, place_creation): the columns [m_dev, m) in one kt_append_throttle_rows, before
+  // any column delta that may list them.  Their status and reservations, when not zero, follow as column deltas (status_cols /
+  // reserved_cols, set by apply_throttle).
+  void sync_appends() {
+    const size_t m = throttles.size();
+    if (m_dev >= m) return;
+    std::vector<size_t> list;
+    for (size_t t = m_dev; t < m; ++t) list.push_back(t);
+    const SelectorColumns scols = selector_columns(list);
+    const ThresholdColumns tcols = threshold_columns(list);
+    kt_throttle_cols tc = tcols.cols();
+    scols.put(&tc);
+    const kt_selector_table st = scols.table();
+    check(kt_append_throttle_rows(ctx, (int64_t)list.size(), &tc, &st, nullptr), "kt_append_throttle_rows");
+    m_dev = m;
   }
   // Deletions and in-place selector / throttlerName edits (delete_throttle, apply_throttle): one kt_update_selector_rows for the
   // listed columns, with the column layout kept.  The engine patches its tables when the new terms fit them and compiles them
@@ -1332,7 +1351,8 @@ struct kth_plugin {
     sync_pods();
     sync_namespaces();
     sync_throttles();
-    sync_selectors();   // (after sync_throttles, which sends these columns too when it uploads the throttles)
+    sync_appends();     // (after sync_throttles, which sends these columns too when it uploads the throttles)
+    sync_selectors();   // (after both: a hole fill or an edit may list an appended column)
     sync_thresholds();
   }
   // Everything a PreFilter view reads: the tables, the informer copy of the statuses and the reservations.  A table change voids
@@ -2956,6 +2976,30 @@ struct kth_plugin {
     auto it = thr_index.find(key);
     if (it == thr_index.end()) {
       o.seq = ++thr_seq;
+      const long at = creation_delta(o, epoch) ? place_creation(o) : -1;
+      if (at >= 0) {  // a column delta: a hole filled in place, or a column appended by the next sync
+        const size_t t = (size_t)at;
+        const bool reserved_any = [&] {
+          auto r = cache[o.kind].by_thr.find(o.nn());
+          return r != cache[o.kind].by_thr.end() && !r->second.empty();
+        }();
+        thr_index[key] = (int)t;
+        if (t < throttles.size()) {
+          free_thr.erase(std::find(free_thr.begin(), free_thr.end(), (int)t));
+          throttles[t] = std::move(o);
+          thr_reused = true;
+          sel_cols.add(t);
+          spec_cols.add(t);
+          status_cols.add(t);
+          reserved_cols.add(t);  // the reservation cache keeps a deleted name's entries: a re-created name gets its totals back
+        } else {
+          throttles.push_back(std::move(o));
+          if (has_status) status_cols.add(t);
+          if (reserved_any) reserved_cols.add(t);
+        }
+        selector_changed(t, true);
+        return;
+      }
       if (!free_thr.empty()) {  // the column of a deleted throttle (everything per column is re-uploaded: throttles_dirty below)
         const int t = free_thr.back();
         free_thr.pop_back();
@@ -3030,6 +3074,42 @@ struct kth_plugin {
   }
   // Whether a deletion or a selector edit can go as a column delta: the engine has the call and no whole upload is pending.
   bool selector_delta() const { return kt_update_selector_rows && !throttles_dirty; }
+  // Whether a creation can go as a column delta: the engine has every call it needs, no whole upload is pending, no resource
+  // column or scale changed (epoch), the selectors mention only known label keys and values, and a Throttle's namespace has an
+  // id already (one first met here changes the namespace rows and keeps the full path).
+  bool creation_delta(const ThrottleObj& o, uint64_t epoch) const {
+    return kt_append_throttle_rows && selector_delta() && kt_update_threshold_rows && kt_update_status_rows && kt_update_reserved_rows &&
+           epoch == col_epoch && in_vocabulary(o) && (o.kind != KT_KIND_THROTTLE || ns_dict.find(o.ns) >= 0);
+  }
+  // The column of a creation that goes as a column delta, or -1 (the full path, which lays the columns out again).  A pass costs
+  // the words on each namespace's list (reorder_columns), so the new column goes where it adds no word to any list beyond what
+  // the creation itself must add.  Its group is its namespace (a Throttle) or its namespace set (a ClusterThrottle,
+  // namespace_set_of), as in reorder_columns:
+  //   1. a hole in a 32-throttle word that holds a live column of the group;
+  //   2. else, when the last word holds a live column of the group and has room, a new column at the end;
+  //   3. else, when the group has no live column (every word it gets is one it must add): any hole, else a new column;
+  //   4. else -1.
+  long place_creation(const ThrottleObj& o) const {
+    std::map<std::string, std::string> set_of;  // ClusterThrottle signature -> namespace set, evaluated once each
+    auto group = [&](const ThrottleObj& x) -> const std::string& {
+      if (x.kind == KT_KIND_THROTTLE) return x.ns;
+      const std::string sig = ns_selector_signature(x);
+      auto it = set_of.find(sig);
+      if (it == set_of.end()) it = set_of.emplace(sig, namespace_set_of(x)).first;
+      return it->second;
+    };
+    const std::string g = group(o);
+    const size_t m = throttles.size();
+    std::vector<char> holds((m + 31) / 32 + 1, 0);
+    bool any = false;
+    for (size_t t = 0; t < m; ++t)
+      if (throttles[t].live && throttles[t].kind == o.kind && group(throttles[t]) == g) holds[t >> 5] = any = true;
+    for (int t : free_thr)
+      if (holds[(size_t)t >> 5]) return t;
+    if (m % 32 && holds[m >> 5]) return (long)m;
+    if (!any) return free_thr.empty() ? (long)m : free_thr.back();
+    return -1;
+  }
   // Every label key and value the throttle's selectors mention is in the dictionaries already: sync_vocabulary would intern
   // nothing, so no pod or namespace row has to be packed again.
   bool in_vocabulary(const ThrottleObj& o) const {

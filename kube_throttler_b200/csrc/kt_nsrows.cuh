@@ -16,6 +16,8 @@
 // A selector column delta changes the other axis: k_ns_cols re-evaluates the listed 32-throttle words for every namespace with
 // the same per-lane walk as k_ns_rows (ns_word_planes), then steps 2-5 follow.  k_scatter_words / k_scatter_kind_flags land the
 // host-recompiled table and need slices of those words and the listed columns' kind and flags.
+// A column append (kt_append_throttle_rows) grows M: k_widen_cols restrides the resident per-throttle arrays (and nsmask when W
+// grows) in one launch, filling in the staged new columns, then k_ns_cols takes the touched words and steps 2-5 follow.
 #pragma once
 #include "kt_keyed.cuh"
 
@@ -134,6 +136,41 @@ __global__ void __launch_bounds__(256) k_scatter_words(int64_t nw, const int32_t
     const int64_t j = i / len, e = i - j * len;
     dst[(int64_t)__ldg(&words[j]) * len + e] = src[i];
   }
+}
+
+// One array of `rows` rows of `esize`-byte elements (1, 4 or 8) widened from m_old to m_new elements per row: element e < m_old of
+// row r from src[r * m_old + e], the others from add[r * (m_new - m_old) + e - m_old], or zero when add is null.  dst must not
+// overlap src.  With m_old = 0 and src null it is a plain copy of `add` into dst.
+struct WidenArray {
+  const unsigned char* src;
+  const unsigned char* add;
+  unsigned char* dst;
+  int64_t rows, m_old, m_new;
+  int32_t esize;
+};
+constexpr int kMaxWiden = 24;
+struct WidenBatch {
+  WidenArray a[kMaxWiden];
+  int32_t n;
+};
+template <class T>
+__device__ __forceinline__ void widen_elems(const WidenArray& a, int64_t i0, int64_t stride) {
+  const T* src = reinterpret_cast<const T*>(a.src);
+  const T* add = reinterpret_cast<const T*>(a.add);
+  T* dst = reinterpret_cast<T*>(a.dst);
+  const int64_t k = a.m_new - a.m_old, n = a.rows * a.m_new;
+  for (int64_t i = i0; i < n; i += stride) {
+    const int64_t r = i / a.m_new, e = i - r * a.m_new;
+    dst[i] = e < a.m_old ? src[r * a.m_old + e] : add ? add[r * k + (e - a.m_old)] : T(0);
+  }
+}
+// grid (x, b.n): blockIdx.y is the array
+__global__ void __launch_bounds__(256) k_widen_cols(const WidenBatch b) {
+  const WidenArray& a = b.a[blockIdx.y];
+  const int64_t i0 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x, stride = (int64_t)gridDim.x * blockDim.x;
+  if (a.esize == 8) widen_elems<uint64_t>(a, i0, stride);
+  else if (a.esize == 4) widen_elems<uint32_t>(a, i0, stride);
+  else widen_elems<uint8_t>(a, i0, stride);
 }
 
 // kind and flags of the k listed throttle columns (kt_update_selector_rows)

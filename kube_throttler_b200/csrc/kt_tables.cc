@@ -306,6 +306,7 @@ std::string compile_tables(const kt_limits& lim, const SelectorSpec& s, int32_t 
 
 bool patch_columns(const kt_limits& lim, const SelectorSpec& old_s, const SelectorSpec& s, const std::vector<int32_t>& listed, HostTables* h) {
   const int32_t M = s.m, TPp = h->TPpad, B = h->B, rows = h->rows;
+  if (M < h->M) return false;
   std::vector<char> is_listed((size_t)M, 0);
   for (int32_t t : listed) {  // does every listed column fit the resident tables?
     is_listed[(size_t)t] = 1;
@@ -317,6 +318,17 @@ bool patch_columns(const kt_limits& lim, const SelectorSpec& old_s, const Select
         for (int32_t i = s.req_val_off[q]; i < s.req_val_off[q + 1]; ++i)
           if (!h->pair_row.count(((uint64_t)s.req_key[q] << 32) | s.req_vals[i])) return false;
       }
+  }
+  for (int32_t t = h->M; t < M; ++t)
+    if (!is_listed[(size_t)t]) return false;  // a column the spec grew by must be listed
+  if (M > h->M) {  // new words appended as compile_tables starts them (sat = 1, pos = 0, no need); existing words keep their place
+    const int32_t W = std::max(1, (M + 31) / 32);
+    h->table.resize((size_t)W * rows * TPp * 2, 0);
+    for (size_t e = (size_t)h->W * rows * TPp * 2; e < h->table.size(); e += 2) h->table[e] = 0xffffffffu;
+    h->need.resize((size_t)W * TPp * B, 0);
+    h->M = M;
+    h->W = W;
+    h->Wp = words_per_row(M);
   }
   // term_unsat follows the new term numbering: the unlisted columns keep theirs
   std::vector<uint8_t> unsat((size_t)s.term_off[M], 0);

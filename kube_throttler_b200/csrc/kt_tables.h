@@ -80,10 +80,12 @@ int32_t compile_column(const kt_limits& lim, const SelectorSpec& spec, int32_t t
                        int32_t TPpad, uint32_t* word_table, int32_t* need, uint8_t* term_unsat);
 
 // The listed columns of h (compiled from old_spec) recompiled in place from `spec`, which equals old_spec but for the listed
-// columns: their table bits, need planes and term_unsat entries, with compile_column.  false when one of them does not fit the
-// resident tables -- a podSelector key or (key, value) without a row, more terms than TPpad, a need beyond the B counter planes,
-// a Throttle namespace beyond NS --; h is then partly patched and must be compiled again.  The namespace masks and word lists
-// are not touched (nsmask, nsw_off, nsw_idx, max_ns_words).
+// columns: their table bits, need planes and term_unsat entries, with compile_column.  `spec` may be longer than old_spec when
+// every column it grew by is listed: M, W and Wp grow, and the words it adds are appended to `table` and `need` (the existing
+// words keep their place).  false when one of them does not fit the resident tables -- a podSelector key or (key, value)
+// without a row, more terms than TPpad, a need beyond the B counter planes, a Throttle namespace beyond NS --; h is then partly
+// patched and must be compiled again.  The namespace masks and word lists are not touched (nsmask, nsw_off, nsw_idx,
+// max_ns_words), nor resized when W grows.
 bool patch_columns(const kt_limits& lim, const SelectorSpec& old_spec, const SelectorSpec& spec, const std::vector<int32_t>& listed,
                    HostTables* h);
 
