@@ -368,6 +368,23 @@ int kt_update_selector_rows(kt_ctx* ctx, int64_t k, const int32_t* idx, const kt
  * buffers on return.  Multi-GPU: the call is local, not collective -- every rank must apply the same appends. */
 int kt_append_throttle_rows(kt_ctx* ctx, int64_t k, const kt_throttle_cols* cols, const kt_selector_table* sel,
                             int32_t* recompiled);
+/* The throttle columns laid out again: column j of the new layout is previous column src[j], for j in [0, m).  Afterwards every
+ * call answers exactly as after a kt_upload_throttles(ctx, m, spec') whose column j is previous column src[j] -- kind, ns_id,
+ * flags, selector terms, threshold and overrides --, followed by re-uploading the status and the reservations held before the
+ * call, gathered the same way.  src[j] == -1 makes an empty column: kind ClusterThrottle, ns_id -1, flags 0, no terms, no
+ * threshold, no overrides, zero status and nothing reserved; it matches nothing and adds no word to any namespace's list.
+ * Previous columns src does not name are dropped; m may be smaller than, equal to or larger than M.  Status or reservations not
+ * held before the call are still not held.  The state flags move as kt_update_selector_rows moves them (a pass is needed again
+ * before the getters that read one); kt_match_words may change.
+ * KT_ERR_INVALID: m < 0; a null src with m > 0; an entry outside [-1, M); a non-negative entry listed twice.  KT_ERR_STATE
+ * before kt_upload_throttles.
+ * Always in place, never a table compile: every per-column thing the device holds is column-local, so the move is a gather.  The
+ * table-row dictionary, TPpad, the counter planes and the namespace count are kept, and the pod rows keep their table offsets.
+ * The table, need and namespace-mask bits are gathered by column on the device, the per-throttle columns restrided and the
+ * override columns rebuilt through the column map, the word lists rebuilt.  One staged copy (src and the new override offsets)
+ * and one synchronisation; the caller may reuse src on return.  Multi-GPU: the call is local, not collective -- every rank must
+ * apply the same move. */
+int kt_move_throttle_columns(kt_ctx* ctx, int32_t m, const int32_t* src /*[m]*/);
 
 /* ---- the pass ------------------------------------------------------------------- */
 /* One batched pass: reconcile every throttle (throttle_controller.go:84-133) and check

@@ -43,7 +43,7 @@ def build(force: bool = False) -> str:
 EXPORTS = [
     "kt_create", "kt_destroy", "kt_last_error", "kt_version", "kt_set_stream", "kt_sync", "kt_enable_timing",
     "kt_enable_trace", "kt_get_trace", "kt_host_alloc", "kt_host_alloc_upload", "kt_host_free", "kt_upload_pods", "kt_upload_pods_compact", "kt_upload_pods_packed", "kt_set_async_uploads", "kt_update_pod_rows", "kt_upload_namespaces", "kt_update_namespace_rows",
-    "kt_upload_throttles", "kt_upload_status", "kt_set_reserved", "kt_update_status_rows", "kt_update_reserved_rows", "kt_update_threshold_rows", "kt_update_selector_rows", "kt_append_throttle_rows", "kt_evaluate", "kt_get_reconcile",
+    "kt_upload_throttles", "kt_upload_status", "kt_set_reserved", "kt_update_status_rows", "kt_update_reserved_rows", "kt_update_threshold_rows", "kt_update_selector_rows", "kt_append_throttle_rows", "kt_move_throttle_columns", "kt_evaluate", "kt_get_reconcile",
     "kt_match_words", "kt_get_match_bitmap", "kt_get_match_rows", "kt_get_match_columns", "kt_get_check_summary", "kt_reconcile_throttles", "kt_get_check", "kt_set_sparse_check", "kt_get_check_sparse", "kt_get_check_rows", "kt_check_pending_rows", "kt_match_pods", "kt_check_pods", "kt_get_changed", "kt_get_reconcile_rows", "kt_step_submit", "kt_step_wait", "kt_admit_queue", "kt_get_timing", "kt_comm_unique_id",
     "kt_comm_init", "kt_comm_destroy", "kt_debug_compile_tables", "kt_debug_set_pass_plan", "kt_debug_get_pass_plan", "kt_debug_get_ns_tables",
     "kt_debug_set_row_order", "kt_debug_get_row_order",
@@ -103,6 +103,7 @@ def lib():
         L.kt_update_threshold_rows.argtypes = [vp, C.c_int64, vp, C.POINTER(abi.ThrottleCols)]
         L.kt_update_selector_rows.argtypes = [vp, C.c_int64, vp, C.POINTER(abi.ThrottleCols), C.POINTER(abi.SelectorTable), vp]
         L.kt_append_throttle_rows.argtypes = [vp, C.c_int64, C.POINTER(abi.ThrottleCols), C.POINTER(abi.SelectorTable), vp]
+        L.kt_move_throttle_columns.argtypes = [vp, C.c_int32, vp]
         L.kt_evaluate.argtypes = [vp, C.c_int64, C.c_uint32]
         L.kt_get_reconcile.argtypes = [vp, C.POINTER(abi.ReconcileOut)]
         L.kt_match_words.argtypes = [vp]
@@ -366,6 +367,13 @@ class Engine:
         self._ck(self._L.kt_append_throttle_rows(self._h, k, C.byref(tc), C.byref(st), abi.ptr(out)))
         self.m += k
         return bool(out[0])
+
+    def move_throttle_columns(self, src) -> None:
+        """kt_move_throttle_columns: the throttle columns laid out again, column j taking previous column src[j] (spec, thresholds,
+        overrides, status and reservations), or an empty column for -1; previous columns src does not name are dropped."""
+        a = abi._arr(src, np.int32)
+        self._ck(self._L.kt_move_throttle_columns(self._h, int(a.shape[0]), abi.ptr(a)))
+        self.m = int(a.shape[0])
 
     def update_reserved_rows(self, idx: np.ndarray, reserved: np.ndarray, present: np.ndarray, cnt: np.ndarray):
         """kt_update_reserved_rows: reserved[R][k], present[k], cnt[k] of the listed throttle columns, replaced in place (the

@@ -173,6 +173,8 @@ struct kt_ctx {
   // Kept for the context's life, so that a creation allocates nothing once they are large enough: after the first append the
   // per-throttle columns (thresholds, status, reservations: (3R + 10) x 8 bytes per throttle at most) take twice their size.
   DevBuf w_spare[16];
+  // kt_move_throttle_columns: the spare table, need and nsmask the column gather writes into before each pair swaps
+  DevBuf g_spare[3];
   // pass state / outputs
   DevBuf d_part;   // 2 x [2R+1][M] u64 by pass parity: a reconciling pass adds into one half and leaves the other zeroed for its successor
   size_t part_stride = 0;  // bytes between the two halves
@@ -927,6 +929,7 @@ void kt_destroy(kt_ctx* c) {
   c->d_sparse.release();
   for (DevBuf* b : all) b->release();
   for (DevBuf& b : c->w_spare) b.release();
+  for (DevBuf& b : c->g_spare) b.release();
   for (auto& e : c->ev)
     if (e) cudaEventDestroy(e);
   if (c->own_stream) cudaStreamDestroy(c->own_stream);
@@ -1526,7 +1529,7 @@ int kt_update_threshold_rows(kt_ctx* c, int64_t k, const int32_t* idx, const kt_
                           c->s_ovr_present.as<uint32_t>(), c->s_ovr_cnt.as<int64_t>(), n_new};
     k_rebuild_overrides<<<(unsigned)((M + 1 + 127) / 128), 128, 0, c->stream>>>(
         M, R, k, staged<int32_t>(c, at[12]), staged<int32_t>(c, at[13]), staged<int32_t>(c, at[11]), c->d_ovr_off.as<int32_t>(), old,
-        staged<int32_t>(c, at[4]), src, c->s_ovr_off.as<int32_t>(), out);
+        staged<int32_t>(c, at[4]), src, c->s_ovr_off.as<int32_t>(), out, nullptr);
     KT_CUDA(c, cudaGetLastError());
     std::swap(c->d_ovr_off, c->s_ovr_off); std::swap(c->d_ovr_begin, c->s_ovr_begin); std::swap(c->d_ovr_end, c->s_ovr_end);
     std::swap(c->d_ovr_flags, c->s_ovr_flags); std::swap(c->d_ovr_thr, c->s_ovr_thr); std::swap(c->d_ovr_present, c->s_ovr_present);
@@ -1652,24 +1655,28 @@ int kt_update_namespace_rows(kt_ctx* c, int32_t n_ns, int64_t k, const int32_t* 
 
 // ---- selector column deltas (kt_tables.cc patch_columns, kt_nsrows.cuh k_ns_cols) --------------------------------------
 namespace {
-// The spec of m >= old.m columns with column idx[i] taking column i of d (kind, ns_id, flags and terms), the others as they were;
-// every column at or above old.m is listed.  The CSR is laid out again column by column: every term's podSelector requirements
-// first, then every term's namespaceSelector ones.
-SelectorSpec splice_spec(const SelectorSpec& old, int64_t k, const int32_t* idx, const SelectorSpec& d, int32_t m) {
+// The spec of m columns with column idx[i] taking column i of d (kind, ns_id, flags and terms), the others old column base[t]
+// -- or, without base, old column t: every column at or above old.m is then listed.  base[t] == -1 makes an empty column
+// (ClusterThrottle, ns_id -1, flags 0, no terms).  The CSR is laid out again column by column: every term's podSelector
+// requirements first, then every term's namespaceSelector ones.
+SelectorSpec splice_spec(const SelectorSpec& old, int64_t k, const int32_t* idx, const SelectorSpec& d, int32_t m, const int32_t* base = nullptr) {
   const int32_t M = m;
   std::vector<int32_t> from((size_t)M, -1);
   for (int64_t i = 0; i < k; ++i) from[(size_t)idx[i]] = (int32_t)i;
   SelectorSpec s;
   s.m = M;
-  s.kind = old.kind; s.flags = old.flags; s.ns_id = old.ns_id;
-  s.kind.resize((size_t)M); s.flags.resize((size_t)M); s.ns_id.resize((size_t)M);
+  s.kind.assign((size_t)M, KT_KIND_CLUSTERTHROTTLE); s.flags.assign((size_t)M, 0); s.ns_id.assign((size_t)M, -1);
   s.term_off.assign(1, 0);
   std::vector<std::pair<const SelectorSpec*, int32_t>> terms;  // (source, term) in the new order
   for (int32_t t = 0; t < M; ++t) {
     const int32_t i = from[(size_t)t];
     const SelectorSpec& src = i >= 0 ? d : old;
-    const int32_t col = i >= 0 ? i : t;
-    if (i >= 0) { s.kind[(size_t)t] = d.kind[(size_t)i]; s.flags[(size_t)t] = d.flags[(size_t)i]; s.ns_id[(size_t)t] = d.ns_id[(size_t)i]; }
+    const int32_t col = i >= 0 ? i : base ? base[t] : t;
+    if (col < 0 || col >= src.m) {
+      s.term_off.push_back((int32_t)terms.size());
+      continue;
+    }
+    s.kind[(size_t)t] = src.kind[(size_t)col]; s.flags[(size_t)t] = src.flags[(size_t)col]; s.ns_id[(size_t)t] = src.ns_id[(size_t)col];
     for (int32_t term = src.term_off[(size_t)col]; term < src.term_off[(size_t)col + 1]; ++term) {
       terms.emplace_back(&src, term);
       s.term_flags.push_back(src.term_flags[(size_t)term]);
@@ -1941,7 +1948,7 @@ int kt_append_throttle_rows(kt_ctx* c, int64_t k, const kt_throttle_cols* cols, 
                         c->s_ovr_present.as<uint32_t>(), c->s_ovr_cnt.as<int64_t>(), n_new};
   k_rebuild_overrides<<<(unsigned)((M1 + 1 + 127) / 128), 128, 0, c->stream>>>(M1, R, k, staged<int32_t>(c, at[13]), staged<int32_t>(c, at[14]),
                                                                              staged<int32_t>(c, at[12]), c->d_ovr_off.as<int32_t>(), old,
-                                                                             staged<int32_t>(c, at[5]), src, c->s_ovr_off.as<int32_t>(), out);
+                                                                             staged<int32_t>(c, at[5]), src, c->s_ovr_off.as<int32_t>(), out, nullptr);
   KT_CUDA(c, cudaGetLastError());
   std::swap(c->d_ovr_off, c->s_ovr_off); std::swap(c->d_ovr_begin, c->s_ovr_begin); std::swap(c->d_ovr_end, c->s_ovr_end);
   std::swap(c->d_ovr_flags, c->s_ovr_flags); std::swap(c->d_ovr_thr, c->s_ovr_thr); std::swap(c->d_ovr_present, c->s_ovr_present);
@@ -1965,6 +1972,145 @@ int kt_append_throttle_rows(kt_ctx* c, int64_t k, const kt_throttle_cols* cols, 
   old_table.release();  // the stream has passed every read of the old buffers (rebuild_ns_words synchronised)
   old_need.release();
   old_nsmask.release();
+  return KT_OK;
+}
+
+// ---- column moves (kt_nsrows.cuh k_gather_bits; k_widen_cols and k_rebuild_overrides through a column map) --------------
+int kt_move_throttle_columns(kt_ctx* c, int32_t m, const int32_t* src) {
+  if (!c) return KT_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(c->mu);
+  if (m < 0) return fail(c, KT_ERR_INVALID, "kt_move_throttle_columns: m = %d", m);
+  if (m > 0 && !src) return fail(c, KT_ERR_INVALID, "kt_move_throttle_columns: null src with m = %d", m);
+  if (!c->have_throttles) return fail(c, KT_ERR_STATE, "kt_move_throttle_columns before kt_upload_throttles");
+  const int32_t M0 = c->M;
+  std::vector<char> named((size_t)M0, 0);
+  for (int32_t j = 0; j < m; ++j) {
+    if (src[j] < -1 || src[j] >= M0)
+      return fail(c, KT_ERR_INVALID, "kt_move_throttle_columns: column %d from %d, out of range [-1,%d)", j, src[j], M0);
+    if (src[j] >= 0 && named[(size_t)src[j]]++) return fail(c, KT_ERR_INVALID, "kt_move_throttle_columns: column %d listed twice", src[j]);
+  }
+  int rc = set_device(c);
+  if (rc) return rc;
+  const int R = c->lim.n_resources;
+  HostTables& h = c->ht;
+  // The gathered spec, its term_unsat entries and override offsets.  The row dictionary, TPpad, B and NS are kept: no column is
+  // compiled, so the table and need bits are gathered on the device and brought back for the host mirror (patch_columns reads
+  // it), which costs one copy of the two arrays instead of a bit-by-bit permutation of them on the host.
+  SelectorSpec spec = splice_spec(c->spec, 0, nullptr, SelectorSpec{}, m, src);
+  std::vector<uint8_t> unsat;
+  unsat.reserve(spec.term_flags.size());
+  std::vector<int32_t> new_off((size_t)m + 1, 0);
+  for (int32_t j = 0; j < m; ++j) {
+    const int32_t t = src[j];
+    int32_t n = 0;
+    if (t >= 0) {
+      unsat.insert(unsat.end(), h.term_unsat.begin() + c->spec.term_off[(size_t)t], h.term_unsat.begin() + c->spec.term_off[(size_t)t + 1]);
+      n = c->h_ovr_off[(size_t)t + 1] - c->h_ovr_off[(size_t)t];
+    }
+    new_off[(size_t)j + 1] = new_off[(size_t)j] + n;  // at most n_ovr: every previous column is named once at most
+  }
+  const int32_t n_new = new_off[(size_t)m];
+  const int32_t W0 = h.W, W1 = std::max(1, (m + 31) / 32), NS = h.NS, TPpad = h.TPpad;
+  const size_t tlen = (size_t)h.rows * TPpad * 2, nlen = (size_t)TPpad * h.B;
+  // pass state sized by M, as kt_upload_throttles reserves it
+  const size_t part_bytes = (size_t)(2 * R + 1) * m * sizeof(unsigned long long);
+  c->part_stride = (part_bytes + 255) & ~(size_t)255;
+  KT_CUDA(c, c->d_part.reserve(2 * c->part_stride + 16));
+  KT_CUDA(c, cudaMemsetAsync(c->d_part.p, 0, c->d_part.cap, c->stream));
+  c->part_parity = 0;
+  c->win_stale = c->win != nullptr;  // laid out for the previous M
+  c->pre_stride = (size_t)((m + 31) & ~31) * pre_record_bytes(R);
+  KT_CUDA(c, c->d_pre.reserve(2 * c->pre_stride + 16));
+  KT_CUDA(c, c->d_changed.reserve(16 + (size_t)m * 5 + 16));
+  KT_CUDA(c, cudaMemsetAsync(c->d_changed.p, 0, 16, c->stream));
+  const size_t out_bytes = status_layout(R, m).bytes;
+  KT_CUDA(c, c->d_out.reserve(out_bytes + 16));
+  // the restrided arrays' spare halves, the spare override set, the gathered bit arrays and the word lists
+  const std::vector<AppendTarget> tg = append_targets(c);
+  for (size_t j = 0; j < tg.size(); ++j) KT_CUDA(c, c->w_spare[j].reserve((size_t)tg[j].rows * m * tg[j].esize + 16));
+  KT_CUDA(c, c->s_ovr_off.reserve(((size_t)m + 1) * 4 + 16));
+  KT_CUDA(c, c->s_ovr_begin.reserve((size_t)n_new * 8 + 16));
+  KT_CUDA(c, c->s_ovr_end.reserve((size_t)n_new * 8 + 16));
+  KT_CUDA(c, c->s_ovr_flags.reserve((size_t)n_new + 16));
+  KT_CUDA(c, c->s_ovr_thr.reserve((size_t)R * n_new * 8 + 16));
+  KT_CUDA(c, c->s_ovr_present.reserve((size_t)n_new * 4 + 16));
+  KT_CUDA(c, c->s_ovr_cnt.reserve((size_t)n_new * 8 + 16));
+  KT_CUDA(c, c->g_spare[0].reserve((size_t)W1 * tlen * 4 + 16));
+  KT_CUDA(c, c->g_spare[1].reserve((size_t)W1 * nlen * 4 + 16));
+  KT_CUDA(c, c->g_spare[2].reserve((size_t)NS * W1 * TPpad * 4 + 16));
+  KT_CUDA(c, c->d_nsw_off.reserve(((size_t)NS + 1) * 4 + 16));
+  KT_CUDA(c, c->d_nsw_idx.reserve((size_t)NS * W1 * 4 + 16));
+  KT_CUDA(c, c->d_call_out.reserve(((size_t)NS + 4) * 4 + 16));
+  // the pinned call block: the staged pieces, then where the gathered table and need land (reserved first: a grown block would
+  // drop the staged pieces)
+  auto pad = [](size_t b) { return (b + 15) & ~(size_t)15; };
+  const size_t land = pad((size_t)m * 4) + pad(((size_t)m + 1) * 4) + 16, tbytes = (size_t)W1 * tlen * 4, nbytes = (size_t)W1 * nlen * 4;
+  KT_CUDA(c, c->h_call.reserve(std::max(out_bytes, land + tbytes + nbytes)));
+  static const int32_t result_slot[4] = {};
+  size_t at[3];
+  if ((rc = stage_pieces(c, {{src, (size_t)m * 4}, {new_off.data(), new_off.size() * 4}, {result_slot, sizeof result_slot}}, at))) return rc;
+  const int32_t* map = staged<int32_t>(c, at[0]);
+  // one launch restrides every per-throttle array through the map
+  WidenBatch wb{};
+  int64_t widest = 0;
+  for (size_t j = 0; j < tg.size(); ++j) {
+    wb.a[wb.n++] = WidenArray{static_cast<const unsigned char*>(tg[j].buf->p), nullptr, static_cast<unsigned char*>(c->w_spare[j].p), tg[j].rows,
+                              M0, m, tg[j].esize, map};
+    widest = std::max(widest, tg[j].rows * m);
+  }
+  const unsigned wblocks = (unsigned)std::min<int64_t>((widest + 255) / 256, 2048);
+  k_widen_cols<<<dim3(std::max(wblocks, 1u), (unsigned)wb.n), 256, 0, c->stream>>>(wb);
+  KT_CUDA(c, cudaGetLastError());
+  for (size_t j = 0; j < tg.size(); ++j) std::swap(*tg[j].buf, c->w_spare[j]);
+  // the override columns rebuilt into the spare set through the map
+  const OverrideCols old{c->d_ovr_begin.as<int64_t>(), c->d_ovr_end.as<int64_t>(), c->d_ovr_flags.as<uint8_t>(), c->d_ovr_thr.as<int64_t>(),
+                         c->d_ovr_present.as<uint32_t>(), c->d_ovr_cnt.as<int64_t>(), c->n_ovr};
+  const OverrideOut out{c->s_ovr_begin.as<int64_t>(), c->s_ovr_end.as<int64_t>(), c->s_ovr_flags.as<uint8_t>(), c->s_ovr_thr.as<int64_t>(),
+                        c->s_ovr_present.as<uint32_t>(), c->s_ovr_cnt.as<int64_t>(), n_new};
+  k_rebuild_overrides<<<(unsigned)((m + 1 + 127) / 128), 128, 0, c->stream>>>(m, R, 0, nullptr, nullptr, staged<int32_t>(c, at[1]),
+                                                                            c->d_ovr_off.as<int32_t>(), old, nullptr, OverrideCols{},
+                                                                            c->s_ovr_off.as<int32_t>(), out, map);
+  KT_CUDA(c, cudaGetLastError());
+  std::swap(c->d_ovr_off, c->s_ovr_off); std::swap(c->d_ovr_begin, c->s_ovr_begin); std::swap(c->d_ovr_end, c->s_ovr_end);
+  std::swap(c->d_ovr_flags, c->s_ovr_flags); std::swap(c->d_ovr_thr, c->s_ovr_thr); std::swap(c->d_ovr_present, c->s_ovr_present);
+  std::swap(c->d_ovr_cnt, c->s_ovr_cnt);
+  // table, need and nsmask gathered by column in one launch
+  GatherBitsBatch gb{};
+  gb.a[0] = GatherBitsArray{c->d_table.as<uint32_t>(), c->g_spare[0].as<uint32_t>(), 1, (int64_t)tlen, W0, W1, true};
+  gb.a[1] = GatherBitsArray{c->d_need.as<uint32_t>(), c->g_spare[1].as<uint32_t>(), 1, (int64_t)nlen, W0, W1, false};
+  gb.a[2] = GatherBitsArray{c->d_nsmask.as<uint32_t>(), c->g_spare[2].as<uint32_t>(), NS, TPpad, W0, W1, false};
+  gb.map = map;
+  gb.m = m;
+  int64_t items = 0;
+  for (const GatherBitsArray& a : gb.a) items = std::max(items, a.outer * a.w_new * ((a.len + 31) / 32));
+  const unsigned gblocks = (unsigned)std::min<int64_t>((items + 7) / 8, 4096);
+  k_gather_bits<<<dim3(std::max(gblocks, 1u), 3), 256, 0, c->stream>>>(gb);
+  KT_CUDA(c, cudaGetLastError());
+  std::swap(c->d_table, c->g_spare[0]);
+  std::swap(c->d_need, c->g_spare[1]);
+  std::swap(c->d_nsmask, c->g_spare[2]);
+  unsigned char* landed = c->h_call.as<unsigned char>() + land;
+  if (tbytes) KT_CUDA(c, cudaMemcpyAsync(landed, c->d_table.p, tbytes, cudaMemcpyDeviceToHost, c->stream));
+  if (nbytes) KT_CUDA(c, cudaMemcpyAsync(landed + tbytes, c->d_need.p, nbytes, cudaMemcpyDeviceToHost, c->stream));
+  // the host side of the new layout
+  c->spec = std::move(spec);
+  h.term_unsat.swap(unsat);
+  h.M = m;
+  h.W = W1;
+  h.Wp = words_per_row(m);
+  h.TP = 1;
+  for (int32_t t = 0; t < m; ++t) h.TP = std::max(h.TP, c->spec.term_off[(size_t)t + 1] - c->spec.term_off[(size_t)t]);
+  c->M = m;
+  c->n_ovr = n_new;
+  c->h_ovr_off.swap(new_off);
+  // as after kt_upload_throttles: a pass is needed again before the getters that read one (status and reservations are kept)
+  c->evaluated = false;
+  c->have_codes = false;
+  c->have_diff = false;
+  if ((rc = stage_ns_spec(c)) || (rc = rebuild_ns_words(c, NS, at[2]))) return rc;  // rebuild_ns_words synchronises
+  const uint32_t* lt = reinterpret_cast<const uint32_t*>(landed);
+  h.table.assign(lt, lt + (size_t)W1 * tlen);
+  h.need.assign(lt + (size_t)W1 * tlen, lt + (size_t)W1 * (tlen + nlen));
   return KT_OK;
 }
 

@@ -41,6 +41,7 @@
 #pragma weak kt_update_threshold_rows  // without it (older engine doubles) every threshold or override edit recompiles the tables
 #pragma weak kt_update_selector_rows   // without it (older engine doubles) every deletion and selector edit recompiles the tables
 #pragma weak kt_append_throttle_rows   // without it (older engine doubles) every creation recompiles the tables, hole fills included
+#pragma weak kt_move_throttle_columns  // without it (older engine doubles) placement rule 4 and hole compaction recompile the tables
 
 namespace {
 
@@ -603,10 +604,45 @@ struct kth_plugin {
     std::unordered_map<int64_t, std::vector<std::pair<uint32_t, uint32_t>>> codes;  // row -> non-zero {code word index, word}
     std::vector<uint32_t> dirty;                    // [Wp] throttles whose status / reservations changed since the pass
     uint64_t passes = 0, hits = 0;
+    // The cache is indexed by the columns of the pass that filled it (m of them).  A column move renumbers the columns without
+    // voiding it: pass_col[t] is the pass column of current column t (-1: a column the pass did not have), composed across
+    // moves; empty means current = pass column.  Rows are translated when read, dirty marks when set.
+    size_t m = 0;
+    std::vector<int32_t> pass_col;
   } queue;
   void queue_void() { queue.valid = false; }
+  static int match_words(size_t m) {  // words per match row of m throttle columns (kt_match_words after they are synced)
+    const int w = (int)((m + 31) / 32);
+    return std::max(4, (w + 3) / 4 * 4);
+  }
+  long pass_column(size_t t) const {
+    if (!queue.pass_col.empty()) return t < queue.pass_col.size() ? queue.pass_col[t] : -1;
+    return t < queue.m ? (long)t : -1;
+  }
   void throttle_state_changed(size_t t) {  // status or reservations of throttle column t
-    if (queue.valid && (t >> 5) < queue.dirty.size()) queue.dirty[t >> 5] |= 1u << (t & 31);
+    const long p = queue.valid ? pass_column(t) : -1;
+    if (p >= 0 && ((size_t)p >> 5) < queue.dirty.size()) queue.dirty[(size_t)p >> 5] |= 1u << (p & 31);
+  }
+  // Queue row `row`'s cached match row and check codes in the current columns, Wp words (and 2 x Wp code words) wide.
+  void cached_row(int64_t row, int Wp, uint32_t* bm, uint32_t* codes) const {
+    const uint32_t* src = &queue.bitmap[(size_t)row * (size_t)queue.Wp];
+    std::vector<uint32_t> pc(2 * (size_t)queue.Wp, 0);
+    auto it = queue.codes.find(row);
+    if (it != queue.codes.end())
+      for (auto& e : it->second) pc[e.first] = e.second;
+    if (queue.pass_col.empty() && Wp == queue.Wp) {
+      std::copy_n(src, Wp, bm);
+      if (codes) std::copy(pc.begin(), pc.end(), codes);
+      return;
+    }
+    std::fill_n(bm, Wp, 0u);
+    if (codes) std::fill_n(codes, 2 * (size_t)Wp, 0u);
+    for (size_t t = 0; t < throttles.size() && t < 32 * (size_t)Wp; ++t) {
+      const long p = pass_column(t);
+      if (p < 0) continue;
+      if ((src[(size_t)p >> 5] >> (p & 31)) & 1u) bm[t >> 5] |= 1u << (t & 31);
+      if (codes) codes[t >> 4] |= ((pc[(size_t)p >> 4] >> (2 * (p & 15))) & 3u) << (2 * (t & 15));
+    }
   }
   void reservation_changed(size_t t) { reserved_cols.add(t); throttle_state_changed(t); }
   bool apply_committed = false;  // kth_apply: the object was stored; whatever fails afterwards must not roll its resource names back
@@ -970,7 +1006,10 @@ struct kth_plugin {
     }
     return set;
   }
-  void reorder_columns() {
+  // The column order of the full path: live throttles only (the holes compacted), ClusterThrottles after Throttles, each
+  // group -- a Throttle's namespace, a ClusterThrottle's namespace set -- together, by creation within it.  Both the whole
+  // upload (reorder_columns) and a column move (move_columns) lay the columns out by it.
+  std::vector<size_t> column_order() const {
     struct Key {
       int kind;
       std::string set;
@@ -979,10 +1018,9 @@ struct kth_plugin {
     };
     std::vector<Key> keys;
     std::map<std::string, std::string> set_of;  // distinct ClusterThrottle signatures: evaluated once
-    bool dead = false;
     for (size_t t = 0; t < throttles.size(); ++t) {
       const ThrottleObj& o = throttles[t];
-      if (!o.live) { dead = true; continue; }
+      if (!o.live) continue;
       Key k{o.kind == KT_KIND_THROTTLE ? 0 : 1, std::string(), o.seq, t};
       if (o.kind == KT_KIND_THROTTLE) {
         k.set = o.ns;
@@ -999,12 +1037,25 @@ struct kth_plugin {
       if (a.set != b.set) return a.set < b.set;
       return a.seq < b.seq;
     });
-    bool same = !dead;
-    for (size_t i = 0; same && i < keys.size(); ++i) same = keys[i].idx == i;
+    std::vector<size_t> order;
+    order.reserve(keys.size());
+    for (auto& k : keys) order.push_back(k.idx);
+    return order;
+  }
+  void reorder_columns() {
+    const std::vector<size_t> order = column_order();
+    bool same = order.size() == throttles.size();
+    for (size_t i = 0; same && i < order.size(); ++i) same = order[i] == i;
     if (same) return;
+    lay_out(order);
+    queue_void();
+    status_dirty = reserved_dirty = true;
+  }
+  // The throttles in the given column order (the ones not listed are dropped), with the index rebuilt.
+  void lay_out(const std::vector<size_t>& order) {
     std::vector<ThrottleObj> laid_out;
-    laid_out.reserve(keys.size());
-    for (auto& k : keys) laid_out.push_back(std::move(throttles[k.idx]));
+    laid_out.reserve(order.size());
+    for (size_t t : order) laid_out.push_back(std::move(throttles[t]));
     throttles = std::move(laid_out);
     thr_index.clear();
     free_thr.clear();
@@ -1014,8 +1065,51 @@ struct kth_plugin {
       if (t && throttles[t].seq < throttles[t - 1].seq) thr_reused = true;  // column order is not creation order
     }
     broken_valid = false;
-    queue_void();
-    status_dirty = reserved_dirty = true;
+  }
+  // A new layout without a whole upload (relayout_pending: placement rule 4, hole compaction): at the next sync, like the whole
+  // upload it replaces, the columns are laid out as the full path would (column_order), and the device follows through one
+  // kt_move_throttle_columns (sync_move), before every other column delta.  src[j] is the device column current column j comes
+  // from, -1 for a live throttle the device does not hold yet (a creation, an append not sent): those become empty columns there
+  // and are filled through the selector, threshold, status and reserved deltas.  The pending column deltas are re-indexed; the
+  // cached verdicts are kept, their columns mapped (QueueCache::pass_col).
+  bool relayout_pending = false;
+  bool status_held = false;  // the engine holds an observed status (kt_upload_status since the last kt_upload_throttles)
+  std::vector<int32_t> move_columns() {
+    const std::vector<size_t> order = column_order();
+    const size_t m0 = throttles.size();
+    std::vector<long> new_of(m0, -1);
+    std::vector<int32_t> src(order.size()), pass(order.size());
+    for (size_t j = 0; j < order.size(); ++j) {
+      const size_t t = order[j];
+      new_of[t] = (long)j;
+      src[j] = t >= m_dev ? -1 : (int32_t)t;
+      pass[j] = (int32_t)pass_column(t);
+    }
+    lay_out(order);
+    for (ColumnSet* cs : {&status_cols, &reserved_cols, &spec_cols, &sel_cols}) {
+      const std::vector<size_t> old = cs->list;
+      cs->clear();
+      for (size_t t : old)
+        if (t < m0 && new_of[t] >= 0) cs->add((size_t)new_of[t]);
+    }
+    for (size_t j = 0; j < src.size(); ++j)
+      if (src[j] < 0) {  // filled through the column deltas
+        sel_cols.add(j);
+        spec_cols.add(j);
+        status_cols.add(j);
+        reserved_cols.add(j);
+      }
+    if (queue.valid) queue.pass_col.swap(pass);
+    words_stat = -1;
+    return src;
+  }
+  void sync_move() {
+    if (!relayout_pending) return;
+    relayout_pending = false;
+    const std::vector<int32_t> src = move_columns();
+    check(kt_move_throttle_columns(ctx, (int32_t)src.size(), src.data()), "kt_move_throttle_columns");
+    m_dev = throttles.size();
+    if (!status_held) status_dirty = true;  // a status column delta replaces columns of a status the engine holds
   }
 
   // Throttle specs -> kt_throttle_cols + kt_selector_table.  Terms after the first invalid podSelector are
@@ -1038,6 +1132,8 @@ struct kth_plugin {
     sync_namespaces();  // Throttle rows may have introduced namespace ids
     check(kt_upload_throttles(ctx, (int32_t)m, &tc, &st), "kt_upload_throttles");
     m_dev = m;
+    relayout_pending = false;  // (the whole upload lays the columns out)
+    status_held = false;
     throttles_dirty = false;
     status_dirty = reserved_dirty = true;  // kt_upload_throttles forgets both
     spec_cols.clear();
@@ -1252,6 +1348,7 @@ struct kth_plugin {
       const StatusColumns sc = status_columns(AllColumns{m});
       const kt_status_cols c = sc.cols();
       check(kt_upload_status(ctx, &c), "kt_upload_status");
+      status_held = true;
     } else if (m > 0 && !status_cols.list.empty()) {
       const StatusColumns sc = status_columns(status_cols.list);
       const kt_status_cols c = sc.cols();
@@ -1351,6 +1448,7 @@ struct kth_plugin {
     sync_pods();
     sync_namespaces();
     sync_throttles();
+    sync_move();        // (after sync_throttles, which carries the new layout when it uploads the throttles; before every delta)
     sync_appends();     // (after sync_throttles, which sends these columns too when it uploads the throttles)
     sync_selectors();   // (after both: a hole fill or an edit may list an appended column)
     sync_thresholds();
@@ -2085,6 +2183,8 @@ struct kth_plugin {
     queue.admit.resize(n);
     queue.bitmap.resize(n * (size_t)Wp);
     queue.row_ok.assign(n, 1);
+    queue.m = throttles.size();
+    queue.pass_col.clear();
     queue.valid = true;
     ++queue.passes;
   }
@@ -2148,12 +2248,10 @@ struct kth_plugin {
   PendingResult queue_result(int64_t row) {
     if (!queue_row_current(row)) refresh_queue();
     else ++queue.hits;
-    PendingResult out(1, queue.Wp);
-    std::copy_n(&queue.bitmap[(size_t)row * (size_t)queue.Wp], queue.Wp, out.bitmap.begin());
+    const int Wp = std::max(queue.Wp, match_words(throttles.size()));
+    PendingResult out(1, Wp);
+    cached_row(row, Wp, out.bitmap.data(), out.codes.data());
     out.admit[0] = queue.admit[(size_t)row];
-    auto it = queue.codes.find(row);
-    if (it != queue.codes.end())
-      for (auto& e : it->second) out.codes[e.first] = e.second;
     return out;
   }
   std::vector<int> affected(const RowView& r, int kind) const {  // the set bits of the pod's match row, in column order
@@ -2417,7 +2515,9 @@ struct kth_plugin {
     if (!current) refresh_queue();
     else ++queue.hits;
     const bool any_broken = !broken_throttles().empty();
-    const std::vector<uint32_t> no_codes(2 * (size_t)queue.Wp, 0);
+    const int Wp = std::max(queue.Wp, match_words(throttles.size()));
+    const std::vector<uint32_t> no_codes(2 * (size_t)Wp, 0);
+    std::vector<uint32_t> bm((size_t)Wp);
     for (int64_t row = 0; row < n && row < cap; ++row) {
       const int64_t slot = pend_pod[(size_t)row];
       if (slot < 0) { verdicts[row] = 0; continue; }
@@ -2425,7 +2525,8 @@ struct kth_plugin {
       const PodObj& pod = pods[(size_t)slot];
       const int nsid = ns_dict.find(pod.ns);
       if (any_broken || nsid < 0 || !namespaces[(size_t)nsid].exists) {  // the error paths that never reach the device
-        const RowView rv{&queue.bitmap[(size_t)row * (size_t)queue.Wp], no_codes.data(), queue.admit[(size_t)row], queue.Wp};
+        cached_row(row, Wp, bm.data(), nullptr);
+        const RowView rv{bm.data(), no_codes.data(), queue.admit[(size_t)row], Wp};
         if (!controller_error(pod, rv, KT_KIND_THROTTLE).empty() || !controller_error(pod, rv, KT_KIND_CLUSTERTHROTTLE).empty()) v = 3;
       }
       verdicts[row] = v;
@@ -2976,7 +3077,16 @@ struct kth_plugin {
     auto it = thr_index.find(key);
     if (it == thr_index.end()) {
       o.seq = ++thr_seq;
-      const long at = creation_delta(o, epoch) ? place_creation(o) : -1;
+      const bool delta = creation_delta(o, epoch);
+      const long at = delta ? place_creation(o) : -1;
+      if (delta && at < 0 && kt_move_throttle_columns) {  // rule 4: the columns laid out again by a move, the new one filled
+        const size_t t = throttles.size();
+        thr_index[key] = (int)t;
+        throttles.push_back(std::move(o));
+        relayout_pending = true;
+        selector_changed(t, true);
+        return;
+      }
       if (at >= 0) {  // a column delta: a hole filled in place, or a column appended by the next sync
         const size_t t = (size_t)at;
         const bool reserved_any = [&] {
@@ -3067,6 +3177,11 @@ struct kth_plugin {
     if (selector_delta() && 2 * free_thr.size() <= throttles.size()) {
       sel_cols.add(t);
       selector_changed(t, false);
+      return;
+    }
+    if (selector_delta() && kt_move_throttle_columns && !thr_index.empty()) {  // past half holes: compacted by a move, not a whole upload
+      throttle_state_changed(t);
+      relayout_pending = true;
       return;
     }
     throttles_dirty = status_dirty = reserved_dirty = true;

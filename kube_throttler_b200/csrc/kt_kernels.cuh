@@ -2194,13 +2194,22 @@ __global__ void __launch_bounds__(128) k_scatter_thresholds(int64_t k, const int
 // Some listed column changes its number of overrides: every entry may move.  Column t of the new layout (new_off[M+1]) takes its
 // entries from the staged input when it is listed (sorted[] holds the listed columns in ascending order, pos[] each one's index in
 // the staged input, whose offsets are src_off[k+1]), else from its old position (old_off); they land in a spare set of columns.
+// With a column map (map[M], a column move; k = 0) column t takes old column map[t]'s entries in place of the sorted-list
+// lookup, and none where map[t] is -1.
 __global__ void __launch_bounds__(128) k_rebuild_overrides(int M, int R, int64_t k, const int32_t* __restrict__ sorted, const int32_t* __restrict__ pos,
                                                            const int32_t* __restrict__ new_off, const int32_t* __restrict__ old_off, const OverrideCols old,
-                                                           const int32_t* __restrict__ src_off, const OverrideCols src, int32_t* out_off, const OverrideOut out) {
+                                                           const int32_t* __restrict__ src_off, const OverrideCols src, int32_t* out_off, const OverrideOut out,
+                                                           const int32_t* __restrict__ map) {
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
   if (t > M) return;
   out_off[t] = new_off[t];
   if (t == M) return;
+  if (map) {
+    const int32_t from = map[t];
+    if (from >= 0)
+      for (int32_t j = new_off[t], e = old_off[from]; j < new_off[t + 1]; ++j, ++e) copy_override(out, j, old, e, R);
+    return;
+  }
   int64_t lo = 0, hi = k;  // first listed column >= t
   while (lo < hi) {
     const int64_t mid = (lo + hi) >> 1;

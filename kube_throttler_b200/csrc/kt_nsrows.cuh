@@ -18,6 +18,9 @@
 // host-recompiled table and need slices of those words and the listed columns' kind and flags.
 // A column append (kt_append_throttle_rows) grows M: k_widen_cols restrides the resident per-throttle arrays (and nsmask when W
 // grows) in one launch, filling in the staged new columns, then k_ns_cols takes the touched words and steps 2-5 follow.
+// A column move (kt_move_throttle_columns) renumbers the columns: every per-column bit is column-local, so k_gather_bits gathers
+// table, need and nsmask by column in one launch, k_widen_cols restrides the per-throttle arrays through the same column map, and
+// steps 2-5 follow -- no namespace is evaluated again.
 #pragma once
 #include "kt_keyed.cuh"
 
@@ -140,13 +143,15 @@ __global__ void __launch_bounds__(256) k_scatter_words(int64_t nw, const int32_t
 
 // One array of `rows` rows of `esize`-byte elements (1, 4 or 8) widened from m_old to m_new elements per row: element e < m_old of
 // row r from src[r * m_old + e], the others from add[r * (m_new - m_old) + e - m_old], or zero when add is null.  dst must not
-// overlap src.  With m_old = 0 and src null it is a plain copy of `add` into dst.
+// overlap src.  With m_old = 0 and src null it is a plain copy of `add` into dst.  With a column map (map[m_new], a column
+// move) element e of row r comes from src[r * m_old + map[e]] instead, or is zero where map[e] is -1; add is then unused.
 struct WidenArray {
   const unsigned char* src;
   const unsigned char* add;
   unsigned char* dst;
   int64_t rows, m_old, m_new;
   int32_t esize;
+  const int32_t* map;
 };
 constexpr int kMaxWiden = 24;
 struct WidenBatch {
@@ -161,7 +166,12 @@ __device__ __forceinline__ void widen_elems(const WidenArray& a, int64_t i0, int
   const int64_t k = a.m_new - a.m_old, n = a.rows * a.m_new;
   for (int64_t i = i0; i < n; i += stride) {
     const int64_t r = i / a.m_new, e = i - r * a.m_new;
-    dst[i] = e < a.m_old ? src[r * a.m_old + e] : add ? add[r * k + (e - a.m_old)] : T(0);
+    if (a.map) {
+      const int32_t from = a.map[e];
+      dst[i] = from >= 0 ? src[r * a.m_old + from] : T(0);
+    } else {
+      dst[i] = e < a.m_old ? src[r * a.m_old + e] : add ? add[r * k + (e - a.m_old)] : T(0);
+    }
   }
 }
 // grid (x, b.n): blockIdx.y is the array
@@ -171,6 +181,47 @@ __global__ void __launch_bounds__(256) k_widen_cols(const WidenBatch b) {
   if (a.esize == 8) widen_elems<uint64_t>(a, i0, stride);
   else if (a.esize == 4) widen_elems<uint32_t>(a, i0, stride);
   else widen_elems<uint8_t>(a, i0, stride);
+}
+
+// A bit-sliced array gathered by column: `outer` blocks of w_old 32-throttle words of `len` u32 each ([outer][w_old][len]) into
+// [outer][w_new][len].  Output word (o, w, l) bit j is bit (s & 31) of input word (o, s >> 5, l) for s = map[32w + j], or the
+// fill bit for s = -1 and for 32w + j >= m: bit 1 at even l when fill_even is set (the table's sat planes, as compile_tables
+// starts a column), else 0.
+struct GatherBitsArray {
+  const uint32_t* src;
+  uint32_t* dst;
+  int64_t outer, len;
+  int32_t w_old, w_new;
+  bool fill_even;
+};
+struct GatherBitsBatch {
+  GatherBitsArray a[3];
+  const int32_t* map;
+  int32_t m;
+};
+// grid (x, 3): blockIdx.y is the array.  One warp per run of 32 output words of one (o, w): lane j holds column 32w + j's source
+// word and bit, each output word is one load per lane -- a broadcast when the run's sources share a word, as they do for a
+// compaction -- and one ballot; lane l of the warp keeps word l of the run, so the run is stored in one coalesced write.
+__global__ void __launch_bounds__(256) k_gather_bits(const GatherBitsBatch b) {
+  const GatherBitsArray& a = b.a[blockIdx.y];
+  const int lane = threadIdx.x & 31;
+  const int64_t runs = (a.len + 31) >> 5, items = a.outer * a.w_new * runs;
+  const int64_t warps = (int64_t)gridDim.x * (blockDim.x >> 5);
+  for (int64_t it = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); it < items; it += warps) {
+    const int64_t run = it % runs, ow = it / runs, o = ow / a.w_new;
+    const int32_t w = (int32_t)(ow - o * a.w_new);
+    const int32_t col = w * 32 + lane;
+    const int32_t s = col < b.m ? b.map[col] : -1;
+    const uint32_t* in = s >= 0 ? a.src + ((size_t)o * a.w_old + (s >> 5)) * a.len : nullptr;
+    const int64_t l0 = run << 5, l1 = min(a.len, l0 + 32);
+    uint32_t mine = 0;
+    for (int64_t l = l0; l < l1; ++l) {
+      const bool bit = in ? (in[l] >> (s & 31)) & 1u : a.fill_even && !(l & 1);
+      const uint32_t word = __ballot_sync(0xffffffffu, bit);
+      if (lane == (int)(l - l0)) mine = word;
+    }
+    if (l0 + lane < l1) a.dst[((size_t)o * a.w_new + w) * a.len + l0 + lane] = mine;
+  }
 }
 
 // kind and flags of the k listed throttle columns (kt_update_selector_rows)
